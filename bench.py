@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — scan-to-map registrations/sec (100k-pt scan vs 1M-pt map) on B200, per BASELINE.json.
+"""bench.py — scan-to-map registrations/sec (100k-pt scan vs 1M-pt map) on H100, per BASELINE.json.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload headline|c2|c1|c3|c4|c5]
+                  [--dump-outputs DIR]
 
 One "step" = one NDT registration (pcl::Registration::align semantics) of a synthetic 64-ring scan (~100k points)
 against a 1M-point map, resolution 2.0, DIRECT7, transformation_epsilon 0.01, max 35 iterations, identity guess —
@@ -13,6 +14,9 @@ the steady state apps/align.cpp:32-36 calls "10times" (target already set).
                N_hit*48 + 224) / its CUDA-event duration on the launching stream, vs MEASURED_PEAKS.json hbm_gbs
  * cpu_baseline: the CPU oracle (restatement of the reference's OpenMP path) on the same workload, bounded sample
  * --impl reference: times that CPU path alone (the reference needs PCL/Eigen/FLANN and cannot be built here)
+ * --dump-outputs DIR: after the timed steps, what the timed call returned (poses, convergence, iteration and evaluation
+               counts, transformation probabilities) as DIR/<name>.npy in float32 / float64; the inputs are seeded, so two
+               builds run with the same arguments can be compared output for output
 N > 1: one process per GPU (torchrun), each rank registers its own K scans (replicas — a single alignment does not
 shard, SURVEY.md §8e) and ONE NCCL all-gather of the K 4x4 poses closes the timed region; value = N*K / max time.
 """
@@ -30,6 +34,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+sys.dont_write_bytecode = True  # the tree may be read-only: bench.py writes nothing into it
 
 WORKLOADS = {
     # name: (synth config, resolution, description)
@@ -68,7 +73,7 @@ def step_scans(base, n_steps: int, rank: int):
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe) by a NATIVE thread
+    """SM clock and throttle reasons sampled DURING the timed region by a NATIVE thread
     (tools/clock_sampler.c: NVML through dlopen; one sample before the region, one 400 us into it — while the batched kernel runs
     and the host only waits — then at a backing-off period, one after the region: NVML queries contend with CUDA / NCCL calls).
     Round 1 polled NVML from a Python thread: eight such pollers fighting eight launch loops for their GILs cost one
@@ -208,18 +213,6 @@ def cpu_info() -> dict:
     return info
 
 
-def ncu_traffic(n_registrations: int):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the solver kernel for a launch of n_registrations, from the committed
-    ncu --set full capture of the batched launch (profiles/r2_ndt_solver_traffic.json holds the bytes per registration of
-    that capture; bench.py itself never runs under a profiler)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r2_ndt_solver_traffic.json")) as f:
-            t = json.load(f)
-        return float(t["dram_bytes_per_registration"]) * n_registrations
-    except Exception:
-        return None
-
-
 def hbm_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -227,7 +220,15 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet"
+
+
+def dump_outputs(out_dir, arrays: dict):
+    """--dump-outputs: one DIR/<name>.npy per returned array, integers widened to float64 (every array here is small)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32 if a.dtype == np.float32 else np.float64))
 
 
 def synchronized_start(world: int, device):
@@ -402,20 +403,24 @@ def run_c5(args, rank, local_rank, world, m):
         torch.cuda.synchronize()
         e0.record()
         t0 = time.perf_counter()
-        errs, n_upd, bytes_in = [], 0, 0
+        errs, n_upd, bytes_in, finals = [], 0, 0, []
         for scan, T_gt in frames:
             pose, final, upd = sm.receiveCloud(scan)
+            finals.append(final)
             n_upd += int(upd)
             bytes_in += scan.shape[0] * scan.shape[1] * 4
             errs.append(synth.pose_error(final, T_gt)[0])
         e1.record()
         torch.cuda.synchronize()
         passes.append({"ms": e0.elapsed_time(e1), "wall": time.perf_counter() - t0, "errs": errs, "n_upd": n_upd, "bytes_in": bytes_in,
+                       "finals": finals,
                        "st": sm.stats(), "launches": int(sm.registration.stats()["kernel_launches"] - launches0 + sm.stats()["kernel_launches"])})
     clocks = sampler.stop()
     passes.sort(key=lambda p: p["ms"])
     mid = passes[1]
     ms, wall, errs, n_upd, bytes_in, st = mid["ms"], mid["wall"], mid["errs"], mid["n_upd"], mid["bytes_in"], mid["st"]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"final_transformation": np.stack(mid["finals"]).astype(np.float32)})
     # CPU restatement of the same callback on a bounded prefix of the same stream
     import oracle
     import oracle.scanmatcher as osm
@@ -470,8 +475,8 @@ def run_c3(args, rank, local_rank, world, m):
     import torch
 
     base, tgt, res, desc = make_workload("headline", rank)
-    K = min(args.steps, 10)
-    scans = step_scans(base, K, rank)
+    K = args.steps
+    scans = step_scans(base, max(K, 2), rank)
     g = m.GeneralizedIterativeClosestPoint(device=local_rank)
     g.setMaxCorrespondenceDistance(5.0)
     g.setTransformationEpsilon(1e-8)
@@ -502,6 +507,8 @@ def run_c3(args, rank, local_rank, world, m):
     torch.cuda.synchronize()
     clocks = sampler.stop()
     ms = float(np.sum([a.elapsed_time(b) for a, b in e]))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"pose": np.stack(poses).astype(np.float32)})
     if rank != 0:
         return
     peak, which = hbm_peak()
@@ -607,6 +614,8 @@ def c4_sweep(args, rank, local_rank, world, m, data, with_cpu: bool, comm=None):
         os.sched_setaffinity(0, prev_aff)  # the CPU leg below gets every core back
     if rank != 0:
         return None
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"c4_" + k: v for k, v in res.items()})
     errs = [synth.pose_error(res["pose"][k], data[int(i)][2]) for k, i in enumerate(res["index"]) if int(i) in data]
     out = {
         "metric": "loop-closure candidate registrations/sec (64 scan<->submap pairs, sharded)", "value": args.pairs / (ms_max * 1e-3),
@@ -672,6 +681,8 @@ def main():
     ap.add_argument("--no-flush", action="store_true")
     ap.add_argument("--no-c4", action="store_true", help="skip the loop-closure sweep object of the headline line")
     ap.add_argument("--slots", type=int, default=3, help="registrations in flight per batched launch (1..3)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the arrays the timed call returned as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -765,7 +776,7 @@ def main():
 
     def flush():
         if not args.no_flush:
-            flush_buf.zero_()  # evict L2 (126 MB); excluded from the timing
+            flush_buf.zero_()  # evict L2 (50 MB on H100); excluded from the timing
             torch.cuda.synchronize()
 
     def timed(fn):
@@ -873,6 +884,8 @@ def main():
     if c4_data is not None:
         c4 = c4_sweep(args, rank, local_rank, world, m, c4_data, with_cpu=not args.no_cpu_baseline, comm=comm)
 
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, {k: v for k, v in rb.items() if k != "gathered"})
     if rank == 0:
         peak, which = hbm_peak()
         achieved = alg_bytes / (kernel_ms * 1e-3) / 1e9 if kernel_ms > 0 else 0.0
@@ -911,10 +924,13 @@ def main():
             "roofline": {"bound": "hbm", "kernel": f"ndt_solver_kernel<DIRECT7> (persistent: all evaluations of {K} registrations, "
                                                    f"{args.slots} in flight)",
                          "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": which,
-                         "traffic": ncu_traffic(K), "alg_bytes_per_launch": alg_bytes,
+                         "traffic": None, "alg_bytes_per_launch": alg_bytes,
                          "launch_ms": kernel_ms, "evaluations_per_launch": n_evals,
                          "us_per_evaluation": 1e3 * kernel_ms / max(1, n_evals),
-                         "hits_per_point": float(np.sum(hits)) / max(1.0, float(np.sum(evals * n_pts)))},
+                         "hits_per_point": float(np.sum(hits)) / max(1.0, float(np.sum(evals * n_pts))),
+                         "note": "algorithmic bytes count every voxel-index probe and record read, most of which hit the "
+                                 "shared-memory index or L2 (about 0.5 MB of records for the 1M-point map): frac > 1 "
+                                 "means the kernel is not bound by HBM bandwidth"},
             "target_build": {"set_input_target_ms": set_target_ms, "set_input_target_pinned_ms": set_target_pinned_ms,
                              "voxel_build_device_ms": target_build_ms,
                              "note": "wall clock of setInputTarget for the 1M-point map from pageable / pinned host memory "

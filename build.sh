@@ -1,9 +1,9 @@
 #!/bin/bash
-# Builds lidarslam_ros2_b200/csrc/libb200reg.so for sm_100a (in-tree; the .so travels to the GPU box).
+# Builds lidarslam_ros2_b200/csrc/libb200reg.so for sm_90a (H100), in-tree.
 set -e
 cd "$(dirname "$0")/lidarslam_ros2_b200/csrc"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -ccbin $(command -v g++) ${B200_NVCC_EXTRA}"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -ccbin $(command -v g++) ${B200_NVCC_EXTRA}"
 OBJS=""
 for f in voxel_map ndt_solver ndt_aux nn_grid voxelgrid gicp cloud_codec deskew comm capi scanmatcher; do
   if [ ! -f $f.o ] || [ $f.cu -nt $f.o ] || [ -n "$(find . -name '*.cuh' -newer $f.o -o -name '*.hpp' -newer $f.o -o -name 'b200reg.h' -newer $f.o 2>/dev/null)" ] || [ ../../include/b200reg.h -nt $f.o ] || [ ../../include/b200comm.h -nt $f.o ]; then
@@ -17,7 +17,7 @@ for f in voxel_map ndt_solver ndt_aux nn_grid voxelgrid gicp cloud_codec deskew 
   fi
   OBJS="$OBJS $f.o"
 done
-$NVCC -gencode arch=compute_100a,code=sm_100a -shared -o libb200reg.so $OBJS -ccbin $(command -v g++) -ldl
+$NVCC -gencode arch=compute_90a,code=sm_90a -shared -o libb200reg.so $OBJS -ccbin $(command -v g++) -ldl
 echo built lidarslam_ros2_b200/csrc/libb200reg.so
 # measurement plumbing of bench.py (NVML clock sampling in a native thread), not part of the engine
 cd ../../tools

@@ -1,4 +1,4 @@
-/* b200reg.h — C-ABI of the B200-native scan-registration engine.
+/* b200reg.h — C-ABI of the H100-native scan-registration engine.
  *
  * Drop-in boundary: the pcl::Registration<PointXYZI,PointXYZI> surface that lidarslam_ros2's nodes hold
  * (scanmatcher/include/scanmatcher/scanmatcher_component.h:93, graph_based_slam/include/graph_based_slam/

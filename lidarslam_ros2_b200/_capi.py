@@ -1,5 +1,5 @@
 """ctypes loader of the C-ABI library (include/b200reg.h). There is no fallback: if the CUDA library is missing
-or cannot be loaded this module raises, and every compute call goes through sm_100a kernels."""
+or cannot be loaded this module raises, and every compute call goes through sm_90a kernels."""
 from __future__ import annotations
 
 import ctypes as C
@@ -80,7 +80,7 @@ class Stats(C.Structure):
 
 
 def build(force: bool = False) -> str:
-    """Compile the sm_100a library in-tree with nvcc (build.sh)."""
+    """Compile the sm_90a library in-tree with nvcc (build.sh)."""
     env = dict(os.environ)
     if force:
         for f in os.listdir(os.path.join(_HERE, "csrc")):

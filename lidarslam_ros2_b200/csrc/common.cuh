@@ -1,4 +1,4 @@
-// Shared device/host definitions of the B200 registration engine (sm_100a only).
+// Shared device/host definitions of the registration engine (H100, sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -8,6 +8,9 @@
 #include <string>
 
 namespace b200 {
+
+// SM count of the H100 SXM: the grid-stride launches are capped at a few waves of it.
+constexpr int H100_SMS = 132;
 
 struct CudaError : std::runtime_error {
   using std::runtime_error::runtime_error;

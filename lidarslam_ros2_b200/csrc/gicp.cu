@@ -380,7 +380,7 @@ void r_derivative(const double* x, const double* R, double* g) {
 // control words, self-validating partial rows double-buffered by round parity.
 // =====================================================================================================================
 constexpr int GI_THREADS = 256;
-constexpr int GI_MAX_CTAS = 160;  // one CTA per SM at most (148 on B200); rows per controller thread = GI_MAX_CTAS / 16
+constexpr int GI_MAX_CTAS = 160;  // one CTA per SM at most (132 on H100 SXM); rows per controller thread = GI_MAX_CTAS / 16
 constexpr int GI_CTL_WORDS = 14;  // T[12] (float bits), want_grad, mode
 constexpr int GI_CTL_COPIES = 4;
 constexpr unsigned long long GI_EMPTY = 0xFFF8DEADFFF8DEADull;
@@ -682,10 +682,10 @@ void GicpSolver::init(int device, cudaStream_t s) {
   counter_.ensure(4);
   B200_CUDA(cudaMemset(counter_.ptr, 0, 4 * sizeof(unsigned)));
   result_.ensure(K7_SLOTS);
-  partials_.ensure((size_t)148 * 4 * K7_SLOTS);
   cudaDeviceProp prop;
   B200_CUDA(cudaGetDeviceProperties(&prop, device));
   sm_count_ = prop.multiProcessorCount;
+  partials_.ensure((size_t)sm_count_ * 4 * K7_SLOTS);
   B200_CUDA(cudaMalloc(&d_inner_work_, sizeof(GicpInnerWork)));
   B200_CUDA(cudaMemset(d_inner_work_, 0, sizeof(GicpInnerWork)));
   gi_arm_kernel<<<64, 256>>>(reinterpret_cast<unsigned long long*>(&d_inner_work_->rows[0][0][0]), (size_t)2 * GI_MAX_CTAS * K7_SLOTS);
@@ -771,7 +771,7 @@ void GicpSolver::fdf(const float* T16, bool want_grad, double* f, double* g_t3, 
   for (int k = 0; k < 12; k++) P.T[k] = T16[k];
   P.n = (int)n_source_;
   P.want_grad = want_grad ? 1 : 0;
-  const int blocks = (int)std::min<size_t>((n_source_ + 255) / 256, 148 * 2);
+  const int blocks = (int)std::min<size_t>((n_source_ + 255) / 256, sm_count_ * 2);
   gicp_cost_kernel<<<std::max(blocks, 1), 256, 0, stream_>>>(P, partials_.ptr, counter_.ptr + 1, result_.ptr, h_result_);
   B200_CUDA(cudaGetLastError());
   B200_CUDA(cudaStreamSynchronize(stream_));

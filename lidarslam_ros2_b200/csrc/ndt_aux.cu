@@ -187,7 +187,7 @@ void ndt_hessian_radius(const VoxelMap& map, const float4* src, size_t n, const 
   P.hd = d_hd;
   P.out = d_out21;
   B200_CUDA(cudaMemsetAsync(d_out21, 0, 21 * sizeof(double), s));
-  int blocks = (int)std::min<size_t>((n + 127) / 128, 148 * 8);
+  int blocks = (int)std::min<size_t>((n + 127) / 128, H100_SMS * 8);
   if (blocks < 1) blocks = 1;
   hessian_radius_kernel<<<blocks, 128, 0, s>>>(P);
   B200_CUDA(cudaGetLastError());
@@ -215,7 +215,7 @@ void ndt_score(const VoxelMap& map, const float4* cloud, size_t n, const NdtConf
   P.T_dev = nullptr;
   P.out = d_out1;
   B200_CUDA(cudaMemsetAsync(d_out1, 0, sizeof(double), s));
-  int blocks = (int)std::min<size_t>((n + 127) / 128, 148 * 8);
+  int blocks = (int)std::min<size_t>((n + 127) / 128, H100_SMS * 8);
   if (blocks < 1) blocks = 1;
   score_kernel<<<blocks, 128, 0, s>>>(P);
   B200_CUDA(cudaGetLastError());

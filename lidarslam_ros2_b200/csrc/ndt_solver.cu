@@ -6,7 +6,7 @@
 //   voxel_grid_covariance_omp_impl.hpp:373-442; pcl::transformPointCloud (ndt_omp_impl.hpp:100,817,862) is fused
 //   into the evaluation.
 //
-// B200 design (not a translation of the OpenMP loop):
+// H100 design (not a translation of the OpenMP loop):
 //   * ONE cooperative kernel launch per align(), one 768-thread CTA per SM. Evaluator CTAs keep their source points in
 //     SHARED MEMORY for the whole solve and loop   evaluate -> CTA partial row -> wait for the next pose;   the last
 //     CTA is the CONTROLLER: it keeps the Newton / More-Thuente state in shared memory and loops
@@ -36,7 +36,7 @@ namespace {
 
 // ONE 768-thread CTA per SM (80 registers/thread fill the register file, so two can never share an SM): 24 warps keep
 // the issue slots of the four schedulers busy, the partial sums of an SM are combined in its own shared memory, and the
-// controller CTA has to ingest 147 rows instead of 441 (its L2 -> SM bandwidth bounds the reduction). The controller
+// controller CTA has to ingest 129 rows instead of 387 (its L2 -> SM bandwidth bounds the reduction). The controller
 // CTA owns an SM by construction.
 constexpr int SOLVER_THREADS = 768;
 constexpr int SOLVER_WARPS = SOLVER_THREADS / 32;

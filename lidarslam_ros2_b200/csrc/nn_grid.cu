@@ -444,14 +444,14 @@ void nn1_query(const NnGrid& grid, const float4* queries, size_t n, const float*
   B200_CUDA(cudaMemsetAsync(gm.unresolved_count.ptr, 0, sizeof(unsigned), s));
   const int blocks = (int)((n * NN_GROUP + 127) / 128);
   nn1_kernel<<<blocks, 128, 0, s>>>(P, queries, n, d_idx, d_d2, gm.unresolved_count.ptr, gm.unresolved.ptr);
-  nn1_far_kernel<<<148 * 4, 256, 0, s>>>(P, queries, gm.unresolved_count.ptr, gm.unresolved.ptr, d_idx, d_d2);
+  nn1_far_kernel<<<H100_SMS * 4, 256, 0, s>>>(P, queries, gm.unresolved_count.ptr, gm.unresolved.ptr, d_idx, d_d2);
   B200_CUDA(cudaGetLastError());
 }
 
 void fitness_reduce(const float* d_d2, const int* d_idx, size_t n, double max_range, double* d_scratch2, double* sum,
                     long long* count, cudaStream_t s) {
   B200_CUDA(cudaMemsetAsync(d_scratch2, 0, 2 * sizeof(double), s));
-  int blocks = (int)std::min<size_t>((n + 255) / 256, 148 * 4);
+  int blocks = (int)std::min<size_t>((n + 255) / 256, H100_SMS * 4);
   if (blocks < 1) blocks = 1;
   fitness_kernel<<<blocks, 256, 0, s>>>(d_d2, d_idx, n, max_range, d_scratch2);
   double res[2];

@@ -153,7 +153,7 @@ __global__ void __launch_bounds__(256) bounds_kernel(const float4* __restrict__ 
 Bounds cloud_bounds(const float4* pts, size_t n, unsigned* d_scratch8, cudaStream_t s) {
   unsigned init[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
   B200_CUDA(cudaMemcpyAsync(d_scratch8, init, sizeof(init), cudaMemcpyHostToDevice, s));
-  int blocks = (int)std::min<size_t>((n + 255) / 256, 148 * 8);
+  int blocks = (int)std::min<size_t>((n + 255) / 256, H100_SMS * 8);
   if (blocks < 1) blocks = 1;
   bounds_kernel<<<blocks, 256, 0, s>>>(pts, n, d_scratch8);
   unsigned res[6];

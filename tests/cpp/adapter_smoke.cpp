@@ -1,6 +1,6 @@
 // C++ smoke test of include/b200reg_pcl.hpp (stand-alone mode, no PCL): reads like apps/align.cpp:18-40 of the
 // reference — setInputTarget, setInputSource, align, getFitnessScore. Built by tests/test_host_logic.py on CPU (where it
-// must fail loudly for lack of a GPU) and run by tests/test_gpu_parity.py on the B200.
+// must fail loudly for lack of a GPU) and run by tests/test_gpu_parity.py on the H100.
 #include <cmath>
 #include <cstddef>
 #include <cstdio>

@@ -1,5 +1,5 @@
 """GPU parity tests: the CUDA path through the C-ABI (include/b200reg.h) against the CPU oracle on identical
-inputs, plus the committed golden fixtures. Run on the B200 box with `pytest -m gpu`.
+inputs, plus the committed golden fixtures. Run on an H100 with `pytest -m gpu`.
 
 Tolerances
   * integer / index results (leaf indices, point counts, NN indices): bit exact
@@ -23,7 +23,7 @@ def b200():
     import torch
 
     if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: the gpu tests must run on the B200 box (there is no CPU fallback)")
+        pytest.fail("no CUDA device: the gpu tests need an H100 (there is no CPU fallback)")
     import lidarslam_ros2_b200 as m
 
     return m

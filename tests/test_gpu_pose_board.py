@@ -18,7 +18,7 @@ def b200():
     import torch
 
     if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: the gpu tests must run on the B200 box (there is no CPU fallback)")
+        pytest.fail("no CUDA device: the gpu tests need an H100 (there is no CPU fallback)")
     import lidarslam_ros2_b200 as m
 
     return m

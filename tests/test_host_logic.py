@@ -215,37 +215,13 @@ def test_cpp_adapter_pcl_mode_type_checks():
     assert rc.returncode == 3 and "no CUDA device" in rc.stdout, rc.stdout
 
 
-def test_recorded_bench_line_follows_the_contract():
-    """The bench line recorded on the B200 (profiles/r1_bench_lines.jsonl, first line = `python bench.py` defaults) carries
-    every key of the driver's contract, with consistent values."""
-    import json
-
-    with open(os.path.join(ROOT, "profiles", "r1_bench_lines.jsonl")) as f:
-        line = json.loads(f.readline())
-    for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline",
-              "dtype", "data", "config", "e2e", "gpu_launches", "clocks", "roofline", "cpu_baseline"):
-        assert k in line, k
-    assert line["metric"] == "scan-to-map registrations/sec" and line["unit"] == "registrations/s"
-    assert line["n_gpus"] == 1 and line["warmup"] >= 3 and line["higher_is_better"] is True and line["vs_baseline"] is None
-    assert "workload" in line["config"] and "model" not in line["config"]
-    assert abs(line["value"] - line["n_gpus"] * 1e3 / line["ms_per_step"]) < 1e-6 * line["value"]
-    r = line["roofline"]
-    assert r["bound"] == "hbm" and r["unit"] == "GB/s" and abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-9 and r["traffic"] > 0
-    c = line["cpu_baseline"]
-    assert c["kind"] == "port" and c["cores"] >= 1 and c["value"] > 0 and "sample" in c
-    e = line["e2e"]
-    assert e["value"] > 0 and e["h2d_bytes_per_step"] > 0 and e["d2h_bytes_per_step"] > 0 and e["value"] < line["value"]
-    assert line["gpu_launches"] >= line["steps"]
-    assert line["clocks"]["sm_mhz"] and not set(line["clocks"]["reasons"]) & {"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown"}
-
-
 def test_recorded_round2_bench_line_follows_the_contract():
-    """profiles/r2_bench_lines.jsonl, first line = `python bench.py --steps 20 --warmup 5` on a B200: every key of the bench
+    """profiles/h100_bench_lines.jsonl, first line = `python bench.py --steps 20 --warmup 5` on an H100: every key of the bench
     contract, a roofline fraction consistent with its own fields, an e2e leg that moved bytes, one solver launch for the K
     steps, and the loop-closure sweep object."""
     import json
 
-    with open(os.path.join(ROOT, "profiles", "r2_bench_lines.jsonl")) as f:
+    with open(os.path.join(ROOT, "profiles", "h100_bench_lines.jsonl")) as f:
         line = json.loads(f.readline())
     for key in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline",
                 "dtype", "data", "config", "e2e", "gpu_launches", "clocks", "roofline", "cpu_baseline"):
@@ -267,6 +243,6 @@ def test_recorded_round2_bench_line_follows_the_contract():
     c4 = line["c4"]
     assert c4["pairs"] == 64 and c4["converged"] == 64 and "ncclAllGather" in c4["collective"]
     # the reference arm of the same round prints the same config keys
-    with open(os.path.join(ROOT, "profiles", "r2_bench_lines.jsonl")) as f:
+    with open(os.path.join(ROOT, "profiles", "h100_bench_lines.jsonl")) as f:
         ref = [json.loads(x) for x in f][1]
     assert ref["impl"] == "reference" and ref["config"] == line["config"]
