@@ -50,8 +50,8 @@ struct RankWord {
 
 // One NDT voxel as the fused kernel reads it (48 B, three 16-byte loads):
 //   mean as a float-float pair (hi + lo carries the f64 mean to ~2^-48 relative) so that
-//   x' = (x_trans - mean_hi) - mean_lo reproduces the reference's f64 subtraction followed by the cast to float
-//   (ndt_omp_impl.hpp:259-262, 490) without FP64 instructions on the hot path;
+//   x' = (x_trans - mean_hi) - mean_lo is within one float ulp of the reference's f64 subtraction followed by the cast
+//   to float (ndt_omp_impl.hpp:259-262, 490; not always equal to it) without FP64 instructions on the hot path;
 //   inverse covariance as the f32 cast the reference applies at ndt_omp_impl.hpp:490-492 (symmetric 6).
 struct __align__(16) VoxelRecord {
   float mhx, mhy, mhz, mlx;

@@ -163,7 +163,7 @@ __device__ __forceinline__ Rec load_record(const VoxelRecord* __restrict__ rec) 
 template <bool HESS>
 __device__ __forceinline__ void accumulate_pair(const Rec& R, bool valid, float3 xt, float d1f, float gd2, PairSums& ps) {
   const float c00 = R.b.z, c01 = R.b.w, c02 = R.c.x, c11 = R.c.y, c12 = R.c.z, c22 = R.c.w;
-  // x' = x_trans - mean (float-float mean: equals the reference's f64 subtraction + cast, :259-262, :490)
+  // x' = x_trans - mean (float-float mean: within one ulp of the reference's f64 subtraction + cast, :259-262, :490)
   const float x0 = __fsub_rn(__fsub_rn(xt.x, R.a.x), R.a.w);
   const float x1 = __fsub_rn(__fsub_rn(xt.y, R.a.y), R.b.x);
   const float x2 = __fsub_rn(__fsub_rn(xt.z, R.a.z), R.b.y);
