@@ -199,6 +199,18 @@ int b200reg_ndt_get_voxels(b200reg_t h, int* leaf_idx, int* npts, double* mean3,
  * source (which = 0) or target (which = 1) cloud after an align(); *n = number of points (out9 may be NULL). */
 int b200reg_gicp_get_covariances(b200reg_t h, int which, double* out9, size_t* n);
 int b200reg_gicp_num_correspondences(b200reg_t h, int* out);
+/* GICP read-back for the kernel tests: the prelude of align() (lazy covariances, source grid, output = guess * source)
+ * and one correspondence pass (gicp_omp_impl.hpp:412-456) at transformation_ = T. guess and T are column-major, NULL =
+ * identity. corr: n_source ints, the target index or -1 (may be NULL); maha9: n_source x 9 floats, row-major
+ * (meaningful where corr >= 0; may be NULL); *m = number of correspondences. The state stays in place for
+ * b200reg_gicp_objective. */
+int b200reg_gicp_correspondences(b200reg_t h, const float* guess, const float* T, int* corr, float* maha9, int* m);
+/* one evaluation of the fixed-correspondence objective (operator() when want_grad == 0, else fdf;
+ * gicp_omp_impl.hpp:244-366) at state x6 on the correspondences of the last align() / b200reg_gicp_correspondences, by
+ * the path align() uses (the persistent kernel, or with B200REG_GICP_HOST_BFGS set at creation one reduction launch).
+ * g6 is written when want_grad; T12 (may be NULL) = the f32 row-major 3x4 transform that path built from x6.
+ * B200REG_ERR_ARG when there are fewer than 4 correspondences or the clouds changed since they were found. */
+int b200reg_gicp_objective(b200reg_t h, const double* x6, int want_grad, double* f, double* g6, float* T12);
 /* exact 1-NN of n query points against the target cloud (building block of getFitnessScore / GICP) */
 int b200reg_nn1(b200reg_t h, const float* base, size_t n, size_t stride_bytes, int* idx, float* d2);
 

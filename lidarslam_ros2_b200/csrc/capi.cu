@@ -845,6 +845,39 @@ int b200reg_gicp_num_correspondences(b200reg_t h, int* out) {
   return B200REG_OK;
 }
 
+int b200reg_gicp_correspondences(b200reg_t h, const float* guess, const float* T, int* corr, float* maha9, int* m) {
+  if (!h || h->kind != B200REG_GICP || !m) return B200REG_ERR_ARG;
+  return guarded(h, [&]() {
+    if (!h->have_target) return fail(h, B200REG_ERR_NO_TARGET, "no input target");
+    if (!h->have_source) return fail(h, B200REG_ERR_NO_SOURCE, "no input source");
+    ensure_nn(h);
+    float G[16], Tr[16];
+    if (guess) col_to_row(guess, G);
+    else set_identity(G);
+    if (T) col_to_row(T, Tr);
+    else set_identity(Tr);
+    h->gicp.corr_dist = h->corr_dist;
+    h->gicp_solver.prepare(h->nn, h->d_target.ptr, h->n_target, h->src_view, h->n_source, h->gicp, G, h->stream);
+    *m = h->gicp_solver.correspondences(h->nn, h->gicp, G, Tr, h->stream);
+    h->gicp_solver.read_correspondences(corr, maha9, h->stream);
+    return (int)B200REG_OK;
+  });
+}
+
+int b200reg_gicp_objective(b200reg_t h, const double* x6, int want_grad, double* f, double* g6, float* T12) {
+  if (!h || h->kind != B200REG_GICP || !x6 || !f || (want_grad && !g6)) return B200REG_ERR_ARG;
+  return guarded(h, [&]() {
+    if (!h->gicp_solver.correspondences_current())
+      return fail(h, B200REG_ERR_ARG, "objective: no correspondences for the current clouds (align or correspondences first)");
+    if (h->gicp_solver.last_correspondences() < 4)
+      return fail(h, B200REG_ERR_ARG, "objective: fewer than 4 correspondences (align() never evaluates then)");
+    float T[12];
+    h->gicp_solver.evaluate(x6, want_grad != 0, f, g6, T);
+    if (T12) std::memcpy(T12, T, sizeof(T));
+    return (int)B200REG_OK;
+  });
+}
+
 int b200reg_nn1(b200reg_t h, const float* base, size_t n, size_t stride_bytes, int* idx, float* d2) {
   if (!h || !base || !idx || !d2 || stride_bytes < 12 || (stride_bytes % 4) != 0) return B200REG_ERR_ARG;
   return guarded(h, [&]() {

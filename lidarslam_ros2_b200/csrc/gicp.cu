@@ -374,6 +374,7 @@ constexpr int GI_CTL_COPIES = 4;
 constexpr unsigned long long GI_EMPTY = 0xFFF8DEADFFF8DEADull;
 constexpr long long GI_TIMEOUT_CYCLES = 4000000000LL;
 enum { GI_MODE_RUN = 0, GI_MODE_EXIT = 1 };
+enum { GI_EVAL_BFGS = 0, GI_EVAL_F = 1, GI_EVAL_FDF = 2 };
 
 }  // namespace
 
@@ -394,6 +395,7 @@ struct GicpInnerLaunch {
   double gradient_tol;
   int max_inner;
   unsigned epoch;
+  int eval_once;  // 0: the BFGS; GI_EVAL_F / GI_EVAL_FDF: exactly one fn.f / fn.fdf call at x0 (read-back tests)
 };
 
 __device__ __forceinline__ unsigned long long gi_ld(const unsigned long long* p) {
@@ -564,14 +566,21 @@ __global__ void __launch_bounds__(GI_THREADS) gicp_inner_kernel(const __grid_con
     double x[6];
     for (int k = 0; k < 6; k++) x[k] = L.x0[k];
     int inner = 0;
-    int result = bfgs.minimizeInit(x);
-    result = BFGS_Running;
-    do {  // gicp_omp_impl.hpp:215-230
-      inner++;
-      result = bfgs.minimizeOneStep(x);
-      if (result) break;
-      result = bfgs.testGradient(L.gradient_tol);
-    } while (result == BFGS_Running && inner < L.max_inner && !fn.failed);
+    int result = BFGS_Running;
+    if (L.eval_once != GI_EVAL_BFGS) {  // exactly one functor call at x0, through the same rows and reduction as the BFGS's
+      for (int k = 0; k < 6; k++) bfgs.gradient[k] = 0.0;
+      if (L.eval_once == GI_EVAL_F) bfgs.f = fn.f(x);
+      else fn.fdf(x, bfgs.f, bfgs.gradient);
+    } else {
+      result = bfgs.minimizeInit(x);
+      result = BFGS_Running;
+      do {  // gicp_omp_impl.hpp:215-230
+        inner++;
+        result = bfgs.minimizeOneStep(x);
+        if (result) break;
+        result = bfgs.testGradient(L.gradient_tol);
+      } while (result == BFGS_Running && inner < L.max_inner && !fn.failed);
+    }
     // tell the evaluators to leave
     if (tid < GI_CTL_WORDS) {
       const unsigned payload = tid == 13 ? (unsigned)GI_MODE_EXIT : 0u;
@@ -583,6 +592,10 @@ __global__ void __launch_bounds__(GI_THREADS) gicp_inner_kernel(const __grid_con
       GicpInnerResult* r = L.result_host;
       for (int k = 0; k < 6; k++) r->x[k] = x[k];
       r->f = bfgs.f;
+      for (int k = 0; k < 6; k++) r->g[k] = bfgs.gradient[k];
+      float T[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+      apply_state_dev(T, x);  // the transform the functor published for x (same function, same input)
+      for (int k = 0; k < 12; k++) r->T[k] = T[k];
       r->status = result;
       r->inner = inner;
       r->evaluations = fn.round;
@@ -682,8 +695,9 @@ void GicpSolver::init(int device, cudaStream_t s) {
   B200_CUDA(cudaMallocHost(&h_inner_result_, sizeof(GicpInnerResult)));
 }
 
-int GicpSolver::inner_loop_device(double* x, const GicpConfig& cfg, int* inner_iterations) {
+int GicpSolver::inner_loop_device(double* x, const GicpConfig& cfg, int* inner_iterations, int eval_once) {
   GicpInnerLaunch L{};
+  L.eval_once = eval_once;
   L.P.moved = moved_.ptr;
   L.P.target = target_;
   L.P.corr = corr_.ptr;
@@ -775,32 +789,12 @@ void GicpSolver::fdf(const float* T16, bool want_grad, double* f, double* g_t3, 
   for (int k = 0; k < 9; k++) R9[k] = h_result_[5 + k] * (2.0 / m);
 }
 
-GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, size_t n_target, const float4* source,
-                              size_t n_source, const GicpConfig& cfg, const float* guess16, cudaStream_t s) {
-  // developer trace (env B200REG_GICP_TRACE=1): host wall clock per phase of one align, printed to stderr
-  static const bool trace = getenv("B200REG_GICP_TRACE") != nullptr;
-  auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-  double t_prev = trace ? now() : 0, t_cov = 0, t_nn = 0, t_inner = 0;
-  auto lap = [&](double& acc) {
-    if (!trace) return;
-    B200_CUDA(cudaStreamSynchronize(s));
-    const double t = now();
-    acc += t - t_prev;
-    t_prev = t;
-  };
+void GicpSolver::prepare(const NnGrid& target_grid, const float4* target, size_t n_target, const float4* source,
+                         size_t n_source, const GicpConfig& cfg, const float* guess16, cudaStream_t s) {
   stream_ = s;
   target_ = target;
   n_target_ = n_target;
   n_source_ = n_source;
-  evaluations_ = 0;
-  inner_ms = 0;
-  inner_launches = 0;
-  inner_pair_evaluations = 0;
-  GicpOutcome out;
-  set_identity16(out.final_T);
-  out.converged = 0;
-  out.iterations = 0;
-  out.evaluations = 0;
   const int k = std::min(cfg.k_correspondences, GICP_MAX_K);
   if (cov_k_ != k || cov_eps_ != cfg.gicp_epsilon) {
     target_cov_valid_ = source_cov_valid_ = false;
@@ -834,39 +828,107 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
   std::memcpy(guess.m, guess16, sizeof(guess.m));
   transform_cloud_device(source, n_source, moved_.ptr, guess, s);
   launches += 1;
+}
+
+int GicpSolver::correspondences(const NnGrid& target_grid, const GicpConfig& cfg, const float* guess16,
+                                const float* transformation, cudaStream_t s) {
+  const size_t n_source = n_source_;
+  const double dist_threshold = cfg.corr_dist * cfg.corr_dist;
+  // transform_R = transformation_ * guess in f64 (:412-418)
+  double TR[16] = {0};
+  for (int i = 0; i < 4; i++)
+    for (int j = 0; j < 4; j++)
+      for (int kk = 0; kk < 4; kk++) TR[i * 4 + j] += double(transformation[i * 4 + kk]) * double(guess16[kk * 4 + j]);
+  CorrParams P;
+  P.cov_src = source_cov_.ptr;
+  P.cov_tgt = target_cov_.ptr;
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) P.R[r * 3 + c] = TR[r * 4 + c];
+  P.dist_threshold_d = dist_threshold;
+  P.dist_threshold = dist_threshold > 3.0e38 ? 3.0e38f : (float)dist_threshold;
+  P.n = (int)n_source;
+  B200_CUDA(cudaMemsetAsync(counter_.ptr, 0, sizeof(unsigned), s));
+  // query = transformation_ * output[i] (:426-427); nn1_query applies the 3x4 transform in f32
+  nn_idx_.ensure(n_source);
+  nn_d2_.ensure(n_source);
+  nn1_query(target_grid, moved_.ptr, n_source, transformation, nn_idx_.ptr, nn_d2_.ptr, s, P.dist_threshold * 1.0001f);
+  gicp_corr_kernel<<<(int)((n_source + 127) / 128), 128, 0, s>>>(P, nn_idx_.ptr, nn_d2_.ptr, corr_.ptr, maha_.ptr, counter_.ptr);
+  unsigned m = 0;
+  B200_CUDA(cudaMemcpyAsync(&m, counter_.ptr, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+  B200_CUDA(cudaStreamSynchronize(s));
+  launches += 1;
+  last_m_ = (int)m;
+  corr_current_ = true;
+  return last_m_;
+}
+
+void GicpSolver::read_correspondences(int* corr, float* maha9, cudaStream_t s) {
+  if (n_source_ == 0) return;
+  if (corr) B200_CUDA(cudaMemcpyAsync(corr, corr_.ptr, n_source_ * sizeof(int), cudaMemcpyDeviceToHost, s));
+  if (maha9) B200_CUDA(cudaMemcpyAsync(maha9, maha_.ptr, n_source_ * 9 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  B200_CUDA(cudaStreamSynchronize(s));
+}
+
+void GicpSolver::evaluate(const double* x, bool want_grad, double* f, double* g6, float* T12) {
+  if (device_bfgs) {
+    double xx[6];
+    for (int k = 0; k < 6; k++) xx[k] = x[k];
+    int inner = 0;
+    inner_loop_device(xx, GicpConfig{}, &inner, want_grad ? GI_EVAL_FDF : GI_EVAL_F);
+    const GicpInnerResult& r = *h_inner_result_;
+    *f = r.f;
+    if (want_grad)
+      for (int k = 0; k < 6; k++) g6[k] = r.g[k];
+    for (int k = 0; k < 12; k++) T12[k] = r.T[k];
+    return;
+  }
+  // the host-driven functor of align() (fn.f / fn.fdf there)
+  float T[16];
+  set_identity16(T);
+  apply_state(T, x);
+  if (!want_grad) {
+    fdf(T, false, f, nullptr, nullptr);
+  } else {
+    double gt[3], R[9];
+    fdf(T, true, f, gt, R);
+    for (int q = 0; q < 3; q++) g6[q] = gt[q];
+    r_derivative(x, R, g6);
+  }
+  for (int k = 0; k < 12; k++) T12[k] = T[k];
+}
+
+GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, size_t n_target, const float4* source,
+                              size_t n_source, const GicpConfig& cfg, const float* guess16, cudaStream_t s) {
+  // developer trace (env B200REG_GICP_TRACE=1): host wall clock per phase of one align, printed to stderr
+  static const bool trace = getenv("B200REG_GICP_TRACE") != nullptr;
+  auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
+  double t_prev = trace ? now() : 0, t_cov = 0, t_nn = 0, t_inner = 0;
+  auto lap = [&](double& acc) {
+    if (!trace) return;
+    B200_CUDA(cudaStreamSynchronize(s));
+    const double t = now();
+    acc += t - t_prev;
+    t_prev = t;
+  };
+  evaluations_ = 0;
+  inner_ms = 0;
+  inner_launches = 0;
+  inner_pair_evaluations = 0;
+  GicpOutcome out;
+  set_identity16(out.final_T);
+  out.converged = 0;
+  out.iterations = 0;
+  out.evaluations = 0;
+  prepare(target_grid, target, n_target, source, n_source, cfg, guess16, s);
 
   lap(t_cov);
   float transformation[16], previous[16];
   set_identity16(transformation);
   set_identity16(previous);
-  const double dist_threshold = cfg.corr_dist * cfg.corr_dist;
   bool converged = false;
   int nr_iterations = 0;
   while (!converged) {
-    // transform_R = transformation_ * guess in f64 (:412-418)
-    double TR[16] = {0};
-    for (int i = 0; i < 4; i++)
-      for (int j = 0; j < 4; j++)
-        for (int kk = 0; kk < 4; kk++) TR[i * 4 + j] += double(transformation[i * 4 + kk]) * double(guess16[kk * 4 + j]);
-    CorrParams P;
-    P.cov_src = source_cov_.ptr;
-    P.cov_tgt = target_cov_.ptr;
-    for (int r = 0; r < 3; r++)
-      for (int c = 0; c < 3; c++) P.R[r * 3 + c] = TR[r * 4 + c];
-    P.dist_threshold_d = dist_threshold;
-    P.dist_threshold = dist_threshold > 3.0e38 ? 3.0e38f : (float)dist_threshold;
-    P.n = (int)n_source;
-    B200_CUDA(cudaMemsetAsync(counter_.ptr, 0, sizeof(unsigned), s));
-    // query = transformation_ * output[i] (:426-427); nn1_query applies the 3x4 transform in f32
-    nn_idx_.ensure(n_source);
-    nn_d2_.ensure(n_source);
-    nn1_query(target_grid, moved_.ptr, n_source, transformation, nn_idx_.ptr, nn_d2_.ptr, s, P.dist_threshold * 1.0001f);
-    gicp_corr_kernel<<<(int)((n_source + 127) / 128), 128, 0, s>>>(P, nn_idx_.ptr, nn_d2_.ptr, corr_.ptr, maha_.ptr, counter_.ptr);
-    unsigned m = 0;
-    B200_CUDA(cudaMemcpyAsync(&m, counter_.ptr, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
-    B200_CUDA(cudaStreamSynchronize(s));
-    launches += 1;
-    last_m_ = (int)m;
+    const int m = correspondences(target_grid, cfg, guess16, transformation, s);
     lap(t_nn);
     std::memcpy(previous, transformation, sizeof(previous));
     if (m < 4) break;  // NotEnoughPointsException → caught → break (:187-192, :494-498)

@@ -27,22 +27,45 @@ struct GicpInnerWork;     // device work area of the persistent inner-loop kerne
 struct GicpInnerResult {  // written by the kernel into pinned host memory
   double x[6];
   double f;
+  double g[6];  // gradient at x: the BFGS's last one, or the evaluate-once call's (zero for an f-only call)
+  float T[12];  // row-major 3x4 transform apply_state_dev builds from x
   int status, inner, evaluations, error;
 };
 
 class GicpSolver {
  public:
   void init(int device, cudaStream_t s);
-  void invalidate_target() { target_cov_valid_ = false; }
+  void invalidate_target() {
+    target_cov_valid_ = false;
+    corr_current_ = false;
+  }
   void invalidate_source() {
     source_cov_valid_ = false;
     source_grid_valid_ = false;
+    corr_current_ = false;
   }
+  // the correspondences of the last K6 pass still refer to the clouds set now (no setInput* since)
+  bool correspondences_current() const { return corr_current_; }
   GicpOutcome align(const NnGrid& target_grid, const float4* target, size_t n_target, const float4* source,
                     size_t n_source, const GicpConfig& cfg, const float* guess_rowmajor16, cudaStream_t s);
+  // the two halves of align()'s work, public for the read-back tests:
+  // prelude: lazy covariances (K5), the source grid, moved = guess * source
+  void prepare(const NnGrid& target_grid, const float4* target, size_t n_target, const float4* source, size_t n_source,
+               const GicpConfig& cfg, const float* guess_rowmajor16, cudaStream_t s);
+  // one K6 pass at transformation_ = transformation_rowmajor16: nearest neighbours, distance gate, Mahalanobis
+  // matrices; returns (and keeps) the correspondence count m
+  int correspondences(const NnGrid& target_grid, const GicpConfig& cfg, const float* guess_rowmajor16,
+                      const float* transformation_rowmajor16, cudaStream_t s);
+  // one functor evaluation at state x on the current correspondences, by the path align() uses: the persistent kernel in
+  // evaluate-once mode (device_bfgs) or one gicp_cost_kernel launch. g6 is written when want_grad; T12 (row-major 3x4) is
+  // the f32 transform that path built from x. Requires m >= 4 (align() never evaluates with fewer).
+  void evaluate(const double* x, bool want_grad, double* f, double* g6, float* T12);
+  // read-back of the last K6 pass: corr n_source ints (-1 = none), maha n_source x 9 floats (meaningful where corr >= 0)
+  void read_correspondences(int* corr, float* maha9, cudaStream_t s);
   // read-back for parity tests (row-major 3x3 doubles per point); which: 0 source, 1 target
   size_t covariances(int which, std::vector<double>& out, cudaStream_t s);
   int last_correspondences() const { return last_m_; }
+  size_t n_source() const { return n_source_; }
   int launches = 0;
   // true: estimateRigidTransformationBFGS runs as ONE persistent cooperative kernel per outer iteration (BFGS on the
   // device); false: host-side BFGS, one K7 launch + synchronisation per functor evaluation
@@ -55,8 +78,9 @@ class GicpSolver {
 
  private:
   void fdf(const float* T_rowmajor16, bool want_grad, double* f, double* g_t3, double* R9);
-  // returns the BFGS status; x is updated in place
-  int inner_loop_device(double* x, const GicpConfig& cfg, int* inner_iterations);
+  // returns the BFGS status; x is updated in place. eval_once: 0 runs the BFGS; 1 (f only) or 2 (f and g) makes exactly
+  // one functor call at x instead, its result left in *h_inner_result_
+  int inner_loop_device(double* x, const GicpConfig& cfg, int* inner_iterations, int eval_once = 0);
   GicpInnerWork* d_inner_work_ = nullptr;
   GicpInnerResult* h_inner_result_ = nullptr;  // pinned
   unsigned inner_epoch_ = 0;
@@ -64,7 +88,7 @@ class GicpSolver {
   int sm_count_ = 0;
   int device_ = 0;
   cudaStream_t stream_ = nullptr;
-  bool target_cov_valid_ = false, source_cov_valid_ = false, source_grid_valid_ = false;
+  bool target_cov_valid_ = false, source_cov_valid_ = false, source_grid_valid_ = false, corr_current_ = false;
   int cov_k_ = 0;
   double cov_eps_ = 0;
   NnGrid source_grid_;

@@ -404,6 +404,31 @@ class GeneralizedIterativeClosestPoint(_Registration):
         self._check(self._lib.b200reg_gicp_num_correspondences(self._h, C.byref(v)))
         return v.value
 
+    def correspondences(self, T=None, guess=None):
+        """align()'s prelude and one correspondence pass (K6) at transformation_ = T (row-major 4x4, None = identity)
+        -> (corr (n,) int32, -1 = none; Mahalanobis matrices (n, 3, 3) float32, meaningful where corr >= 0; m)."""
+        g = _colmajor(guess) if guess is not None else None
+        t = _colmajor(T) if T is not None else None
+        corr = np.empty(self._n_source, dtype=np.int32)
+        maha = np.empty((self._n_source, 3, 3), dtype=np.float32)
+        m = C.c_int(0)
+        self._check(self._lib.b200reg_gicp_correspondences(self._h, _ptr(g) if g is not None else None,
+                                                           _ptr(t) if t is not None else None, _ptr(corr), _ptr(maha),
+                                                           C.byref(m)))
+        return corr, maha, m.value
+
+    def objective(self, x6, want_grad: bool = True):
+        """One functor evaluation (operator() without want_grad, fdf with it) on the current correspondences, by the path
+        align() uses -> (f, g (6,) or None, T (4, 4) float32: the transform that path built from x6)."""
+        x = np.ascontiguousarray(x6, dtype=np.float64)
+        f = C.c_double(0)
+        g = np.zeros(6)
+        T = np.zeros(12, dtype=np.float32)
+        self._check(self._lib.b200reg_gicp_objective(self._h, _ptr(x), int(want_grad), C.byref(f), _ptr(g), _ptr(T)))
+        T4 = np.eye(4, dtype=np.float32)
+        T4[:3] = T.reshape(3, 4)
+        return f.value, (g if want_grad else None), T4
+
 
 def align_batch(engines, guesses=None) -> np.ndarray:
     """Batched loop-closure sweep on one GPU: all solves are enqueued before any is awaited. Returns (K,4,4)."""

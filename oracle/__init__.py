@@ -93,6 +93,10 @@ def lib() -> C.CDLL:
         L.oracle_gicp_fdf.restype = C.c_double
         L.oracle_gicp_num_correspondences.argtypes = [vp]
         L.oracle_gicp_num_correspondences.restype = C.c_int
+        L.oracle_gicp_f_only.argtypes = [vp, vp]
+        L.oracle_gicp_f_only.restype = C.c_double
+        L.oracle_gicp_apply_state.argtypes = [vp, vp, vp]
+        L.oracle_gicp_correspondences.argtypes = [vp, vp, vp, vp]
         _lib = L
     return _lib
 
@@ -282,6 +286,28 @@ class GICP:
 
     def num_correspondences(self) -> int:
         return int(lib().oracle_gicp_num_correspondences(self._h))
+
+    def f_only(self, x6) -> float:
+        """The functor's operator() (f32 residual and M r, f64 sum) at state x on the last correspondences."""
+        x = np.ascontiguousarray(x6, dtype=np.float64)
+        return float(lib().oracle_gicp_f_only(self._h, _ptr(x)))
+
+    def apply_state(self, x6) -> np.ndarray:
+        """applyState(base_transformation_, x): the f32 transform the functor evaluates at, row-major 4x4."""
+        x = np.ascontiguousarray(x6, dtype=np.float64)
+        out = np.empty(16, dtype=np.float32)
+        lib().oracle_gicp_apply_state(self._h, _ptr(x), _ptr(out))
+        return _from_colmajor(out)
+
+    def correspondences(self):
+        """(src_idx, tgt_idx, mahalanobis (m, 3, 3) float32) of the last outer iteration."""
+        m = self.num_correspondences()
+        s = np.empty(m, dtype=np.int32)
+        t = np.empty(m, dtype=np.int32)
+        M = np.empty((m, 3, 3), dtype=np.float32)
+        if m:
+            lib().oracle_gicp_correspondences(self._h, _ptr(s), _ptr(t), _ptr(M))
+        return s, t, M
 
 
 # ---- known-answer hooks ----

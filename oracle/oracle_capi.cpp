@@ -268,5 +268,26 @@ double oracle_gicp_fdf(void* h, const double* x6, double* g6) {
   return f;
 }
 int oracle_gicp_num_correspondences(void* h) { return (int)static_cast<GICP*>(h)->src_idx.size(); }
+// functor operator(), the f32 path (gicp_omp_impl.hpp:244-274), at state x on the last correspondences
+double oracle_gicp_f_only(void* h, const double* x6) { return static_cast<GICP*>(h)->f_only(x6); }
+// base_transformation_ with the state applied (applyState, gicp_omp_impl.hpp:517-528), column-major
+void oracle_gicp_apply_state(void* h, const double* x6, float* T_colmajor) {
+  GICP* g = static_cast<GICP*>(h);
+  float T[16];
+  std::memcpy(T, g->base_transformation, sizeof(T));
+  GICP::applyState(T, x6);
+  row_to_col(T, T_colmajor);
+}
+// correspondences of the last outer iteration: source / target indices and the source point's Mahalanobis matrix
+// (row-major 3x3 floats), m of each
+void oracle_gicp_correspondences(void* h, int* src_idx, int* tgt_idx, float* maha9) {
+  GICP* g = static_cast<GICP*>(h);
+  const size_t m = g->src_idx.size();
+  for (size_t i = 0; i < m; i++) {
+    src_idx[i] = g->src_idx[i];
+    tgt_idx[i] = g->tgt_idx[i];
+    std::memcpy(maha9 + i * 9, &g->mahalanobis[(size_t)g->src_idx[i] * 9], 9 * sizeof(float));
+  }
+}
 
 }  // extern "C"

@@ -269,14 +269,16 @@ def test_cpp_adapter_end_to_end(b200):
     """The C++ adapter (include/b200reg_pcl.hpp) driven like apps/align.cpp: recovers a known shift on the GPU."""
     import os
     import subprocess
+    import tempfile
 
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    exe = os.path.join(root, "tests", "cpp", "adapter_smoke")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(root, "include"),
-                           os.path.join(root, "tests", "cpp", "adapter_smoke.cpp"), "-o", exe,
-                           "-L" + os.path.join(root, "lidarslam_ros2_b200", "csrc"), "-lb200reg",
-                           "-Wl,-rpath," + os.path.join(root, "lidarslam_ros2_b200", "csrc")])
-    out = subprocess.run([exe], capture_output=True, text=True)
+    with tempfile.TemporaryDirectory() as tmp:  # the program is built outside the tree, which may be read-only
+        exe = os.path.join(tmp, "adapter_smoke")
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(root, "include"),
+                               os.path.join(root, "tests", "cpp", "adapter_smoke.cpp"), "-o", exe,
+                               "-L" + os.path.join(root, "lidarslam_ros2_b200", "csrc"), "-lb200reg",
+                               "-Wl,-rpath," + os.path.join(root, "lidarslam_ros2_b200", "csrc")])
+        out = subprocess.run([exe], capture_output=True, text=True)
     assert out.returncode == 0, out.stdout + out.stderr
 
 
@@ -287,15 +289,17 @@ def test_cpp_adapter_pcl_mode_keeps_the_host_tree_out(b200):
     the host tree, or if the aligned-cloud copy is not opt-in."""
     import os
     import subprocess
+    import tempfile
 
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    exe = os.path.join(root, "tests", "cpp", "adapter_pcl_mode")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Werror", "-DB200REG_WITH_PCL",
-                           "-I" + os.path.join(root, "tests", "cpp", "fake_pcl"), "-I" + os.path.join(root, "include"),
-                           os.path.join(root, "tests", "cpp", "adapter_pcl_mode.cpp"), "-o", exe,
-                           "-L" + os.path.join(root, "lidarslam_ros2_b200", "csrc"), "-lb200reg",
-                           "-Wl,-rpath," + os.path.join(root, "lidarslam_ros2_b200", "csrc")])
-    out = subprocess.run([exe], capture_output=True, text=True)
+    with tempfile.TemporaryDirectory() as tmp:  # the program is built outside the tree, which may be read-only
+        exe = os.path.join(tmp, "adapter_pcl_mode")
+        subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Werror", "-DB200REG_WITH_PCL",
+                               "-I" + os.path.join(root, "tests", "cpp", "fake_pcl"), "-I" + os.path.join(root, "include"),
+                               os.path.join(root, "tests", "cpp", "adapter_pcl_mode.cpp"), "-o", exe,
+                               "-L" + os.path.join(root, "lidarslam_ros2_b200", "csrc"), "-lb200reg",
+                               "-Wl,-rpath," + os.path.join(root, "lidarslam_ros2_b200", "csrc")])
+        out = subprocess.run([exe], capture_output=True, text=True)
     assert out.returncode == 0, (out.returncode, out.stdout + out.stderr)
 
 

@@ -135,10 +135,11 @@ def test_gather_rows_world2_gloo():
         assert it == [5 + i for i in range(n_pairs)]
 
 
-def _build_adapter():
+def _build_adapter(out_dir):
+    """Builds the adapter program into out_dir (a temporary directory: the tree may be read-only)."""
     import subprocess
 
-    exe = os.path.join(ROOT, "tests", "cpp", "adapter_smoke")
+    exe = os.path.join(out_dir, "adapter_smoke")
     src = os.path.join(ROOT, "tests", "cpp", "adapter_smoke.cpp")
     subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), src, "-o", exe,
                            "-L" + os.path.join(ROOT, "lidarslam_ros2_b200", "csrc"), "-lb200reg",
@@ -150,11 +151,13 @@ def test_cpp_adapter_compiles_and_fails_loudly_without_gpu():
     """include/b200reg_pcl.hpp (the C++ host side of the boundary) builds against the C-ABI; without a GPU the
     engine refuses to construct (exit code 3) instead of falling back to a CPU path."""
     import subprocess
+    import tempfile
 
     import torch
 
-    exe = _build_adapter()
-    rc = subprocess.run([exe], capture_output=True, text=True)
+    with tempfile.TemporaryDirectory() as tmp:
+        exe = _build_adapter(tmp)
+        rc = subprocess.run([exe], capture_output=True, text=True)
     if torch.cuda.is_available():
         assert rc.returncode == 0, rc.stdout
     else:
@@ -205,13 +208,16 @@ def test_cpp_adapter_pcl_mode_type_checks():
 
     if torch.cuda.is_available():
         pytest.skip("a GPU is present")
-    exe = os.path.join(ROOT, "tests", "cpp", "adapter_pcl_mode")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Werror", "-DB200REG_WITH_PCL",
-                           "-I" + os.path.join(ROOT, "tests", "cpp", "fake_pcl"), "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "cpp", "adapter_pcl_mode.cpp"), "-o", exe,
-                           "-L" + os.path.join(ROOT, "lidarslam_ros2_b200", "csrc"), "-lb200reg",
-                           "-Wl,-rpath," + os.path.join(ROOT, "lidarslam_ros2_b200", "csrc")])
-    rc = subprocess.run([exe], capture_output=True, text=True)
+    import tempfile
+
+    with tempfile.TemporaryDirectory() as tmp:  # the program is built outside the tree, which may be read-only
+        exe = os.path.join(tmp, "adapter_pcl_mode")
+        subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Werror", "-DB200REG_WITH_PCL",
+                               "-I" + os.path.join(ROOT, "tests", "cpp", "fake_pcl"), "-I" + os.path.join(ROOT, "include"),
+                               os.path.join(ROOT, "tests", "cpp", "adapter_pcl_mode.cpp"), "-o", exe,
+                               "-L" + os.path.join(ROOT, "lidarslam_ros2_b200", "csrc"), "-lb200reg",
+                               "-Wl,-rpath," + os.path.join(ROOT, "lidarslam_ros2_b200", "csrc")])
+        rc = subprocess.run([exe], capture_output=True, text=True)
     assert rc.returncode == 3 and "no CUDA device" in rc.stdout, rc.stdout
 
 
