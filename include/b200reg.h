@@ -211,6 +211,41 @@ int b200reg_gicp_correspondences(b200reg_t h, const float* guess, const float* T
  * g6 is written when want_grad; T12 (may be NULL) = the f32 row-major 3x4 transform that path built from x6.
  * B200REG_ERR_ARG when there are fewer than 4 correspondences or the clouds changed since they were found. */
 int b200reg_gicp_objective(b200reg_t h, const double* x6, int want_grad, double* f, double* g6, float* T12);
+/* NDT read-back for the controller tests: an opt-in per-round trace of b200reg_align (batch calls are never traced).
+ * Each round of the solver's Newton / More-Thuente controller (ndt_omp_impl.hpp:80-171, 756-916) appends one record:
+ * the totals it consumed, its state after the step and the control block it published. Launches that resume after a K2
+ * pass continue the trace of their align(). b200reg_ndt_set_trace(h, capacity) keeps room for `capacity` records
+ * (0 turns tracing off); b200reg_ndt_get_trace copies min(*n, capacity, cap) records of the last align() and sets *n to
+ * the number of rounds it ran, which exceeds the capacity when the trace overflowed.
+ * phase: 0 initial evaluation, 1 first evaluation of a line search, 2 More-Thuente iteration, 3 K2 Hessian pending. */
+typedef struct b200reg_ndt_trace_record {
+  int round;              /* round within its launch                                                              */
+  int launch;             /* 0 for the first launch of the align(), +1 for each launch resumed after a K2 pass     */
+  int phase_before, phase_after;
+  int fast;               /* 1: the warp-parallel Newton step handled the round, 0: the scalar controller          */
+  int evaluated;          /* 1: the round consumed a fresh evaluation (0: the first round of a resumed launch)     */
+  int built;              /* 1: the round built a control block: T, jang, hang, compute_hessian are valid           */
+  int build_f64;          /* 1: ... and the f64 angle tables jd, hd                                                */
+  int mode;               /* control word published: 0 evaluate, 1 done, 2 leave for a K2 pass                    */
+  int compute_hessian;
+  int interval_converged, open_interval, step_iterations, nr_iterations, evaluations, converged;
+  int done;               /* 0 continue, 1 finished, 2 leave for a K2 pass                                        */
+  int pad0;
+  long long hits_total;
+  double tot[32];         /* totals consumed: [0] score, [1..6] g, [7..27] upper H row-major, [28] hits, rest 0    */
+  double score, g[6];     /* score and gradient the controller holds after the step                               */
+  double p[6], dir[6], x_t[6];
+  double a_t, phi_0, d_phi_0;
+  double a_l, f_l, g_l, a_u, f_u, g_u;  /* More-Thuente interval; 0 on fast rounds, which keep none                */
+  double H[36];           /* first round of a resumed launch: the Hessian the K2 pass injected; 0 otherwise       */
+  double jd[24], hd[45];  /* f64 angle tables at x_t (hd row d1 carries -sy) when build_f64, 0 otherwise         */
+  float T[12];            /* 3x4 row-major transform of the published control block                               */
+  float jang[24], hang[45];
+  float final_T[16];      /* final_transformation_ after the step, row-major                                      */
+  float pad1;
+} b200reg_ndt_trace_record;
+int b200reg_ndt_set_trace(b200reg_t h, int capacity);
+int b200reg_ndt_get_trace(b200reg_t h, b200reg_ndt_trace_record* out, int capacity, int* n);
 /* exact 1-NN of n query points against the target cloud (building block of getFitnessScore / GICP) */
 int b200reg_nn1(b200reg_t h, const float* base, size_t n, size_t stride_bytes, int* idx, float* d2);
 

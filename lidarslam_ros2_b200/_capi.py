@@ -35,7 +35,7 @@ SYMBOLS = [
     "b200reg_voxelgrid", "b200reg_get_stats", "b200reg_ndt_derivatives", "b200reg_ndt_hessian_radius",
     "b200reg_ndt_num_voxels", "b200reg_ndt_get_voxels", "b200reg_nn1",
     "b200reg_gicp_get_covariances", "b200reg_gicp_num_correspondences", "b200reg_gicp_correspondences",
-    "b200reg_gicp_objective", "b200reg_get_kind",
+    "b200reg_gicp_objective", "b200reg_ndt_set_trace", "b200reg_ndt_get_trace", "b200reg_get_kind",
     "b200sm_create", "b200sm_destroy", "b200sm_last_error", "b200sm_set_params", "b200sm_set_initial_pose",
     "b200sm_set_scan", "b200sm_update_map", "b200sm_receive_cloud", "b200sm_num_submaps", "b200sm_get_targeted",
     "b200sm_get_submap", "b200sm_get_filtered_scan", "b200sm_get_stats", "b200sm_search_loop", "b200sm_search_loop_all", "b200sm_import_submap",
@@ -147,6 +147,8 @@ def lib() -> C.CDLL:
     L.b200reg_gicp_num_correspondences.argtypes = [vp, C.POINTER(i)]
     L.b200reg_gicp_correspondences.argtypes = [vp, vp, vp, vp, vp, C.POINTER(i)]
     L.b200reg_gicp_objective.argtypes = [vp, vp, i, C.POINTER(d), vp, vp]
+    L.b200reg_ndt_set_trace.argtypes = [vp, i]
+    L.b200reg_ndt_get_trace.argtypes = [vp, vp, i, C.POINTER(i)]
     L.b200reg_get_kind.argtypes = [vp, C.POINTER(i)]
     L.b200sm_create.argtypes = [i, C.POINTER(vp)]
     L.b200sm_destroy.argtypes = [vp]

@@ -764,6 +764,22 @@ int b200reg_ndt_calculate_score(b200reg_t h, const float* base, size_t n, size_t
   });
 }
 
+int b200reg_ndt_set_trace(b200reg_t h, int capacity) {
+  if (!h || h->kind != B200REG_NDT || capacity < 0) return B200REG_ERR_ARG;
+  return guarded(h, [&]() {
+    h->solver.set_trace(capacity);
+    return (int)B200REG_OK;
+  });
+}
+
+int b200reg_ndt_get_trace(b200reg_t h, b200reg_ndt_trace_record* out, int capacity, int* n) {
+  if (!h || h->kind != B200REG_NDT || !n || capacity < 0) return B200REG_ERR_ARG;
+  return guarded(h, [&]() {
+    *n = h->solver.read_trace(out, capacity);
+    return (int)B200REG_OK;
+  });
+}
+
 int b200reg_ndt_num_voxels(b200reg_t h, size_t* out) {
   if (!h || !out) return B200REG_ERR_ARG;
   return guarded(h, [&]() {

@@ -8,6 +8,7 @@
 #include <string>
 #include <vector>
 
+#include "../../include/b200reg.h"
 #include "common.cuh"
 #include "ndt_math.cuh"
 
@@ -287,6 +288,9 @@ class NdtSolver {
   bool batch_profile = false;   // developer instrumentation (env B200REG_BATCH_PROFILE=1): per-CTA wait / evaluate / reduce cycles
   void read_timing(unsigned long long* out48x8) const;
   void read_cta_eval_ns(unsigned* out, int n) const;
+  // per-round trace of align-mode single launches (b200reg_ndt_set_trace / b200reg_ndt_get_trace)
+  void set_trace(int capacity);
+  int read_trace(b200reg_ndt_trace_record* out, int cap);  // copies up to cap records, returns the rounds counted
   void reset_barrier();
   void fetch_result();
 
@@ -304,6 +308,9 @@ class NdtSolver {
   NdtJob* h_jobs_ = nullptr;       // ... and its pinned host image
   NdtResult* h_batch_results_ = nullptr;  // pinned + device-visible: the controllers write the results there
   size_t jobs_cap_ = 0;
+  b200reg_ndt_trace_record* d_trace_ = nullptr;
+  int trace_cap_ = 0;
+  int trace_launch_ = 0;
   void fill_common(NdtLaunch& L, const VoxelMap& map, const NdtConfig& cfg, int mode, int n_slots, size_t& dyn_smem);
   int eval_ctas_for(size_t n_src) const;
 };

@@ -29,6 +29,18 @@
 #define B200_ADDF(a, b) ((a) + (b))
 #define B200_SUBF(a, b) ((a) - (b))
 #endif
+// the same for double: the More-Thuente arithmetic is spelled out un-fused, in the reference's evaluation order, so that
+// every psi, slope and trial value the controller decides on is bitwise the reference's for the same inputs (ties
+// included: once the interval has collapsed, f_t is compared with an f_l that an earlier round computed the same way)
+#if defined(__CUDA_ARCH__)
+#define B200_MULD(a, b) __dmul_rn((a), (b))
+#define B200_ADDD(a, b) __dadd_rn((a), (b))
+#define B200_SUBD(a, b) __dsub_rn((a), (b))
+#else
+#define B200_MULD(a, b) ((a) * (b))
+#define B200_ADDD(a, b) ((a) + (b))
+#define B200_SUBD(a, b) ((a) - (b))
+#endif
 
 namespace b200 {
 
@@ -306,8 +318,10 @@ B200_HD void solve6(const double* H, const double* b, double* x) {
 }
 
 // ---- More-Thuente helpers -------------------------------------------------------------------------------
-B200_HD double mt_psi(double a, double f_a, double f_0, double g_0, double mu) { return f_a - f_0 - mu * g_0 * a; }
-B200_HD double mt_dpsi(double g_a, double g_0, double mu) { return g_a - mu * g_0; }
+B200_HD double mt_psi(double a, double f_a, double f_0, double g_0, double mu) {
+  return B200_SUBD(B200_SUBD(f_a, f_0), B200_MULD(B200_MULD(mu, g_0), a));
+}
+B200_HD double mt_dpsi(double g_a, double g_0, double mu) { return B200_SUBD(g_a, B200_MULD(mu, g_0)); }
 
 B200_HD bool mt_update_interval(double& a_l, double& f_l, double& g_l, double& a_u, double& f_u, double& g_u,
                                 double a_t, double f_t, double g_t) {
@@ -328,29 +342,37 @@ B200_HD bool mt_update_interval(double& a_l, double& f_l, double& g_l, double& a
 }
 
 B200_HD double mt_cubic_min(double a_l, double f_l, double g_l, double a_t, double f_t, double g_t) {
-  double z = 3 * (f_t - f_l) / (a_t - a_l) - g_t - g_l;
-  double w = sqrt(z * z - g_t * g_l);
-  return a_l + (a_t - a_l) * (w - g_l - z) / (g_t - g_l + 2 * w);
+  double z = B200_SUBD(B200_SUBD(B200_MULD(3.0, B200_SUBD(f_t, f_l)) / B200_SUBD(a_t, a_l), g_t), g_l);
+  double w = sqrt(B200_SUBD(B200_MULD(z, z), B200_MULD(g_t, g_l)));
+  return B200_ADDD(a_l, B200_MULD(B200_SUBD(a_t, a_l), B200_SUBD(B200_SUBD(w, g_l), z)) /
+                            B200_ADDD(B200_SUBD(g_t, g_l), B200_MULD(2.0, w)));
+}
+
+// a_l - (a_l - a_t) / (g_l - g_t) * g_l
+B200_HD double mt_secant(double a_l, double g_l, double a_t, double g_t) {
+  return B200_SUBD(a_l, B200_MULD(B200_SUBD(a_l, a_t) / B200_SUBD(g_l, g_t), g_l));
 }
 
 B200_HD double mt_trial_value(double a_l, double f_l, double g_l, double a_u, double f_u, double g_u, double a_t,
                               double f_t, double g_t) {
   if (f_t > f_l) {  // case 1
     double a_c = mt_cubic_min(a_l, f_l, g_l, a_t, f_t, g_t);
-    double a_q = a_l - 0.5 * (a_l - a_t) * g_l / (g_l - (f_l - f_t) / (a_l - a_t));
-    return (fabs(a_c - a_l) < fabs(a_q - a_l)) ? a_c : 0.5 * (a_q + a_c);
+    double a_q = B200_SUBD(a_l, B200_MULD(B200_MULD(0.5, B200_SUBD(a_l, a_t)), g_l) /
+                                    B200_SUBD(g_l, B200_SUBD(f_l, f_t) / B200_SUBD(a_l, a_t)));
+    return (fabs(B200_SUBD(a_c, a_l)) < fabs(B200_SUBD(a_q, a_l))) ? a_c : B200_MULD(0.5, B200_ADDD(a_q, a_c));
   }
-  if (g_t * g_l < 0) {  // case 2
+  if (B200_MULD(g_t, g_l) < 0) {  // case 2
     double a_c = mt_cubic_min(a_l, f_l, g_l, a_t, f_t, g_t);
-    double a_s = a_l - (a_l - a_t) / (g_l - g_t) * g_l;
-    return (fabs(a_c - a_t) >= fabs(a_s - a_t)) ? a_c : a_s;
+    double a_s = mt_secant(a_l, g_l, a_t, g_t);
+    return (fabs(B200_SUBD(a_c, a_t)) >= fabs(B200_SUBD(a_s, a_t))) ? a_c : a_s;
   }
   if (fabs(g_t) <= fabs(g_l)) {  // case 3
     double a_c = mt_cubic_min(a_l, f_l, g_l, a_t, f_t, g_t);
-    double a_s = a_l - (a_l - a_t) / (g_l - g_t) * g_l;
-    double a_n = (fabs(a_c - a_t) < fabs(a_s - a_t)) ? a_c : a_s;
-    if (a_t > a_l) return fmin(a_t + 0.66 * (a_u - a_t), a_n);
-    return fmax(a_t + 0.66 * (a_u - a_t), a_n);
+    double a_s = mt_secant(a_l, g_l, a_t, g_t);
+    double a_n = (fabs(B200_SUBD(a_c, a_t)) < fabs(B200_SUBD(a_s, a_t))) ? a_c : a_s;
+    const double a_far = B200_ADDD(a_t, B200_MULD(0.66, B200_SUBD(a_u, a_t)));
+    if (a_t > a_l) return fmin(a_far, a_n);
+    return fmax(a_far, a_n);
   }
   return mt_cubic_min(a_u, f_u, g_u, a_t, f_t, g_t);  // case 4
 }

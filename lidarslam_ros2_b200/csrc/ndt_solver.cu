@@ -403,6 +403,8 @@ struct CtlShared {
   int n_rows;      // evaluator CTAs that own points of it = partial rows to reduce
   int job_done;    // batch: finish() ran this round — hand the result over and start the next registration
   NdtResult result;  // batch: result under construction (copied to the mapped host array by the warp)
+  int trace_phase;   // traced launches: st.phase before this round's controller step ...
+  int trace_fast;    // ... and 1 when controller_fast handled it
 };
 
 // evaluator CTAs that get points of a scan of n_src points: as soon as each gets at least four warps of points, all of
@@ -706,9 +708,9 @@ __device__ __noinline__ void controller(const NdtLaunch& L, CtlShared& cs, NdtSo
 
   auto eval_point_values = [&]() {
     phi_t = -st.score;
-    double dd = 0;
+    double dd = 0;  // un-fused like the More-Thuente helpers (ndt_math.cuh): the decisions below are the reference's
 #pragma unroll
-    for (int k = 0; k < 6; k++) dd += st.g[k] * st.dir[k];
+    for (int k = 0; k < 6; k++) dd = B200_ADDD(dd, B200_MULD(st.g[k], st.dir[k]));
     d_phi_t = -dd;
     psi_t = mt_psi(st.a_t, phi_t, st.phi_0, st.d_phi_0, mu);
     d_psi_t = mt_dpsi(d_phi_t, st.d_phi_0, mu);
@@ -729,10 +731,10 @@ __device__ __noinline__ void controller(const NdtLaunch& L, CtlShared& cs, NdtSo
       eval_point_values();
       if (st.open_interval && (psi_t <= 0 && d_psi_t >= 0)) {  // :878-889
         st.open_interval = 0;
-        st.f_l = st.f_l + st.phi_0 - mu * st.d_phi_0 * st.a_l;
-        st.g_l = st.g_l + mu * st.d_phi_0;
-        st.f_u = st.f_u + st.phi_0 - mu * st.d_phi_0 * st.a_u;
-        st.g_u = st.g_u + mu * st.d_phi_0;
+        st.f_l = B200_SUBD(B200_ADDD(st.f_l, st.phi_0), B200_MULD(B200_MULD(mu, st.d_phi_0), st.a_l));
+        st.g_l = B200_ADDD(st.g_l, B200_MULD(mu, st.d_phi_0));
+        st.f_u = B200_SUBD(B200_ADDD(st.f_u, st.phi_0), B200_MULD(B200_MULD(mu, st.d_phi_0), st.a_u));
+        st.g_u = B200_ADDD(st.g_u, B200_MULD(mu, st.d_phi_0));
       }
       {
         double a_l = st.a_l, f_l = st.f_l, g_l = st.g_l, a_u = st.a_u, f_u = st.f_u, g_u = st.g_u;
@@ -853,6 +855,74 @@ __device__ __noinline__ void controller(const NdtLaunch& L, CtlShared& cs, NdtSo
   finish(L, cs, W, lane);
 }
 
+// Traced align() launches (L.trace != nullptr), whole warp 0 after the step and build_control: one record of the round.
+// Kept out of line so that the untraced controller loop is the code it was. Tables and a transform the round did not
+// build, and st.H outside the first round of a resumed launch, are written as zeros.
+__device__ __noinline__ void trace_round(const NdtLaunch& L, const CtlShared& cs, int lane, int round) {
+  unsigned idx = 0;
+  if (lane == 0) idx = atomicAdd(&L.work->trace_count, 1u);
+  idx = __shfl_sync(0xffffffffu, idx, 0);
+  if (idx >= (unsigned)L.trace_cap) return;
+  b200reg_ndt_trace_record& R = L.trace[idx];
+  const NdtState& st = cs.st;
+  const bool resumed = L.resume && round == 0;
+  const bool built = cs.build != 0, f64 = built && cs.build_f64 != 0;
+  R.tot[lane] = cs.tot[lane];
+  for (int k = lane; k < 36; k += 32) R.H[k] = resumed ? st.H[k] : 0.0;
+  if (lane < 24) R.jd[lane] = f64 ? st.jd[lane] : 0.0;
+  for (int k = lane; k < 45; k += 32) R.hd[k] = f64 ? st.hd[k] : 0.0;
+  if (lane < 24) R.jang[lane] = built ? cs.next.jang[lane] : 0.0f;
+  for (int k = lane; k < 45; k += 32) R.hang[k] = built ? cs.next.hang[k] : 0.0f;
+  if (lane < 12) R.T[lane] = built ? cs.next.T[lane] : 0.0f;
+  if (lane < 16) R.final_T[lane] = st.final_T[lane];
+  if (lane < 6) {
+    R.g[lane] = st.g[lane];
+    R.p[lane] = st.p[lane];
+    R.dir[lane] = st.dir[lane];
+    R.x_t[lane] = st.x_t[lane];
+  }
+  if (lane == 0) {
+    R.round = round;
+    R.launch = L.trace_launch;
+    R.phase_before = cs.trace_phase;
+    R.phase_after = st.phase;
+    R.fast = cs.trace_fast;
+    R.evaluated = resumed ? 0 : 1;
+    R.built = built ? 1 : 0;
+    R.build_f64 = f64 ? 1 : 0;
+    R.mode = cs.next.mode;
+    R.compute_hessian = built ? cs.next.compute_hessian : 0;
+    R.interval_converged = st.interval_converged;
+    R.open_interval = st.open_interval;
+    R.step_iterations = st.step_iterations;
+    R.nr_iterations = st.nr_iterations;
+    R.evaluations = st.evaluations;
+    R.converged = st.converged;
+    R.done = cs.done;
+    R.pad0 = 0;
+    R.hits_total = st.hits_total;
+    R.score = st.score;
+    R.a_t = st.a_t;
+    R.phi_0 = st.phi_0;
+    R.d_phi_0 = st.d_phi_0;
+    R.a_l = st.a_l;
+    R.f_l = st.f_l;
+    R.g_l = st.g_l;
+    R.a_u = st.a_u;
+    R.f_u = st.f_u;
+    R.g_u = st.g_u;
+    R.pad1 = 0.0f;
+  }
+}
+
+// Traced launches that start an align(): clear the controller state first, so that fields a solve never writes (the
+// fast path keeps no More-Thuente interval) read as zeros in the trace instead of what shared memory held before.
+__device__ __noinline__ void trace_clear_state(CtlShared& cs, int tid) {
+  int* s = reinterpret_cast<int*>(&cs.st);
+  for (int k = tid; k < (int)(sizeof(NdtState) / 4); k += SOLVER_THREADS) s[k] = 0;
+  __syncthreads();
+}
+
 // =====================================================================================================
 // controller CTA
 // =====================================================================================================
@@ -864,6 +934,7 @@ __device__ __noinline__ void controller_cta(const NdtLaunch& L, CtlShared& cs, d
   // sequence number of the control block published at the end of round r: single launches hand round 0's block over
   // in the launch parameters, batch launches publish it (index 0) before the first reduction
   const int pub_shift = batch ? 1 : 0;
+  if (L.trace && !L.resume) trace_clear_state(cs, tid);
   // state: fresh, or restored from global after a K2 pass
   if (L.resume) {
     const int* src = reinterpret_cast<const int*>(&W->state);
@@ -1027,13 +1098,19 @@ __device__ __noinline__ void controller_cta(const NdtLaunch& L, CtlShared& cs, d
           cs.next.mode = EVAL_DONE;
         }
       } else {
+        if (L.trace && lane == 0) cs.trace_phase = cs.st.phase;
         const bool handled = controller_fast(L, cs, lane);  // warp-uniform result
+        if (L.trace && lane == 0) cs.trace_fast = handled ? 1 : 0;
         if (!handled && lane == 0) controller(L, cs, W);
         __syncwarp();
         B200_STAMP(lane == 0, round, 8);
         if (cs.build) build_control(cs, lane);
         B200_STAMP(lane == 0, round, 9);
         __syncwarp();
+        if (L.trace) {
+          trace_round(L, cs, lane, round);
+          __syncwarp();
+        }
         if (batch && cs.job_done) {
           // this registration is finished: its result goes straight to the mapped host array, the slot takes the next one
           const int* src = reinterpret_cast<const int*>(&cs.result);
@@ -1414,6 +1491,7 @@ KernelFn kernel_for(int method) {
 // =====================================================================================================
 NdtSolver::~NdtSolver() {
   if (d_work_) cudaFree(d_work_);
+  if (d_trace_) cudaFree(d_trace_);
   if (h_result_) cudaFreeHost(h_result_);
   if (d_jobs_) cudaFree(d_jobs_);
   if (h_jobs_) cudaFreeHost(h_jobs_);
@@ -1445,6 +1523,27 @@ void NdtSolver::read_cta_eval_ns(unsigned* out, int n) const {
 void NdtSolver::read_timing(unsigned long long* out) const {
   B200_CUDA(cudaMemcpy(out, d_work_->timing, sizeof(unsigned long long) * NDT_TIMING_ROUNDS * NDT_TIMING_SLOTS,
                        cudaMemcpyDeviceToHost));
+}
+void NdtSolver::set_trace(int capacity) {
+  if (d_trace_) cudaFree(d_trace_);
+  d_trace_ = nullptr;
+  trace_cap_ = 0;
+  if (capacity <= 0) return;
+  B200_CUDA(cudaMalloc(&d_trace_, (size_t)capacity * sizeof(b200reg_ndt_trace_record)));
+  trace_cap_ = capacity;
+  B200_CUDA(cudaMemsetAsync(&d_work_->trace_count, 0, sizeof(unsigned), stream_));
+  B200_CUDA(cudaStreamSynchronize(stream_));
+}
+int NdtSolver::read_trace(b200reg_ndt_trace_record* out, int cap) {
+  if (!trace_cap_) return 0;
+  unsigned n = 0;
+  B200_CUDA(cudaMemcpyAsync(&n, &d_work_->trace_count, sizeof(unsigned), cudaMemcpyDeviceToHost, stream_));
+  B200_CUDA(cudaStreamSynchronize(stream_));
+  const int m = std::min(std::min((int)n, trace_cap_), cap);
+  if (out && m > 0)
+    B200_CUDA(cudaMemcpyAsync(out, d_trace_, (size_t)m * sizeof(b200reg_ndt_trace_record), cudaMemcpyDeviceToHost, stream_));
+  B200_CUDA(cudaStreamSynchronize(stream_));
+  return (int)n;
 }
 const double* NdtSolver::state_jd() const { return d_work_->state.jd; }
 const double* NdtSolver::state_hd() const { return d_work_->state.hd; }
@@ -1558,6 +1657,13 @@ void NdtSolver::launch(const VoxelMap& map, const float4* src, size_t n_src, con
   L.n_src = (int)n_src;
   L.resume = resume;
   initial_pose(T_rowmajor16, p6, L.p0, L.init_final, L.init, compute_hessian);
+  if (trace_cap_ > 0 && mode == NDT_MODE_ALIGN) {
+    trace_launch_ = resume ? trace_launch_ + 1 : 0;
+    if (!resume) B200_CUDA(cudaMemsetAsync(&d_work_->trace_count, 0, sizeof(unsigned), stream_));
+    L.trace = d_trace_;
+    L.trace_cap = trace_cap_;
+    L.trace_launch = trace_launch_;
+  }
 
   grid_ = eval_ctas_for(n_src) + 1;  // + the controller CTA
   block_ = SOLVER_THREADS;

@@ -1,5 +1,6 @@
 // Device-side structures shared by the NDT solver kernels (ndt_solver.cu, ndt_aux.cu).
 #pragma once
+#include "../../include/b200reg.h"
 #include "common.cuh"
 #include "engine.hpp"
 #include "grid_index.cuh"
@@ -87,7 +88,8 @@ struct NdtJob {
 struct NdtSolverWork {
   unsigned error;
   unsigned next_job;     // batch launches: next unassigned registration (atomicAdd by the controllers)
-  unsigned pad[2];
+  unsigned trace_count;  // traced align(): rounds recorded so far (counts on past NdtLaunch::trace_cap); host-reset per align
+  unsigned pad;
   NdtControl control;    // plain copy of the control block, written only when the kernel leaves for a K2 pass
   NdtState state;
   NdtResult result;
@@ -131,6 +133,10 @@ struct NdtLaunch {
   double p0[6];
   float init_final[16];
   NdtControl init;
+  // trace != nullptr (single align() launches only): warp 0 of the controller CTA appends one record per round
+  b200reg_ndt_trace_record* trace;
+  int trace_cap;
+  int trace_launch;  // 0 for the first launch of an align(), +1 for every launch resumed after a K2 pass
 };
 
 // ---- rank-index probe ----------------------------------------------------------------------------------

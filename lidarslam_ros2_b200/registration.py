@@ -361,6 +361,30 @@ class NormalDistributionsTransform(_Registration):
         self._check(self._lib.b200reg_ndt_hessian_radius(self._h, _ptr(Tc), _ptr(p), _ptr(H)))
         return H
 
+    # b200reg_ndt_trace_record as a numpy record (include/b200reg.h); tests/test_host_logic.py checks size and offsets
+    TRACE_DTYPE = np.dtype([(k, np.int32) for k in (
+        "round", "launch", "phase_before", "phase_after", "fast", "evaluated", "built", "build_f64", "mode", "compute_hessian",
+        "interval_converged", "open_interval", "step_iterations", "nr_iterations", "evaluations", "converged", "done", "pad0")]
+        + [("hits_total", np.int64), ("tot", np.float64, (32,)), ("score", np.float64), ("g", np.float64, (6,)),
+           ("p", np.float64, (6,)), ("dir", np.float64, (6,)), ("x_t", np.float64, (6,))]
+        + [(k, np.float64) for k in ("a_t", "phi_0", "d_phi_0", "a_l", "f_l", "g_l", "a_u", "f_u", "g_u")]
+        + [("H", np.float64, (36,)), ("jd", np.float64, (24,)), ("hd", np.float64, (45,)), ("T", np.float32, (12,)),
+           ("jang", np.float32, (24,)), ("hang", np.float32, (45,)), ("final_T", np.float32, (16,)), ("pad1", np.float32)])
+
+    def setTrace(self, capacity: int):
+        """Record the controller's rounds of every following align() (b200reg_ndt_set_trace); 0 turns it off."""
+        self._trace_cap = int(capacity)
+        self._check(self._lib.b200reg_ndt_set_trace(self._h, self._trace_cap))
+
+    def trace(self):
+        """The rounds of the last traced align() as a TRACE_DTYPE record array, and the number of rounds the solver counted
+        (larger than the array when the capacity set by setTrace was exceeded)."""
+        cap = getattr(self, "_trace_cap", 0)
+        out = np.zeros(cap, dtype=self.TRACE_DTYPE)
+        n = C.c_int(0)
+        self._check(self._lib.b200reg_ndt_get_trace(self._h, _ptr(out) if cap else None, cap, C.byref(n)))
+        return out[:min(n.value, cap)].copy(), n.value
+
     def voxels(self) -> dict:
         n = C.c_size_t(0)
         self._check(self._lib.b200reg_ndt_num_voxels(self._h, C.byref(n)))

@@ -75,10 +75,11 @@ def gauss_constants(outlier_ratio, resolution):
     return d1, d2
 
 
-def angle_tables(p6, minus_sy=False):
+def angle_tables(p6, minus_sy=False, f64=False):
     """computeAngleDerivatives (ndt_omp_impl.hpp:287-393): the float32 tables (8 x 3 for J's angular columns a..h,
     15 x 3 for the second derivatives a2 a3 b2 b3 c2 c3 d1 d2 d3 e1 e2 e3 f1 f2 f3), angles below 1e-4 snapped to
-    (cos, sin) = (1, 0). The live f32 table keeps +sy in d1.z; minus_sy gives the f64 convention."""
+    (cos, sin) = (1, 0). The live f32 table keeps +sy in d1.z; minus_sy gives the f64 convention. f64=True also returns
+    the float64 values before the cast (J64, H64), the values the K2 pass reads and that decide float32 rounding."""
     def cs(a):
         return (1.0, 0.0) if abs(a) < 10e-5 else (math.cos(a), math.sin(a))
 
@@ -106,6 +107,8 @@ def angle_tables(p6, minus_sy=False):
          [-cy * cz, cy * sz, 0.0],
          [-cx * sz - sx * sy * cz, -cx * cz + sx * sy * sz, 0.0],
          [-sx * sz + cx * sy * cz, -cx * sy * sz - sx * cz, 0.0]]
+    if f64:
+        return np.array(J, dtype=F32), np.array(H, dtype=F32), np.array(J), np.array(H)
     return np.array(J, dtype=F32), np.array(H, dtype=F32)
 
 

@@ -198,6 +198,27 @@ def test_abi_header_is_plain_c():
                                "-fsyntax-only", src])
 
 
+def test_ndt_trace_record_layout_matches_numpy():
+    """NormalDistributionsTransform.trace() reads b200reg_ndt_trace_record through a numpy dtype: its size and every field
+    offset must be what a C compiler lays out for include/b200reg.h."""
+    import subprocess
+    import tempfile
+
+    from lidarslam_ros2_b200.registration import NormalDistributionsTransform as NDT
+
+    dt = NDT.TRACE_DTYPE
+    body = "".join(f'printf("{k} %zu\\n", offsetof(b200reg_ndt_trace_record, {k}));' for k in dt.names)
+    with tempfile.TemporaryDirectory() as d:
+        src, exe = os.path.join(d, "layout.c"), os.path.join(d, "layout")
+        with open(src, "w") as f:
+            f.write('#include <stddef.h>\n#include <stdio.h>\n#include "b200reg.h"\nint main(void){'
+                    'printf("sizeof %zu\\n", sizeof(b200reg_ndt_trace_record));' + body + "return 0;}\n")
+        subprocess.check_call(["gcc", "-std=c99", "-Wall", "-Werror", "-I" + os.path.join(ROOT, "include"), src, "-o", exe])
+        got = dict(line.split() for line in subprocess.check_output([exe], text=True).splitlines())
+    assert int(got.pop("sizeof")) == dt.itemsize
+    assert {k: int(v) for k, v in got.items()} == {k: dt.fields[k][1] for k in dt.names}
+
+
 def test_cpp_adapter_pcl_mode_type_checks():
     """include/b200reg_pcl.hpp compiled with -DB200REG_WITH_PCL against a PCL-1.12-shaped stub (tests/cpp/fake_pcl): the
     classes must derive from pcl::Registration, override its virtuals and be assignable to the nodes' `registration_` pointer
