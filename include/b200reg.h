@@ -338,6 +338,38 @@ int b200sm_search_loop_all(b200sm_t s, b200reg_t reg, float voxel_leaf_size, dou
                            int shard_rank, int shard_world, b200sm_loop_result* out, size_t capacity, size_t* n_out,
                            size_t* n_candidates_total);
 
+/* ---- backend pose adjustment: GraphBasedSlamComponent::doPoseAdjustment (gbs.cpp:262-371) ----------------------------
+ * LoopEdge of graph_based_slam_component.h: pair_id = (from, to), relative_pose = from^-1 * to (gbs.cpp:240-247).
+ * A b200sm_search_loop result with accepted = 1 gives from = id_min, relative_pose = relative_pose and
+ * to = the newest submap index at the time of the search (b200sm_num_submaps - 1), exactly as gbs.cpp:241 does.     */
+typedef struct b200sm_loop_edge {
+  int from, to;
+  double relative_pose[16]; /* column-major */
+} b200sm_loop_edge;
+typedef struct b200sm_pose_adjust_result {
+  double chi2_initial, chi2_final; /* sum of e^T e over all edges before / after                       */
+  int iterations;                  /* LM iterations run (<= max_iterations; fewer when g2o would stop)  */
+  int trials;                      /* damped solves tried, accepted and rejected                       */
+  int n_vertices, n_edges;
+} b200sm_pose_adjust_result;
+/* doPoseAdjustment's graph and solve (gbs.cpp:262-319) on the session's submap poses, on the host in double precision:
+ * one SE3 vertex per submap (vertex 0 fixed), for i > num_adjacent_pose_cnstraints (k) the odometry edges
+ * (i-k+j, i), j = 0..k-1, then the loop edges; identity information; g2o's Levenberg-Marquardt for max_iterations
+ * (the node uses 10), with an exact block-envelope Cholesky solve. poses_out = 16 * n_submaps doubles, column-major
+ * (the adjusted Isometry3d of every vertex; vertex 0 is fixed). The session's own submap poses are NOT changed:
+ * searchLoop, updateMap and the targeted cloud keep using the frontend's poses, as in the reference.
+ * B200REG_ERR_ARG for a loop edge id outside [0, n_submaps) or from == to, a non-finite relative_pose,
+ * num_adjacent_pose_cnstraints < 1 or max_iterations < 0. optimizer.save("pose_graph.g2o") (:319) is not reproduced. */
+int b200sm_pose_adjust(b200sm_t s, int num_adjacent_pose_cnstraints, const b200sm_loop_edge* loop_edges, int n_loop_edges,
+                       int max_iterations, double* poses_out, b200sm_pose_adjust_result* result);
+/* The map of every submap moved by a pose cast to float (modified map gbs.cpp:321-368; publishMap sm.cpp:529-552 when
+ * poses == NULL, i.e. the submaps' own poses), assembled on the device in one launch. Output is x, y, z, intensity
+ * floats in submap order. *n = total points; min(*n, capacity) points are copied, so capacity 0 is a size query (it
+ * launches nothing). offsets (may be NULL) = n_submaps + 1 prefix sums: submap i is out[offsets[i] .. offsets[i+1]),
+ * which is the cloud of modified_map_array's i-th SubMap. savePCDFileASCII("map.pcd") (:369) is not reproduced.      */
+int b200sm_assemble_map(b200sm_t s, const double* poses_colmajor16, float* out_xyzi, size_t capacity, size_t* n,
+                        size_t* offsets);
+
 typedef struct b200sm_stats {
   size_t n_scan, n_filtered, n_targeted, n_submaps;
   int kernel_launches;

@@ -318,6 +318,24 @@ class ScanMatcherSession {
     b200sm_num_submaps(s_.get(), &n);
     return n;
   }
+  // doPoseAdjustment's solve (gbs.cpp:262-319): poses = 16 * numSubmaps() doubles, column-major per submap
+  b200sm_pose_adjust_result poseAdjust(const std::vector<b200sm_loop_edge>& loop_edges, std::vector<double>& poses,
+                                       int num_adjacent_pose_cnstraints = 5, int max_iterations = 10) {
+    poses.resize(16 * numSubmaps());
+    b200sm_pose_adjust_result r{};
+    check(b200sm_pose_adjust(s_.get(), num_adjacent_pose_cnstraints, loop_edges.data(), (int)loop_edges.size(), max_iterations,
+                             poses.data(), &r));
+    return r;
+  }
+  // the map moved by `poses` (nullptr: the submaps' own poses, publishMap); xyzi = 4 floats per point in submap order,
+  // offsets = numSubmaps() + 1 prefix sums (modified_map_array's i-th cloud is [offsets[i], offsets[i+1]))
+  void assembleMap(const double* poses_colmajor16, std::vector<float>& xyzi, std::vector<size_t>& offsets) {
+    size_t n = 0;
+    offsets.resize(numSubmaps() + 1);
+    check(b200sm_assemble_map(s_.get(), poses_colmajor16, nullptr, 0, &n, offsets.data()));
+    xyzi.resize(4 * n);
+    check(b200sm_assemble_map(s_.get(), poses_colmajor16, xyzi.data(), n, &n, nullptr));
+  }
   b200sm_t handle() const { return s_.get(); }
 
  private:

@@ -40,7 +40,7 @@ SYMBOLS = [
     "b200sm_set_scan", "b200sm_update_map", "b200sm_receive_cloud", "b200sm_num_submaps", "b200sm_get_targeted",
     "b200sm_get_submap", "b200sm_get_filtered_scan", "b200sm_get_stats", "b200sm_search_loop", "b200sm_search_loop_all", "b200sm_import_submap",
     "b200sm_imu_set_scan_period", "b200sm_imu_push", "b200sm_deskew_next_scan", "b200sm_imu_adjust_distortion",
-    "b200sm_imu_get_state", "b200sm_imu_get_sample",
+    "b200sm_imu_get_state", "b200sm_imu_get_sample", "b200sm_pose_adjust", "b200sm_assemble_map",
     # include/b200comm.h
     "b200comm_unique_id", "b200comm_create", "b200comm_destroy", "b200comm_all_gather_rows", "b200comm_rank", "b200comm_last_error",
     "b200comm_board_create", "b200comm_board_destroy", "b200comm_board_info",
@@ -51,6 +51,15 @@ class SmLoopResult(C.Structure):
     _fields_ = [("is_candidate", C.c_int), ("id_min", C.c_int), ("accepted", C.c_int), ("pad", C.c_int),
                 ("min_dist", C.c_double), ("fitness", C.c_double), ("final_T", C.c_float * 16),
                 ("relative_pose", C.c_double * 16), ("n_source", C.c_size_t), ("n_target", C.c_size_t)]
+
+
+class SmLoopEdge(C.Structure):
+    _fields_ = [("from_", C.c_int), ("to", C.c_int), ("relative_pose", C.c_double * 16)]
+
+
+class SmPoseAdjustResult(C.Structure):
+    _fields_ = [("chi2_initial", C.c_double), ("chi2_final", C.c_double), ("iterations", C.c_int), ("trials", C.c_int),
+                ("n_vertices", C.c_int), ("n_edges", C.c_int)]
 
 
 class SmStats(C.Structure):
@@ -174,6 +183,8 @@ def lib() -> C.CDLL:
     L.b200sm_imu_adjust_distortion.argtypes = [vp, vp, sz, sz, C.c_long, d]
     L.b200sm_imu_get_state.argtypes = [vp, C.POINTER(i), C.POINTER(i), C.POINTER(i)]
     L.b200sm_imu_get_sample.argtypes = [vp, i, C.POINTER(d), vp, vp, vp]
+    L.b200sm_pose_adjust.argtypes = [vp, i, vp, i, i, vp, C.POINTER(SmPoseAdjustResult)]
+    L.b200sm_assemble_map.argtypes = [vp, vp, vp, sz, C.POINTER(sz), vp]
     L.b200comm_unique_id.argtypes = [vp]
     L.b200comm_create.argtypes = [vp, i, i, i, C.POINTER(vp)]
     L.b200comm_destroy.argtypes = [vp]

@@ -9,6 +9,10 @@
 //              num_targeted_cloud-1 submaps through transformPointCloud(Affine3d::matrix())      :438-463   -> b200sm_update_map
 //   receiveCloud: setInputTarget(targeted) (GICP: VoxelGrid(vg_size_for_input) first)             :300-322   -> b200sm_update_map
 //   receiveCloud / publishMapAndPose pose bookkeeping                     :330-353, 391-434     -> b200sm_receive_cloud
+//   publishMap: transformPointCloud(Matrix4f) of every submap + concatenation                :529-552   -> b200sm_assemble_map
+// and in the backend node (graph_based_slam/src/graph_based_slam_component.cpp):
+//   doPoseAdjustment: g2o pose graph + LM (host, pose_graph.hpp)                            :262-319   -> b200sm_pose_adjust
+//   doPoseAdjustment: modified_map / modified_map_array                                     :321-368   -> b200sm_assemble_map
 // The submaps (sensor-frame, voxel-filtered) and the targeted cloud never leave the GPU; read-back entry points exist for
 // the parity tests and for the node's publishers.
 #include <cmath>
@@ -20,6 +24,7 @@
 #include "../../include/b200reg.h"
 #include "deskew.hpp"
 #include "engine.hpp"
+#include "pose_graph.hpp"
 
 namespace b200 {
 namespace {
@@ -91,6 +96,52 @@ struct Submap {
   double distance = 0;
 };
 
+// Map assembly (publishMap sm.cpp:529-552, modified_map gbs.cpp:321-368): one table entry per submap, uploaded per call.
+struct AssembleEntry {
+  const float4* cloud;
+  unsigned long long out_offset;  // first output point of this submap
+  unsigned n, first_tile;         // points; first tile (block) of this submap in the launch
+  Mat34f T;                       // pose cast to float, 3x4 row-major
+};
+constexpr int ASSEMBLE_THREADS = 256, ASSEMBLE_PER_THREAD = 4, ASSEMBLE_TILE = ASSEMBLE_THREADS * ASSEMBLE_PER_THREAD;
+
+// Every submap moved by its float pose, concatenated in submap order, in ONE launch: block b serves tile b of the map; its
+// submap is the last entry with first_tile <= b (empty submaps own no tile). Each point is one float4 read and one float4
+// write; the arithmetic is transform_point's, so a point is bitwise what transform_cloud_device gives for its submap and
+// what pcl::transformPointCloud(Matrix4f) gives on the host. The intensity in .w is copied.
+__global__ void __launch_bounds__(ASSEMBLE_THREADS) assemble_map_kernel(const AssembleEntry* __restrict__ table, int n_sub,
+                                                                        float4* __restrict__ out) {
+  const unsigned tile = blockIdx.x;
+  int lo = 0, hi = n_sub - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (table[mid].first_tile <= tile) lo = mid;
+    else hi = mid - 1;
+  }
+  const AssembleEntry& e = table[lo];
+  float T[12];
+#pragma unroll
+  for (int k = 0; k < 12; k++) T[k] = e.T.m[k];
+  const unsigned n = e.n;
+  const unsigned base = (tile - e.first_tile) * (unsigned)ASSEMBLE_TILE + threadIdx.x;
+  const float4* __restrict__ in = e.cloud;
+  float4* __restrict__ dst = out + e.out_offset;
+  float4 p[ASSEMBLE_PER_THREAD];
+#pragma unroll
+  for (int j = 0; j < ASSEMBLE_PER_THREAD; j++) {  // all loads in flight before the first store
+    const unsigned i = base + j * ASSEMBLE_THREADS;
+    if (i < n) p[j] = in[i];
+  }
+#pragma unroll
+  for (int j = 0; j < ASSEMBLE_PER_THREAD; j++) {
+    const unsigned i = base + j * ASSEMBLE_THREADS;
+    if (i < n) {
+      const float3 r = transform_point(T, p[j]);
+      dst[i] = make_float4(r.x, r.y, r.z, p[j].w);
+    }
+  }
+}
+
 }  // namespace
 }  // namespace b200
 
@@ -124,6 +175,8 @@ struct b200sm_session {
   DeviceBuffer<float4> targeted;
   size_t n_targeted = 0;
   DeviceBuffer<float4> loop_src, loop_tgt;  // search_loop scratch
+  DeviceBuffer<AssembleEntry> assemble_table;
+  DeviceBuffer<float4> assembled;           // the last map b200sm_assemble_map built
   int launches = 0;
   // frontend bookkeeping (ScanMatcherComponent members)
   bool initial_cloud_received = false;
@@ -162,44 +215,6 @@ int sm_guarded(b200sm_t s, F&& f) {
 int sm_fail(b200sm_t s, int code, const char* msg) {
   s->err = msg;
   return code;
-}
-
-// tf2::fromMsg(pose, Affine3d) = Translation3d(p) * Quaterniond(w, x, y, z): Eigen's QuaternionBase::toRotationMatrix
-void pose_to_matrix_d(const double* p, const double* q, double* M /* row-major 16 */) {
-  const double x = q[0], y = q[1], z = q[2], w = q[3];
-  const double tx = 2.0 * x, ty = 2.0 * y, tz = 2.0 * z;
-  const double twx = tx * w, twy = ty * w, twz = tz * w;
-  const double txx = tx * x, txy = ty * x, txz = tz * x;
-  const double tyy = ty * y, tyz = tz * y, tzz = tz * z;
-  M[0] = 1.0 - (tyy + tzz); M[1] = txy - twz;         M[2] = txz + twy;          M[3] = p[0];
-  M[4] = txy + twz;         M[5] = 1.0 - (txx + tzz); M[6] = tyz - twx;          M[7] = p[1];
-  M[8] = txz - twy;         M[9] = tyz + twx;         M[10] = 1.0 - (txx + tyy); M[11] = p[2];
-  M[12] = 0; M[13] = 0; M[14] = 0; M[15] = 1;
-}
-
-// Eigen::Quaterniond(Matrix3d): the trace / largest-diagonal branches of Eigen's quaternionbase_assign_impl (3x3)
-void matrix_to_quat_d(const double* R /* row-major 9 */, double* q /* x y z w */) {
-  auto m = [&](int r, int c) { return R[r * 3 + c]; };
-  double t = m(0, 0) + m(1, 1) + m(2, 2);
-  if (t > 0.0) {
-    t = std::sqrt(t + 1.0);
-    q[3] = 0.5 * t;
-    t = 0.5 / t;
-    q[0] = (m(2, 1) - m(1, 2)) * t;
-    q[1] = (m(0, 2) - m(2, 0)) * t;
-    q[2] = (m(1, 0) - m(0, 1)) * t;
-  } else {
-    int i = 0;
-    if (m(1, 1) > m(0, 0)) i = 1;
-    if (m(2, 2) > m(i, i)) i = 2;
-    const int j = (i + 1) % 3, k = (j + 1) % 3;
-    t = std::sqrt(m(i, i) - m(j, j) - m(k, k) + 1.0);
-    q[i] = 0.5 * t;
-    t = 0.5 / t;
-    q[3] = (m(k, j) - m(j, k)) * t;
-    q[j] = (m(j, i) + m(i, j)) * t;
-    q[k] = (m(k, i) + m(i, k)) * t;
-  }
 }
 
 void upload_frame(b200sm_t s, const float* points, size_t n, size_t stride, long intensity_off) {
@@ -728,6 +743,85 @@ int b200sm_import_submap(b200sm_t s, const float* points, size_t n, size_t strid
     s->latest_distance = distance;
     s->submaps.push_back(std::move(sub));
     return (int)B200REG_OK;
+  });
+}
+
+// doPoseAdjustment (gbs.cpp:262-319): the pose graph over the submaps' poses and LM on the host (csrc/pose_graph.hpp).
+// The session's poses stay as they are.
+int b200sm_pose_adjust(b200sm_t s, int num_adjacent_pose_cnstraints, const b200sm_loop_edge* loop_edges, int n_loop_edges,
+                       int max_iterations, double* poses_out, b200sm_pose_adjust_result* result) {
+  if (!s || !poses_out || num_adjacent_pose_cnstraints < 1 || max_iterations < 0 || n_loop_edges < 0 || (n_loop_edges && !loop_edges))
+    return B200REG_ERR_ARG;
+  const int n = (int)s->submaps.size();
+  for (int l = 0; l < n_loop_edges; l++) {
+    const b200sm_loop_edge& e = loop_edges[l];
+    if (e.from < 0 || e.from >= n || e.to < 0 || e.to >= n || e.from == e.to)
+      return sm_fail(s, B200REG_ERR_ARG, "pose_adjust: loop edge with a submap id out of range or from == to");
+    for (int k = 0; k < 16; k++)
+      if (!std::isfinite(e.relative_pose[k])) return sm_fail(s, B200REG_ERR_ARG, "pose_adjust: non-finite relative_pose");
+  }
+  return sm_guarded(s, [&]() {
+    std::vector<pg::Iso> X(n);
+    for (int i = 0; i < n; i++) X[i] = pg::iso_from_rowmajor16(s->submaps[i]->pose);
+    std::vector<int> ids(2 * (size_t)n_loop_edges);
+    std::vector<pg::Iso> rel(n_loop_edges);
+    for (int l = 0; l < n_loop_edges; l++) {
+      ids[2 * l] = loop_edges[l].from;
+      ids[2 * l + 1] = loop_edges[l].to;
+      rel[l] = pg::iso_from_colmajor16(loop_edges[l].relative_pose);
+    }
+    const std::vector<pg::Edge> edges = pg::build_edges(X, num_adjacent_pose_cnstraints, ids.data(), rel.data(), n_loop_edges);
+    const pg::LmResult r = pg::optimize(X, edges, max_iterations);
+    for (int i = 0; i < n; i++) pg::iso_to_colmajor16(X[i], poses_out + 16 * (size_t)i);
+    if (result) {
+      result->chi2_initial = r.chi2_initial;
+      result->chi2_final = r.chi2_final;
+      result->iterations = r.iterations;
+      result->trials = r.trials;
+      result->n_vertices = n;
+      result->n_edges = (int)edges.size();
+    }
+    return (int)B200REG_OK;
+  });
+}
+
+// publishMap (sm.cpp:529-552) / modified_map (gbs.cpp:321-368): every submap through its pose cast to float, concatenated in
+// submap order, in one launch into a session buffer, then read back (count always reported, at most capacity copied).
+int b200sm_assemble_map(b200sm_t s, const double* poses_colmajor16, float* out_xyzi, size_t capacity, size_t* n, size_t* offsets) {
+  if (!s || (!out_xyzi && capacity)) return B200REG_ERR_ARG;
+  return sm_guarded(s, [&]() {
+    const int n_sub = (int)s->submaps.size();
+    size_t total = 0;
+    for (int i = 0; i < n_sub; i++) {
+      if (offsets) offsets[i] = total;
+      total += s->submaps[i]->n;
+    }
+    if (offsets) offsets[n_sub] = total;
+    if (n) *n = total;
+    if (capacity == 0 || total == 0) return (int)B200REG_OK;  // a size query launches nothing
+    std::vector<AssembleEntry> table(n_sub);
+    unsigned long long tiles = 0;
+    for (int i = 0; i < n_sub; i++) {
+      const Submap& sub = *s->submaps[i];
+      AssembleEntry& e = table[i];
+      e.cloud = sub.cloud;
+      e.out_offset = i ? table[i - 1].out_offset + table[i - 1].n : 0;
+      if (sub.n > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "assemble_map: a submap of 2^32 points or more");
+      e.n = (unsigned)sub.n;
+      e.first_tile = (unsigned)tiles;
+      tiles += (sub.n + ASSEMBLE_TILE - 1) / ASSEMBLE_TILE;
+      for (int r = 0; r < 3; r++)
+        for (int c = 0; c < 4; c++)
+          e.T.m[r * 4 + c] = poses_colmajor16 ? (float)poses_colmajor16[16 * (size_t)i + c * 4 + r] : (float)sub.pose[r * 4 + c];
+    }
+    if (tiles > 0x7fffffffull) return sm_fail(s, B200REG_ERR_ARG, "assemble_map: map too large for one launch");
+    s->assemble_table.ensure(n_sub);
+    s->assembled.ensure(total);
+    B200_CUDA(cudaMemcpyAsync(s->assemble_table.ptr, table.data(), n_sub * sizeof(AssembleEntry), cudaMemcpyHostToDevice, s->stream));
+    assemble_map_kernel<<<(unsigned)tiles, ASSEMBLE_THREADS, 0, s->stream>>>(s->assemble_table.ptr, n_sub, s->assembled.ptr);
+    B200_CUDA(cudaGetLastError());
+    s->launches += 1;
+    return read_back(s, s->assembled.ptr, total, out_xyzi, capacity, n);
   });
 }
 

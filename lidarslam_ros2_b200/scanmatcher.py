@@ -135,6 +135,38 @@ class ScanMatcher:
             out.append(d)
         return out
 
+    def poseAdjust(self, loop_edges, num_adjacent_pose_cnstraints: int = 5, max_iterations: int = 10):
+        """GraphBasedSlamComponent::doPoseAdjustment's pose-graph solve (gbs.cpp:262-319) over the session's submap poses:
+        loop_edges is a list of (from, to, relative_pose 4x4), e.g. (r["id_min"], numSubmaps() - 1, r["relative_pose"]) of
+        an accepted searchLoop. Returns (adjusted poses (N, 4, 4) float64, result dict); the session's poses are unchanged."""
+        edges = (_capi.SmLoopEdge * max(1, len(loop_edges)))()
+        for k, (f, t, Z) in enumerate(loop_edges):
+            edges[k].from_, edges[k].to = int(f), int(t)
+            edges[k].relative_pose[:] = np.asarray(Z, dtype=np.float64).T.reshape(16).tolist()
+        n = self.numSubmaps()
+        poses = np.zeros((max(1, n), 16), dtype=np.float64)
+        r = _capi.SmPoseAdjustResult()
+        self._check(self._lib.b200sm_pose_adjust(self._h, int(num_adjacent_pose_cnstraints), edges, len(loop_edges),
+                                                 int(max_iterations), _ptr(poses), C.byref(r)))
+        return (poses[:n].reshape(n, 4, 4).transpose(0, 2, 1).copy(),
+                {k: getattr(r, k) for k, _ in _capi.SmPoseAdjustResult._fields_})
+
+    def assembleMap(self, poses=None, capacity=None):
+        """The map of every submap moved by its pose cast to float (publishMap sm.cpp:529-552 when poses is None, else the
+        modified map of gbs.cpp:321-368), assembled on the device in one launch. Returns (cloud (M, 4) float32, offsets
+        (N + 1,) int64): submap i is cloud[offsets[i]:offsets[i + 1]]. capacity: copy at most that many points."""
+        n_sub = self.numSubmaps()
+        P = None
+        if poses is not None:
+            P = np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(n_sub, 4, 4).transpose(0, 2, 1))
+        offsets = np.zeros(n_sub + 1, dtype=np.uint64)
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_assemble_map(self._h, _ptr(P) if P is not None else None, None, 0, C.byref(n), _ptr(offsets)))
+        cap = n.value if capacity is None else min(int(capacity), n.value)
+        out = np.empty((max(cap, 1), 4), dtype=np.float32)
+        self._check(self._lib.b200sm_assemble_map(self._h, _ptr(P) if P is not None else None, _ptr(out), cap, C.byref(n), None))
+        return out[:cap], offsets.astype(np.int64)
+
     # ---- read-back ----
     def stats(self) -> dict:
         st = _capi.SmStats()
