@@ -246,6 +246,35 @@ typedef struct b200reg_ndt_trace_record {
 } b200reg_ndt_trace_record;
 int b200reg_ndt_set_trace(b200reg_t h, int capacity);
 int b200reg_ndt_get_trace(b200reg_t h, b200reg_ndt_trace_record* out, int capacity, int* n);
+/* GICP read-back for the optimiser tests: an opt-in trace of b200reg_align (batch calls are never traced), one stream of
+ * records in the order they happen. estimateRigidTransformationBFGS (gicp_omp_impl.hpp:180-241) appends a type 0 record
+ * per functor call and a type 1 record per minimizeOneStep; each outer iteration of computeTransformation (:369-515)
+ * ends with a type 2 record. Both BFGS paths trace: the device controller (each of the twelve T words is written by the
+ * controller thread that published it) and the host BFGS of a handle created with B200REG_GICP_HOST_BFGS.
+ * b200reg_gicp_set_trace(h, capacity) keeps room for `capacity` records (0 turns tracing off); b200reg_gicp_get_trace
+ * copies min(*n, capacity, cap) records of the last align() and sets *n to the number of records it produced, which
+ * exceeds the capacity when the trace overflowed. Fields a record type does not use are 0. */
+typedef struct b200reg_gicp_trace_record {
+  int type;               /* 0 functor call, 1 minimizeOneStep, 2 outer iteration                                    */
+  int outer;              /* outer iteration, from 0                                                                 */
+  int inner;              /* 0, 1: the inner iteration (0 = minimizeInit's call); 2: inner iterations the BFGS ran   */
+  int evaluation;         /* 0: index of the call in its BFGS run, from 0; 1, 2: calls made so far in the run        */
+  int want_grad;          /* 0: 0 operator() (f only), 1 fdf / df                                                    */
+  int status;             /* 1: minimizeOneStep's status; 2: the BFGS result, -2 when m < 4 stopped the loop         */
+  int m;                  /* 2: correspondences of the iteration                                                     */
+  int nr_iterations;      /* 2: after the iteration                                                                  */
+  int converged;          /* 2: after the iteration                                                                  */
+  int last;               /* 2: 1 on the last record of the align(), which carries final_T                           */
+  double x[6];            /* 0: the state the call was made at; 1: x after the step; 2: x the BFGS returned          */
+  double f;               /* 0: f returned to the BFGS; 1: f after the step                                          */
+  double g[6];            /* 0: g returned to the BFGS (0 for f-only calls); 1: the gradient after the step          */
+  double x0[6];           /* 2: the state extracted from transformation_                                             */
+  double delta;           /* 2: the convergence delta                                                                */
+  float T[12];            /* 0: the row-major 3x4 transform published for the call; 2: transformation_ after applyState */
+  float final_T[16];      /* 2, last record: final_transformation_, row-major                                        */
+} b200reg_gicp_trace_record;
+int b200reg_gicp_set_trace(b200reg_t h, int capacity);
+int b200reg_gicp_get_trace(b200reg_t h, b200reg_gicp_trace_record* out, int capacity, int* n);
 /* exact 1-NN of n query points against the target cloud (building block of getFitnessScore / GICP) */
 int b200reg_nn1(b200reg_t h, const float* base, size_t n, size_t stride_bytes, int* idx, float* d2);
 

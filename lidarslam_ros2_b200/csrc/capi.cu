@@ -252,7 +252,7 @@ int ndt_align_end(b200reg_t h) {
   return fail(h, B200REG_ERR_TIMEOUT, "NDT solver did not finish");
 }
 
-int gicp_align(b200reg_t h, const float* guess_colmajor) {
+int gicp_align(b200reg_t h, const float* guess_colmajor, bool traced) {
   h->converged = 0;
   set_identity(h->final_T);
   if (!h->have_target) return fail(h, B200REG_ERR_NO_TARGET, "align: no input target");
@@ -264,7 +264,7 @@ int gicp_align(b200reg_t h, const float* guess_colmajor) {
   h->gicp.corr_dist = h->corr_dist;
   B200_CUDA(cudaEventRecord(h->ev0, h->stream));
   GicpOutcome out = h->gicp_solver.align(h->nn, h->d_target.ptr, h->n_target, h->src_view, h->n_source, h->gicp, T,
-                                         h->stream);
+                                         h->stream, traced);
   B200_CUDA(cudaEventRecord(h->ev1, h->stream));
   B200_CUDA(cudaEventSynchronize(h->ev1));
   B200_CUDA(cudaEventElapsedTime(&h->solve_ms, h->ev0, h->ev1));
@@ -502,7 +502,7 @@ int b200reg_align(b200reg_t h, const float* guess, float* final_out) {
       rc = ndt_align_begin(h, guess);
       if (rc == B200REG_OK) rc = ndt_align_end(h);
     } else {
-      rc = gicp_align(h, guess);
+      rc = gicp_align(h, guess, true);
     }
     if (final_out) row_to_col(h->final_T, final_out);
     return rc;
@@ -519,7 +519,7 @@ int b200reg_align_batch(b200reg_t* handles, int count, const float* guesses, flo
     if (!h) return B200REG_ERR_ARG;
     const float* g = guesses ? guesses + 16 * i : nullptr;
     const int rc = guarded(h, [&]() {
-      if (h->kind != B200REG_NDT) return gicp_align(h, g);
+      if (h->kind != B200REG_NDT) return gicp_align(h, g, false);
       int r = ndt_align_begin(h, g);
       if (r == B200REG_OK) r = ndt_align_end(h);
       return r;
@@ -776,6 +776,22 @@ int b200reg_ndt_get_trace(b200reg_t h, b200reg_ndt_trace_record* out, int capaci
   if (!h || h->kind != B200REG_NDT || !n || capacity < 0) return B200REG_ERR_ARG;
   return guarded(h, [&]() {
     *n = h->solver.read_trace(out, capacity);
+    return (int)B200REG_OK;
+  });
+}
+
+int b200reg_gicp_set_trace(b200reg_t h, int capacity) {
+  if (!h || h->kind != B200REG_GICP || capacity < 0) return B200REG_ERR_ARG;
+  return guarded(h, [&]() {
+    h->gicp_solver.set_trace(capacity);
+    return (int)B200REG_OK;
+  });
+}
+
+int b200reg_gicp_get_trace(b200reg_t h, b200reg_gicp_trace_record* out, int capacity, int* n) {
+  if (!h || h->kind != B200REG_GICP || !n || capacity < 0) return B200REG_ERR_ARG;
+  return guarded(h, [&]() {
+    *n = h->gicp_solver.read_trace(out, capacity);
     return (int)B200REG_OK;
   });
 }

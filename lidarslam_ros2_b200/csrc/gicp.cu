@@ -396,6 +396,8 @@ struct GicpInnerLaunch {
   int max_inner;
   unsigned epoch;
   int eval_once;  // 0: the BFGS; GI_EVAL_F / GI_EVAL_FDF: exactly one fn.f / fn.fdf call at x0 (read-back tests)
+  b200reg_gicp_trace_record* trace;  // nullptr: not traced; else pinned host records [trace_base, trace_cap) are free
+  int trace_cap, trace_base, trace_outer;
 };
 
 __device__ __forceinline__ unsigned long long gi_ld(const unsigned long long* p) {
@@ -459,7 +461,42 @@ __device__ void r_derivative_dev(const double* x, const double* R, double* g) {
   g[5] = r5;
 }
 
-// the functor the controller CTA's BFGS drives: every thread of the CTA calls it with identical arguments
+// a[k] for k in [0, 6) without indexing the array dynamically (which would move it, and the BFGS state around it, to
+// local memory); 0 otherwise
+__device__ __forceinline__ double pick6(const double* a, int k) {
+  double v = 0.0;
+#pragma unroll
+  for (int i = 0; i < 6; i++)
+    if (i == k) v = a[i];
+  return v;
+}
+
+// one trace record, written by the controller threads together: thread k < 12 writes the transform word k it published
+// itself (so that a record whose twelve words match the transform of its x shows that the threads agreed), thread 12 the
+// header and f, threads 16..21 x and 24..29 g
+__device__ __noinline__ void gi_trace_write(b200reg_gicp_trace_record* r, int type, int outer, int inner, int evaluation,
+                                            int want_grad, int status, double f, double xv, double gv, unsigned word) {
+  const int tid = threadIdx.x;
+  if (tid < 12) {
+    if (type == 0) r->T[tid] = __uint_as_float(word);
+  } else if (tid == 12) {
+    r->type = type;
+    r->outer = outer;
+    r->inner = inner;
+    r->evaluation = evaluation;
+    r->want_grad = want_grad;
+    r->status = status;
+    r->f = f;
+  } else if (tid >= 16 && tid < 22) {
+    r->x[tid - 16] = xv;
+  } else if (tid >= 24 && tid < 30) {
+    r->g[tid - 24] = gv;
+  }
+}
+
+// the functor the controller CTA's BFGS drives: every thread of the CTA calls it with identical arguments. Trace: the
+// instantiation of traced launches (the untraced one carries no trace code)
+template <bool Trace>
 struct GicpDeviceFunctor {
   const GicpInnerLaunch* L;
   double (*red)[K7_SLOTS];  // shared [16][16]
@@ -467,6 +504,20 @@ struct GicpDeviceFunctor {
   int n_eval;
   int round;                // evaluations published so far (identical in every thread)
   int failed;
+  int inner;                // inner iteration of the BFGS the calls belong to (0: minimizeInit), for the trace
+  int tn;                   // trace records written by this launch (identical in every thread)
+
+  // appends one trace record of this launch (every thread counts it; nothing is written past the capacity). Each thread
+  // picks the one value it writes here, so that the BFGS state stays in registers; the stores are out of line.
+  __device__ void trace(int type, int evaluation, int want_grad, int status, const double* x, const double* g, double f,
+                        unsigned word) {
+    const int idx = L->trace_base + tn;
+    tn += 1;
+    if (idx >= L->trace_cap) return;
+    const int tid = threadIdx.x;
+    gi_trace_write(L->trace + idx, type, L->trace_outer, inner, evaluation, want_grad, status, f, pick6(x, tid - 16),
+                   g ? pick6(g, tid - 24) : 0.0, word);
+  }
 
   __device__ void evaluate(const double* x, int want_grad, double& f, double* g) {
     GicpInnerWork* W = L->work;
@@ -474,8 +525,9 @@ struct GicpDeviceFunctor {
     float T[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
     apply_state_dev(T, x);
     // publish {payload, sequence}: thread k owns word k
+    unsigned payload = 0;
     if (tid < GI_CTL_WORDS) {
-      const unsigned payload = tid < 12 ? __float_as_uint(T[tid]) : (tid == 12 ? (unsigned)want_grad : (unsigned)GI_MODE_RUN);
+      payload = tid < 12 ? __float_as_uint(T[tid]) : (tid == 12 ? (unsigned)want_grad : (unsigned)GI_MODE_RUN);
       const unsigned long long v = ((unsigned long long)(L->epoch * 65536u + (unsigned)round + 1u) << 32) | payload;
 #pragma unroll
       for (int c = 0; c < GI_CTL_COPIES; c++) gi_st(&W->ctl[c][tid], v);
@@ -534,13 +586,14 @@ struct GicpDeviceFunctor {
     const double m = L->m;
     if (!want_grad) {
       f = tot[0] / m;
-      return;
+    } else {
+      f = tot[1] / m;
+      double R[9];
+      for (int k = 0; k < 3; k++) g[k] = tot[2 + k] * (2.0 / m);
+      for (int k = 0; k < 9; k++) R[k] = tot[5 + k] * (2.0 / m);
+      r_derivative_dev(x, R, g);
     }
-    f = tot[1] / m;
-    double R[9];
-    for (int k = 0; k < 3; k++) g[k] = tot[2 + k] * (2.0 / m);
-    for (int k = 0; k < 9; k++) R[k] = tot[5 + k] * (2.0 / m);
-    r_derivative_dev(x, R, g);
+    if (Trace) trace(0, round - 1, want_grad, 0, x, want_grad ? g : nullptr, f, payload);  // one record per call
   }
   __device__ double f(const double* x) {
     double v;
@@ -554,6 +607,7 @@ struct GicpDeviceFunctor {
   }
 };
 
+template <bool Trace>
 __global__ void __launch_bounds__(GI_THREADS) gicp_inner_kernel(const __grid_constant__ GicpInnerLaunch L) {
   GicpInnerWork* W = L.work;
   const int tid = threadIdx.x;
@@ -561,8 +615,8 @@ __global__ void __launch_bounds__(GI_THREADS) gicp_inner_kernel(const __grid_con
   if ((int)blockIdx.x == n_eval) {  // ---- controller CTA: every thread runs the same BFGS ----
     __shared__ double red[16][K7_SLOTS];
     __shared__ double tot[K7_SLOTS];
-    GicpDeviceFunctor fn{&L, red, tot, n_eval, 0, 0};
-    Bfgs6T<GicpDeviceFunctor> bfgs(fn);
+    GicpDeviceFunctor<Trace> fn{&L, red, tot, n_eval, 0, 0, 0, 0};
+    Bfgs6T<GicpDeviceFunctor<Trace>> bfgs(fn);
     double x[6];
     for (int k = 0; k < 6; k++) x[k] = L.x0[k];
     int inner = 0;
@@ -576,7 +630,9 @@ __global__ void __launch_bounds__(GI_THREADS) gicp_inner_kernel(const __grid_con
       result = BFGS_Running;
       do {  // gicp_omp_impl.hpp:215-230
         inner++;
+        fn.inner = inner;
         result = bfgs.minimizeOneStep(x);
+        if (Trace) fn.trace(1, fn.round, 0, result, x, bfgs.gradient, bfgs.f, 0u);  // one record per step
         if (result) break;
         result = bfgs.testGradient(L.gradient_tol);
       } while (result == BFGS_Running && inner < L.max_inner && !fn.failed);
@@ -600,6 +656,7 @@ __global__ void __launch_bounds__(GI_THREADS) gicp_inner_kernel(const __grid_con
       r->inner = inner;
       r->evaluations = fn.round;
       r->error = fn.failed ? 1 : 0;
+      r->trace_n = L.trace_base + fn.tn;
       __threadfence_system();
     }
     return;
@@ -710,6 +767,12 @@ int GicpSolver::inner_loop_device(double* x, const GicpConfig& cfg, int* inner_i
   L.gradient_tol = cfg.gradient_tol;
   L.max_inner = cfg.max_inner_iterations;
   L.epoch = inner_epoch_++;
+  if (tracing_ && eval_once == GI_EVAL_BFGS) {
+    L.trace = h_trace_;
+    L.trace_cap = trace_cap_;
+    L.trace_base = trace_n_;
+    L.trace_outer = trace_outer_;
+  }
   h_inner_result_->error = 3;  // "the kernel never wrote a result"
   const int max_ctas = std::min(sm_count_, GI_MAX_CTAS);
   const int n_eval = std::max(1, std::min((int)((n_source_ + GI_THREADS - 1) / GI_THREADS), max_ctas - 1));
@@ -721,7 +784,8 @@ int GicpSolver::inner_loop_device(double* x, const GicpConfig& cfg, int* inner_i
   {
     std::lock_guard<std::mutex> coop(cooperative_launch_mutex(device_));
     B200_CUDA(cudaEventRecord(ev0_, stream_));
-    B200_CUDA(cudaLaunchCooperativeKernel((const void*)gicp_inner_kernel, dim3(n_eval + 1), dim3(GI_THREADS), args, 0, stream_));
+    const void* kernel = L.trace ? (const void*)gicp_inner_kernel<true> : (const void*)gicp_inner_kernel<false>;
+    B200_CUDA(cudaLaunchCooperativeKernel(kernel, dim3(n_eval + 1), dim3(GI_THREADS), args, 0, stream_));
     B200_CUDA(cudaEventRecord(ev1_, stream_));
     B200_CUDA(cudaStreamSynchronize(stream_));
   }
@@ -740,6 +804,7 @@ int GicpSolver::inner_loop_device(double* x, const GicpConfig& cfg, int* inner_i
     throw CudaError("GICP inner-loop kernel watchdog fired");
   }
   for (int k = 0; k < 6; k++) x[k] = r.x[k];
+  if (L.trace) trace_n_ = r.trace_n;
   evaluations_ += r.evaluations;
   inner_pair_evaluations += (double)r.evaluations * (double)last_m_;
   *inner_iterations = r.inner;
@@ -897,8 +962,34 @@ void GicpSolver::evaluate(const double* x, bool want_grad, double* f, double* g6
   for (int k = 0; k < 12; k++) T12[k] = T[k];
 }
 
+void GicpSolver::set_trace(int capacity) {
+  if (h_trace_) B200_CUDA(cudaFreeHost(h_trace_));
+  h_trace_ = nullptr;
+  trace_cap_ = 0;
+  trace_n_ = 0;
+  if (capacity > 0) {
+    B200_CUDA(cudaMallocHost(&h_trace_, (size_t)capacity * sizeof(b200reg_gicp_trace_record)));
+    trace_cap_ = capacity;
+  }
+}
+
+int GicpSolver::read_trace(b200reg_gicp_trace_record* out, int cap) const {
+  const int k = std::min(std::min(trace_n_, trace_cap_), cap);
+  if (out && k > 0) std::memcpy(out, h_trace_, (size_t)k * sizeof(b200reg_gicp_trace_record));
+  return trace_n_;
+}
+
+b200reg_gicp_trace_record* GicpSolver::trace_slot(int type) {
+  const int idx = trace_n_++;
+  if (idx >= trace_cap_) return nullptr;
+  b200reg_gicp_trace_record* r = h_trace_ + idx;
+  r->type = type;
+  r->outer = trace_outer_;
+  return r;
+}
+
 GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, size_t n_target, const float4* source,
-                              size_t n_source, const GicpConfig& cfg, const float* guess16, cudaStream_t s) {
+                              size_t n_source, const GicpConfig& cfg, const float* guess16, cudaStream_t s, bool traced) {
   // developer trace (env B200REG_GICP_TRACE=1): host wall clock per phase of one align, printed to stderr
   static const bool trace = getenv("B200REG_GICP_TRACE") != nullptr;
   auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
@@ -914,6 +1005,11 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
   inner_ms = 0;
   inner_launches = 0;
   inner_pair_evaluations = 0;
+  tracing_ = traced && trace_cap_ > 0;
+  trace_n_ = 0;
+  trace_outer_ = 0;
+  if (tracing_) std::memset(h_trace_, 0, (size_t)trace_cap_ * sizeof(b200reg_gicp_trace_record));
+  b200reg_gicp_trace_record* outer_rec = nullptr;  // the outer iteration's record (the last one receives final_T)
   GicpOutcome out;
   set_identity16(out.final_T);
   out.converged = 0;
@@ -931,7 +1027,14 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
     const int m = correspondences(target_grid, cfg, guess16, transformation, s);
     lap(t_nn);
     std::memcpy(previous, transformation, sizeof(previous));
-    if (m < 4) break;  // NotEnoughPointsException → caught → break (:187-192, :494-498)
+    if (m < 4) {  // NotEnoughPointsException → caught → break (:187-192, :494-498)
+      if (tracing_ && (outer_rec = trace_slot(2))) {
+        outer_rec->status = BFGS_NotStarted;
+        outer_rec->m = m;
+        outer_rec->nr_iterations = nr_iterations;
+      }
+      break;
+    }
 
     // estimateRigidTransformationBFGS (:180-241)
     double x[6];
@@ -941,6 +1044,21 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
     x[3] = std::atan2(transformation[9], transformation[10]);
     x[4] = std::asin(-transformation[8]);
     x[5] = std::atan2(transformation[4], transformation[0]);
+    double x0[6];
+    for (int k = 0; k < 6; k++) x0[k] = x[k];
+    int inner = 0, calls = 0;
+    // trace of the host BFGS: one record per functor call, as the device controller writes them
+    auto trace_call = [&](const double* xx, int want_grad, double f, const double* gg, const float* T) {
+      b200reg_gicp_trace_record* r = trace_slot(0);
+      if (!r) return;
+      r->inner = inner;
+      r->evaluation = calls;
+      r->want_grad = want_grad;
+      r->f = f;
+      for (int k = 0; k < 6; k++) r->x[k] = xx[k];
+      for (int k = 0; k < 6; k++) r->g[k] = want_grad ? gg[k] : 0.0;
+      for (int k = 0; k < 12; k++) r->T[k] = T[k];
+    };
     BfgsFunctor6 fn;
     fn.f = [&](const double* xx) {
       float T[16];
@@ -948,6 +1066,8 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
       apply_state(T, xx);
       double f;
       fdf(T, false, &f, nullptr, nullptr);
+      if (tracing_) trace_call(xx, 0, f, nullptr, T);
+      calls++;
       return f;
     };
     fn.fdf = [&](const double* xx, double& f, double* gg) {
@@ -958,13 +1078,15 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
       fdf(T, true, &f, gt, R);
       for (int q = 0; q < 3; q++) gg[q] = gt[q];
       r_derivative(xx, R, gg);
+      if (tracing_) trace_call(xx, 1, f, gg, T);
+      calls++;
     };
     fn.df = [&](const double* xx, double* gg) {
       double f;
       fn.fdf(xx, f, gg);
     };
-    int inner = 0;
     int result;
+    const int evaluations_before = evaluations_;
     if (device_bfgs) {
       result = inner_loop_device(x, cfg, &inner);
     } else {
@@ -974,11 +1096,30 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
       do {
         inner++;
         result = bfgs.minimizeOneStep(x);
+        if (tracing_) {
+          if (b200reg_gicp_trace_record* r = trace_slot(1)) {
+            r->inner = inner;
+            r->evaluation = calls;
+            r->status = result;
+            r->f = bfgs.f;
+            for (int k = 0; k < 6; k++) r->x[k] = x[k];
+            for (int k = 0; k < 6; k++) r->g[k] = bfgs.gradient[k];
+          }
+        }
         if (result) break;
         result = bfgs.testGradient(cfg.gradient_tol);
       } while (result == BFGS_Running && inner < cfg.max_inner_iterations);
     }
     lap(t_inner);
+    if (tracing_ && (outer_rec = trace_slot(2))) {
+      outer_rec->inner = inner;
+      outer_rec->evaluation = evaluations_ - evaluations_before;
+      outer_rec->status = result;
+      outer_rec->m = m;
+      outer_rec->nr_iterations = nr_iterations;
+      for (int k = 0; k < 6; k++) outer_rec->x0[k] = x0[k];
+      for (int k = 0; k < 6; k++) outer_rec->x[k] = x[k];
+    }
     if (!(result == BFGS_NoProgress || result == BFGS_Success || inner == cfg.max_inner_iterations)) break;  // throws in the reference
     set_identity16(transformation);
     apply_state(transformation, x);
@@ -995,6 +1136,14 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
       converged = true;
       std::memcpy(previous, transformation, sizeof(previous));
     }
+    if (outer_rec) {
+      for (int k = 0; k < 12; k++) outer_rec->T[k] = transformation[k];
+      outer_rec->delta = delta;
+      outer_rec->nr_iterations = nr_iterations;
+      outer_rec->converged = converged ? 1 : 0;
+    }
+    trace_outer_ += 1;
+    outer_rec = nullptr;
   }
   // final = previous * guess in f32 (:511)
   for (int i = 0; i < 4; i++)
@@ -1006,6 +1155,12 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
   out.converged = converged ? 1 : 0;
   out.iterations = nr_iterations;
   out.evaluations = evaluations_;
+  if (tracing_ && trace_n_ > 0 && trace_n_ <= trace_cap_ && h_trace_[trace_n_ - 1].type == 2) {
+    b200reg_gicp_trace_record* r = h_trace_ + trace_n_ - 1;
+    r->last = 1;
+    std::memcpy(r->final_T, out.final_T, sizeof(r->final_T));
+  }
+  tracing_ = false;
   if (trace)
     std::fprintf(stderr, "[gicp trace] source grid + covariances + transform %.3f ms, correspondences (NN + Mahalanobis) %.3f ms, "
                          "inner BFGS launches %.3f ms (kernel events %.3f ms), %d outer iterations, %d evaluations\n",

@@ -30,10 +30,14 @@ struct GicpInnerResult {  // written by the kernel into pinned host memory
   double g[6];  // gradient at x: the BFGS's last one, or the evaluate-once call's (zero for an f-only call)
   float T[12];  // row-major 3x4 transform apply_state_dev builds from x
   int status, inner, evaluations, error;
+  int trace_n;  // trace records produced so far in the align(), when traced
 };
 
 class GicpSolver {
  public:
+  ~GicpSolver() {
+    if (h_trace_) cudaFreeHost(h_trace_);
+  }
   void init(int device, cudaStream_t s);
   void invalidate_target() {
     target_cov_valid_ = false;
@@ -46,8 +50,10 @@ class GicpSolver {
   }
   // the correspondences of the last K6 pass still refer to the clouds set now (no setInput* since)
   bool correspondences_current() const { return corr_current_; }
+  // traced: record the trace set up by set_trace (single aligns; batch calls pass false)
   GicpOutcome align(const NnGrid& target_grid, const float4* target, size_t n_target, const float4* source,
-                    size_t n_source, const GicpConfig& cfg, const float* guess_rowmajor16, cudaStream_t s);
+                    size_t n_source, const GicpConfig& cfg, const float* guess_rowmajor16, cudaStream_t s,
+                    bool traced = false);
   // the two halves of align()'s work, public for the read-back tests:
   // prelude: lazy covariances (K5), the source grid, moved = guess * source
   void prepare(const NnGrid& target_grid, const float4* target, size_t n_target, const float4* source, size_t n_source,
@@ -75,6 +81,9 @@ class GicpSolver {
   float inner_ms = 0;
   int inner_launches = 0;
   double inner_pair_evaluations = 0;
+  // opt-in trace of align() (b200reg_gicp_set_trace / b200reg_gicp_get_trace): functor calls, BFGS steps, outer iterations
+  void set_trace(int capacity);
+  int read_trace(b200reg_gicp_trace_record* out, int cap) const;  // copies up to cap records, returns the records counted
 
  private:
   void fdf(const float* T_rowmajor16, bool want_grad, double* f, double* g_t3, double* R9);
@@ -106,6 +115,13 @@ class GicpSolver {
   const float4* target_ = nullptr;
   int last_m_ = 0;
   int evaluations_ = 0;
+  // pinned, device-visible: the inner kernel's controller writes its call and step records there directly
+  b200reg_gicp_trace_record* h_trace_ = nullptr;
+  int trace_cap_ = 0;
+  int trace_n_ = 0;      // records produced by the current / last align()
+  int trace_outer_ = 0;  // outer iteration being traced
+  bool tracing_ = false; // the current align() is traced
+  b200reg_gicp_trace_record* trace_slot(int type);  // next record, zeroed (nullptr past the capacity); counts it
 };
 
 // k-NN based point covariances of a cloud against its own grid (gicp_omp_impl.hpp:48-122)

@@ -453,6 +453,28 @@ class GeneralizedIterativeClosestPoint(_Registration):
         T4[:3] = T.reshape(3, 4)
         return f.value, (g if want_grad else None), T4
 
+    # b200reg_gicp_trace_record as a numpy record (include/b200reg.h); tests/test_host_logic.py checks size and offsets.
+    # type: 0 functor call, 1 minimizeOneStep, 2 outer iteration
+    TRACE_DTYPE = np.dtype([(k, np.int32) for k in (
+        "type", "outer", "inner", "evaluation", "want_grad", "status", "m", "nr_iterations", "converged", "last")]
+        + [("x", np.float64, (6,)), ("f", np.float64), ("g", np.float64, (6,)), ("x0", np.float64, (6,)),
+           ("delta", np.float64), ("T", np.float32, (12,)), ("final_T", np.float32, (16,))])
+
+    def setTrace(self, capacity: int):
+        """Record the optimiser's functor calls, BFGS steps and outer iterations of every following align()
+        (b200reg_gicp_set_trace); 0 turns it off."""
+        self._trace_cap = int(capacity)
+        self._check(self._lib.b200reg_gicp_set_trace(self._h, self._trace_cap))
+
+    def trace(self):
+        """The records of the last traced align() as a TRACE_DTYPE record array, and the number of records it produced
+        (larger than the array when the capacity set by setTrace was exceeded)."""
+        cap = getattr(self, "_trace_cap", 0)
+        out = np.zeros(cap, dtype=self.TRACE_DTYPE)
+        n = C.c_int(0)
+        self._check(self._lib.b200reg_gicp_get_trace(self._h, _ptr(out) if cap else None, cap, C.byref(n)))
+        return out[:min(n.value, cap)].copy(), n.value
+
 
 def align_batch(engines, guesses=None) -> np.ndarray:
     """Batched loop-closure sweep on one GPU: all solves are enqueued before any is awaited. Returns (K,4,4)."""

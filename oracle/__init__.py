@@ -97,6 +97,9 @@ def lib() -> C.CDLL:
         L.oracle_gicp_f_only.restype = C.c_double
         L.oracle_gicp_apply_state.argtypes = [vp, vp, vp]
         L.oracle_gicp_correspondences.argtypes = [vp, vp, vp, vp]
+        L.oracle_gicp_set_trace.argtypes = [vp, C.c_int]
+        L.oracle_gicp_get_trace.argtypes = [vp, vp, C.c_int]
+        L.oracle_gicp_get_trace.restype = C.c_int
         _lib = L
     return _lib
 
@@ -234,6 +237,12 @@ class NDT:
 class GICP:
     """CPU restatement of pclomp::GeneralizedIterativeClosestPoint (gicp_omp.h:60-369)."""
 
+    # GicpTraceRec (oracle/gicp.hpp), the layout of the engine's b200reg_gicp_trace_record
+    TRACE_DTYPE = np.dtype([(k, np.int32) for k in (
+        "type", "outer", "inner", "evaluation", "want_grad", "status", "m", "nr_iterations", "converged", "last")]
+        + [("x", np.float64, (6,)), ("f", np.float64), ("g", np.float64, (6,)), ("x0", np.float64, (6,)),
+           ("delta", np.float64), ("T", np.float32, (12,)), ("final_T", np.float32, (16,))])
+
     def __init__(self, **params):
         self._h = lib().oracle_gicp_create()
         self.final_transformation = np.eye(4, dtype=np.float32)
@@ -270,6 +279,18 @@ class GICP:
 
     def fitness(self, max_range: float = np.finfo(np.float64).max) -> float:
         return float(lib().oracle_gicp_fitness(self._h, float(max_range)))
+
+    def set_trace(self, on: bool = True):
+        """Record the optimiser's functor calls, BFGS steps and outer iterations of every following align()."""
+        lib().oracle_gicp_set_trace(self._h, int(bool(on)))
+
+    def trace(self) -> np.ndarray:
+        """The records of the last align() as a TRACE_DTYPE record array."""
+        n = lib().oracle_gicp_get_trace(self._h, None, 0)
+        out = np.zeros(n, dtype=self.TRACE_DTYPE)
+        if n:
+            lib().oracle_gicp_get_trace(self._h, _ptr(out), n)
+        return out
 
     def covariances(self, which: str):
         w = 1 if which == "target" else 0

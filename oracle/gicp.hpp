@@ -30,6 +30,14 @@
 
 namespace oracle {
 
+// opt-in record of the optimiser (same layout as the engine's b200reg_gicp_trace_record, include/b200reg.h): type 0 per
+// functor call, 1 per minimizeOneStep, 2 per outer iteration
+struct GicpTraceRec {
+  int type, outer, inner, evaluation, want_grad, status, m, nr_iterations, converged, last;
+  double x[6], f, g[6], x0[6], delta;
+  float T[12], final_T[16];
+};
+
 class GICP {
  public:
   // gicp_omp.h:108-128
@@ -45,6 +53,8 @@ class GICP {
   float final_transformation[16];
   bool converged = false;
   int nr_iterations = 0;
+  bool trace_on = false;
+  std::vector<GicpTraceRec> trace;
 
   std::vector<P3> target, input;
   KdTree tree, tree_reciprocal;
@@ -217,7 +227,18 @@ class GICP {
 
   // gicp_omp_impl.hpp:180-241. Returns false where the reference throws.
   bool estimateRigidTransformationBFGS(float* transformation_matrix) {
-    if (src_idx.size() < 4) return false;
+    if (src_idx.size() < 4) {
+      if (trace_on) {
+        GicpTraceRec r{};
+        r.type = 2;
+        r.outer = nr_iterations;
+        r.status = -2;  // BFGS not started
+        r.m = (int)src_idx.size();
+        r.nr_iterations = nr_iterations;
+        trace.push_back(r);
+      }
+      return false;
+    }
     double x[6];
     const float* t = transformation_matrix;
     x[0] = t[3];
@@ -226,20 +247,59 @@ class GICP {
     x[3] = std::atan2(t[9], t[10]);   // (2,1),(2,2)
     x[4] = std::asin(-t[8]);          // -(2,0)
     x[5] = std::atan2(t[4], t[0]);    // (1,0),(0,0)
+    double x0[6];
+    std::memcpy(x0, x, sizeof(x0));
+    int inner_iterations = 0, calls = 0;
+    auto record = [&](int type, int want_grad, const double* xx, double f, const double* gg) {
+      GicpTraceRec r{};
+      r.type = type;
+      r.outer = nr_iterations;
+      r.inner = inner_iterations;
+      r.evaluation = calls;
+      r.want_grad = want_grad;
+      std::memcpy(r.x, xx, sizeof(r.x));
+      r.f = f;
+      if (gg) std::memcpy(r.g, gg, sizeof(r.g));
+      if (type == 0) {
+        float T[16];
+        std::memcpy(T, base_transformation, sizeof(T));
+        applyState(T, xx);
+        std::memcpy(r.T, T, sizeof(r.T));
+      }
+      trace.push_back(r);
+      return &trace.back();
+    };
     BfgsFunctor6 fn;
-    fn.f = [this](const double* xx) { return f_only(xx); };
-    fn.df = [this](const double* xx, double* gg) { double f; fdf(xx, f, gg); };
-    fn.fdf = [this](const double* xx, double& f, double* gg) { fdf(xx, f, gg); };
+    fn.f = [&](const double* xx) {
+      const double f = f_only(xx);
+      if (trace_on) record(0, 0, xx, f, nullptr);
+      calls++;
+      return f;
+    };
+    fn.df = [&](const double* xx, double* gg) { double f; fn.fdf(xx, f, gg); };
+    fn.fdf = [&](const double* xx, double& f, double* gg) {
+      fdf(xx, f, gg);
+      if (trace_on) record(0, 1, xx, f, gg);
+      calls++;
+    };
     BFGS6 bfgs(fn);
-    int inner_iterations = 0;
     int result = bfgs.minimizeInit(x);
     result = BFGS_Running;
     do {
       inner_iterations++;
       result = bfgs.minimizeOneStep(x);
+      if (trace_on) record(1, 0, x, bfgs.f, bfgs.gradient)->status = result;
       if (result) break;
       result = bfgs.testGradient(gradient_tol);
     } while (result == BFGS_Running && inner_iterations < max_inner_iterations);
+    if (trace_on) {
+      GicpTraceRec* r = record(2, 0, x, 0.0, nullptr);
+      r->f = 0;
+      r->status = result;
+      r->m = (int)src_idx.size();
+      r->nr_iterations = nr_iterations;
+      std::memcpy(r->x0, x0, sizeof(x0));
+    }
     if (result == BFGS_NoProgress || result == BFGS_Success || inner_iterations == max_inner_iterations) {
       NDT::set_identity(transformation_matrix);
       applyState(transformation_matrix, x);
@@ -252,6 +312,7 @@ class GICP {
   void align(const float* guess_in) {
     converged = false;
     NDT::set_identity(final_transformation);
+    trace.clear();
     if (target.empty() || input.empty()) return;
     float guess[16];
     if (guess_in) std::memcpy(guess, guess_in, sizeof(guess));
@@ -325,6 +386,13 @@ class GICP {
         converged = true;
         std::memcpy(previous, transformation, sizeof(previous));
       }
+      if (trace_on) {
+        GicpTraceRec& r = trace.back();
+        std::memcpy(r.T, transformation, sizeof(r.T));
+        r.delta = delta;
+        r.nr_iterations = nr_iterations;
+        r.converged = converged ? 1 : 0;
+      }
     }
     // final = previous * guess (float)
     for (int i = 0; i < 4; i++)
@@ -333,6 +401,10 @@ class GICP {
         for (int k = 0; k < 4; k++) s += previous[i * 4 + k] * guess[k * 4 + j];
         final_transformation[i * 4 + j] = s;
       }
+    if (trace_on && !trace.empty() && trace.back().type == 2) {
+      trace.back().last = 1;
+      std::memcpy(trace.back().final_T, final_transformation, sizeof(final_transformation));
+    }
   }
 
   double getFitnessScore(double max_range = std::numeric_limits<double>::max()) {

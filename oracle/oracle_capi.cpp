@@ -278,6 +278,14 @@ void oracle_gicp_apply_state(void* h, const double* x6, float* T_colmajor) {
   GICP::applyState(T, x6);
   row_to_col(T, T_colmajor);
 }
+// opt-in trace of align()'s optimiser (GicpTraceRec); get returns the record count and copies up to cap records
+void oracle_gicp_set_trace(void* h, int on) { static_cast<GICP*>(h)->trace_on = on != 0; }
+int oracle_gicp_get_trace(void* h, void* out, int cap) {
+  const auto& t = static_cast<GICP*>(h)->trace;
+  const size_t k = std::min(t.size(), (size_t)std::max(cap, 0));
+  if (out && k) std::memcpy(out, t.data(), k * sizeof(GicpTraceRec));
+  return (int)t.size();
+}
 // correspondences of the last outer iteration: source / target indices and the source point's Mahalanobis matrix
 // (row-major 3x3 floats), m of each
 void oracle_gicp_correspondences(void* h, int* src_idx, int* tgt_idx, float* maha9) {

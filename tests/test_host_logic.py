@@ -198,6 +198,32 @@ def test_abi_header_is_plain_c():
                                "-fsyntax-only", src])
 
 
+def _check_trace_layout(dt, ctype):
+    import subprocess
+    import tempfile
+
+    body = "".join(f'printf("{k} %zu\\n", offsetof({ctype}, {k}));' for k in dt.names)
+    with tempfile.TemporaryDirectory() as d:
+        src, exe = os.path.join(d, "layout.c"), os.path.join(d, "layout")
+        with open(src, "w") as f:
+            f.write('#include <stddef.h>\n#include <stdio.h>\n#include "b200reg.h"\nint main(void){'
+                    f'printf("sizeof %zu\\n", sizeof({ctype}));' + body + "return 0;}\n")
+        subprocess.check_call(["gcc", "-std=c99", "-Wall", "-Werror", "-I" + os.path.join(ROOT, "include"), src, "-o", exe])
+        got = dict(line.split() for line in subprocess.check_output([exe], text=True).splitlines())
+    assert int(got.pop("sizeof")) == dt.itemsize
+    assert {k: int(v) for k, v in got.items()} == {k: dt.fields[k][1] for k in dt.names}
+
+
+def test_gicp_trace_record_layout_matches_numpy():
+    """GeneralizedIterativeClosestPoint.trace() reads b200reg_gicp_trace_record through a numpy dtype (and the oracle's
+    trace uses the same layout): size and field offsets must be what a C compiler lays out for include/b200reg.h."""
+    import oracle
+    from lidarslam_ros2_b200.registration import GeneralizedIterativeClosestPoint as GICP
+
+    _check_trace_layout(GICP.TRACE_DTYPE, "b200reg_gicp_trace_record")
+    assert oracle.GICP.TRACE_DTYPE == GICP.TRACE_DTYPE
+
+
 def test_ndt_trace_record_layout_matches_numpy():
     """NormalDistributionsTransform.trace() reads b200reg_ndt_trace_record through a numpy dtype: its size and every field
     offset must be what a C compiler lays out for include/b200reg.h."""
