@@ -43,7 +43,8 @@ enum b200reg_status {
   B200REG_ERR_NO_SOURCE = -3, /* align without setInputSource                                          */
   B200REG_ERR_CUDA = -4,      /* CUDA runtime error, or no device                                      */
   B200REG_ERR_TIMEOUT = -5,   /* device-side watchdog fired inside the persistent solver               */
-  B200REG_ERR_GRID = -6       /* voxel grid would overflow int32 (voxel_grid_covariance_omp_impl.hpp:79) */
+  B200REG_ERR_GRID = -6,      /* voxel grid would overflow int32 (voxel_grid_covariance_omp_impl.hpp:79) */
+  B200REG_ERR_IO = -7         /* a file could not be opened or written                                 */
 };
 
 /* ---- lifetime --------------------------------------------------------------------------------------- */
@@ -395,9 +396,23 @@ int b200sm_pose_adjust(b200sm_t s, int num_adjacent_pose_cnstraints, const b200s
  * poses == NULL, i.e. the submaps' own poses), assembled on the device in one launch. Output is x, y, z, intensity
  * floats in submap order. *n = total points; min(*n, capacity) points are copied, so capacity 0 is a size query (it
  * launches nothing). offsets (may be NULL) = n_submaps + 1 prefix sums: submap i is out[offsets[i] .. offsets[i+1]),
- * which is the cloud of modified_map_array's i-th SubMap. savePCDFileASCII("map.pcd") (:369) is not reproduced.      */
+ * which is the cloud of modified_map_array's i-th SubMap.                                                            */
 int b200sm_assemble_map(b200sm_t s, const double* poses_colmajor16, float* out_xyzi, size_t capacity, size_t* n,
                         size_t* offsets);
+/* pcl::io::savePCDFileASCII(path, map) (gbs.cpp:369, the map_save service gbs.cpp:90-103) where map is what
+ * b200sm_assemble_map(s, poses_colmajor16, ...) returns (poses == NULL: the submaps' own poses): the PCD v0.7 header of a
+ * PointXYZI cloud and one "x y z intensity" line per point, every float as PCL prints it (ostream precision 8, "nan").
+ * The map is assembled and its text formatted on the device; the text comes to the host in chunks of a fixed number of
+ * points through two pinned buffers, the calling thread writing one chunk while the device encodes and copies the next.
+ * No point of the map is read back. The file is written in place. n_points, n_bytes (may be NULL) = points and file size.
+ * B200REG_ERR_ARG for an empty map (no file is created), B200REG_ERR_IO when the file cannot be opened or written.      */
+int b200sm_save_map_pcd_ascii(b200sm_t s, const double* poses_colmajor16, const char* path, size_t* n_points, size_t* n_bytes);
+/* The same text for a HOST PointXYZI cloud (records as in b200sm_import_submap; intensity_offset_bytes >= 0), formatted
+ * on `device`. *n_bytes = size of the whole file content (header and data); min(*n_bytes, capacity) bytes are copied to
+ * out, so capacity 0 is a size query. B200REG_ERR_ARG for n == 0, a negative intensity offset, or a stride or offset that
+ * is not a multiple of 4. */
+int b200reg_encode_pcd_ascii(int device, const float* base, size_t n, size_t stride_bytes, long intensity_offset_bytes,
+                             char* out, size_t capacity, size_t* n_bytes);
 
 typedef struct b200sm_stats {
   size_t n_scan, n_filtered, n_targeted, n_submaps;

@@ -336,6 +336,13 @@ class ScanMatcherSession {
     xyzi.resize(4 * n);
     check(b200sm_assemble_map(s_.get(), poses_colmajor16, xyzi.data(), n, &n, nullptr));
   }
+  // pcl::io::savePCDFileASCII(path, map) of the map assembleMap(poses_colmajor16, ...) builds (the map_save service),
+  // formatted on the device; throws like PCL for an empty map or a file that cannot be written. Returns the file size.
+  size_t saveMapPCDASCII(const std::string& path, const double* poses_colmajor16 = nullptr) {
+    size_t n = 0, bytes = 0;
+    check(b200sm_save_map_pcd_ascii(s_.get(), poses_colmajor16, path.c_str(), &n, &bytes));
+    return bytes;
+  }
   b200sm_t handle() const { return s_.get(); }
 
  private:

@@ -347,4 +347,23 @@ struct VoxelGridFilter {
   long long filter_device(const float4* d_in, size_t n, float leaf, cudaStream_t s, const Bounds* known_bounds = nullptr);
 };
 
+// ---- ASCII PCD text of a float4 (x, y, z, intensity) cloud (pcd_codec.cu) ------------------------------------------
+// The text is produced in chunks of PCD_CHUNK_POINTS points, so that a writer can hold two chunks in host memory and one
+// on the device whatever the size of the map.
+constexpr size_t PCD_CHUNK_POINTS = (size_t)1 << 22;
+// the header savePCDFileASCII writes for n PointXYZI points, "DATA ascii\n" included
+std::string pcd_ascii_header(size_t n);
+struct PcdEncoder {
+  DeviceBuffer<unsigned> counts;  // per chunk: tile byte counts, scanned in place into tile offsets, then the chunk's total
+  DeviceBuffer<unsigned> scan_tmp;
+  DeviceBuffer<char> text;        // the text of one chunk
+  PinnedBuffer<unsigned> h_counts;
+  std::vector<size_t> chunk_bytes;  // text bytes of every chunk, known after measure()
+  int launches = 0;
+  // pass 1 over the whole cloud and the per-chunk scans; fills chunk_bytes and sizes `text` (synchronises the stream)
+  void measure(const float4* pts, size_t n, cudaStream_t s);
+  // pass 2: the text of chunk c into `text` (enqueue only; the offsets are those of the last measure() of the same cloud)
+  void encode_chunk(const float4* pts, size_t n, size_t c, cudaStream_t s);
+};
+
 }  // namespace b200

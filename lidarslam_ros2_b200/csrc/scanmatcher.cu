@@ -13,9 +13,12 @@
 // and in the backend node (graph_based_slam/src/graph_based_slam_component.cpp):
 //   doPoseAdjustment: g2o pose graph + LM (host, pose_graph.hpp)                            :262-319   -> b200sm_pose_adjust
 //   doPoseAdjustment: modified_map / modified_map_array                                     :321-368   -> b200sm_assemble_map
+//   doPoseAdjustment: savePCDFileASCII("map.pcd", modified_map)                             :369       -> b200sm_save_map_pcd_ascii
 // The submaps (sensor-frame, voxel-filtered) and the targeted cloud never leave the GPU; read-back entry points exist for
 // the parity tests and for the node's publishers.
+#include <cerrno>
 #include <cmath>
+#include <cstdio>
 #include <cstring>
 #include <memory>
 #include <string>
@@ -176,7 +179,9 @@ struct b200sm_session {
   size_t n_targeted = 0;
   DeviceBuffer<float4> loop_src, loop_tgt;  // search_loop scratch
   DeviceBuffer<AssembleEntry> assemble_table;
-  DeviceBuffer<float4> assembled;           // the last map b200sm_assemble_map built
+  DeviceBuffer<float4> assembled;           // the last map b200sm_assemble_map / b200sm_save_map_pcd_ascii built
+  PcdEncoder pcd;                           // its ASCII PCD text, chunk by chunk
+  PinnedBuffer<char> pcd_staging[2];        // two chunks of text on the host: one being written while the next arrives
   int launches = 0;
   // frontend bookkeeping (ScanMatcherComponent members)
   bool initial_cloud_received = false;
@@ -785,8 +790,50 @@ int b200sm_pose_adjust(b200sm_t s, int num_adjacent_pose_cnstraints, const b200s
   });
 }
 
+}  // extern "C"
+
+namespace {
+
+size_t map_points(b200sm_t s) {
+  size_t total = 0;
+  for (const auto& sub : s->submaps) total += sub->n;
+  return total;
+}
+
 // publishMap (sm.cpp:529-552) / modified_map (gbs.cpp:321-368): every submap through its pose cast to float, concatenated in
-// submap order, in one launch into a session buffer, then read back (count always reported, at most capacity copied).
+// submap order, in one launch into s->assembled (total = map_points(s) > 0). Enqueue only.
+int assemble_on_device(b200sm_t s, const double* poses_colmajor16, size_t total) {
+  const int n_sub = (int)s->submaps.size();
+  std::vector<AssembleEntry> table(n_sub);
+  unsigned long long tiles = 0;
+  for (int i = 0; i < n_sub; i++) {
+    const Submap& sub = *s->submaps[i];
+    AssembleEntry& e = table[i];
+    e.cloud = sub.cloud;
+    e.out_offset = i ? table[i - 1].out_offset + table[i - 1].n : 0;
+    if (sub.n > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "assemble_map: a submap of 2^32 points or more");
+    e.n = (unsigned)sub.n;
+    e.first_tile = (unsigned)tiles;
+    tiles += (sub.n + ASSEMBLE_TILE - 1) / ASSEMBLE_TILE;
+    for (int r = 0; r < 3; r++)
+      for (int c = 0; c < 4; c++)
+        e.T.m[r * 4 + c] = poses_colmajor16 ? (float)poses_colmajor16[16 * (size_t)i + c * 4 + r] : (float)sub.pose[r * 4 + c];
+  }
+  if (tiles > 0x7fffffffull) return sm_fail(s, B200REG_ERR_ARG, "assemble_map: map too large for one launch");
+  s->assemble_table.ensure(n_sub);
+  s->assembled.ensure(total);
+  B200_CUDA(cudaMemcpyAsync(s->assemble_table.ptr, table.data(), n_sub * sizeof(AssembleEntry), cudaMemcpyHostToDevice, s->stream));
+  assemble_map_kernel<<<(unsigned)tiles, ASSEMBLE_THREADS, 0, s->stream>>>(s->assemble_table.ptr, n_sub, s->assembled.ptr);
+  B200_CUDA(cudaGetLastError());
+  s->launches += 1;
+  return (int)B200REG_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+// the assembled map read back (count always reported, at most capacity copied)
 int b200sm_assemble_map(b200sm_t s, const double* poses_colmajor16, float* out_xyzi, size_t capacity, size_t* n, size_t* offsets) {
   if (!s || (!out_xyzi && capacity)) return B200REG_ERR_ARG;
   return sm_guarded(s, [&]() {
@@ -799,29 +846,76 @@ int b200sm_assemble_map(b200sm_t s, const double* poses_colmajor16, float* out_x
     if (offsets) offsets[n_sub] = total;
     if (n) *n = total;
     if (capacity == 0 || total == 0) return (int)B200REG_OK;  // a size query launches nothing
-    std::vector<AssembleEntry> table(n_sub);
-    unsigned long long tiles = 0;
-    for (int i = 0; i < n_sub; i++) {
-      const Submap& sub = *s->submaps[i];
-      AssembleEntry& e = table[i];
-      e.cloud = sub.cloud;
-      e.out_offset = i ? table[i - 1].out_offset + table[i - 1].n : 0;
-      if (sub.n > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "assemble_map: a submap of 2^32 points or more");
-      e.n = (unsigned)sub.n;
-      e.first_tile = (unsigned)tiles;
-      tiles += (sub.n + ASSEMBLE_TILE - 1) / ASSEMBLE_TILE;
-      for (int r = 0; r < 3; r++)
-        for (int c = 0; c < 4; c++)
-          e.T.m[r * 4 + c] = poses_colmajor16 ? (float)poses_colmajor16[16 * (size_t)i + c * 4 + r] : (float)sub.pose[r * 4 + c];
-    }
-    if (tiles > 0x7fffffffull) return sm_fail(s, B200REG_ERR_ARG, "assemble_map: map too large for one launch");
-    s->assemble_table.ensure(n_sub);
-    s->assembled.ensure(total);
-    B200_CUDA(cudaMemcpyAsync(s->assemble_table.ptr, table.data(), n_sub * sizeof(AssembleEntry), cudaMemcpyHostToDevice, s->stream));
-    assemble_map_kernel<<<(unsigned)tiles, ASSEMBLE_THREADS, 0, s->stream>>>(s->assemble_table.ptr, n_sub, s->assembled.ptr);
-    B200_CUDA(cudaGetLastError());
-    s->launches += 1;
+    const int rc = assemble_on_device(s, poses_colmajor16, total);
+    if (rc != B200REG_OK) return rc;
     return read_back(s, s->assembled.ptr, total, out_xyzi, capacity, n);
+  });
+}
+
+// savePCDFileASCII("map.pcd", modified_map) (gbs.cpp:369): the map assembled and formatted on the device, its text copied
+// out chunk by chunk into two pinned buffers in turn. Chunk c + 1 is encoded and copied (one stream: encode, copy, encode,
+// ...) while this thread writes chunk c; a buffer is refilled only after its previous chunk has been written.
+int b200sm_save_map_pcd_ascii(b200sm_t s, const double* poses_colmajor16, const char* path, size_t* n_points, size_t* n_bytes) {
+  if (!s || !path) return B200REG_ERR_ARG;
+  return sm_guarded(s, [&]() {
+    const size_t total = map_points(s);
+    if (total == 0) return sm_fail(s, B200REG_ERR_ARG, "save_map_pcd_ascii: the map has no points");  // PCL throws, writes nothing
+    int rc = assemble_on_device(s, poses_colmajor16, total);
+    if (rc != B200REG_OK) return rc;
+    PcdEncoder& E = s->pcd;
+    const int launches_before = E.launches;
+    E.measure(s->assembled.ptr, total, s->stream);
+    s->launches += E.launches - launches_before;
+    const std::string header = pcd_ascii_header(total);
+    size_t file_bytes = header.size(), most = 0;
+    for (size_t b : E.chunk_bytes) {
+      file_bytes += b;
+      most = std::max(most, b);
+    }
+    if (n_points) *n_points = total;
+    if (n_bytes) *n_bytes = file_bytes;
+    for (auto& st : s->pcd_staging) st.ensure(most);
+    FILE* fp = std::fopen(path, "wb");
+    if (!fp) {
+      s->err = std::string("save_map_pcd_ascii: cannot open ") + path + ": " + std::strerror(errno);
+      return (int)B200REG_ERR_IO;
+    }
+    cudaEvent_t copied[2] = {nullptr, nullptr};
+    auto finish = [&](int code) {
+      for (cudaEvent_t& e : copied)
+        if (e) cudaEventDestroy(e);
+      if (std::fclose(fp) != 0 && code == B200REG_OK) {
+        s->err = std::string("save_map_pcd_ascii: writing ") + path + ": " + std::strerror(errno);
+        return (int)B200REG_ERR_IO;
+      }
+      return code;
+    };
+    try {
+      for (cudaEvent_t& e : copied) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+      const size_t chunks = E.chunk_bytes.size();
+      auto enqueue = [&](size_t c) {
+        E.encode_chunk(s->assembled.ptr, total, c, s->stream);
+        s->launches += 1;
+        B200_CUDA(cudaMemcpyAsync(s->pcd_staging[c & 1].ptr, E.text.ptr, E.chunk_bytes[c], cudaMemcpyDeviceToHost, s->stream));
+        B200_CUDA(cudaEventRecord(copied[c & 1], s->stream));
+      };
+      enqueue(0);
+      bool ok = std::fwrite(header.data(), 1, header.size(), fp) == header.size();
+      for (size_t c = 0; c < chunks && ok; c++) {
+        if (c + 1 < chunks) enqueue(c + 1);  // its buffer held chunk c - 1, already written
+        B200_CUDA(cudaEventSynchronize(copied[c & 1]));
+        ok = std::fwrite(s->pcd_staging[c & 1].ptr, 1, E.chunk_bytes[c], fp) == E.chunk_bytes[c];
+      }
+      if (!ok) {
+        s->err = std::string("save_map_pcd_ascii: writing ") + path + ": " + std::strerror(errno);
+        B200_CUDA(cudaStreamSynchronize(s->stream));  // no copy into the staging buffers is left in flight
+        return finish(B200REG_ERR_IO);
+      }
+    } catch (...) {
+      finish(B200REG_ERR_CUDA);
+      throw;
+    }
+    return finish(B200REG_OK);
   });
 }
 

@@ -6,6 +6,7 @@ The submaps and the targeted cloud live on the GPU; a frame costs one host-to-de
 from __future__ import annotations
 
 import ctypes as C
+import os
 
 import numpy as np
 
@@ -166,6 +167,18 @@ class ScanMatcher:
         out = np.empty((max(cap, 1), 4), dtype=np.float32)
         self._check(self._lib.b200sm_assemble_map(self._h, _ptr(P) if P is not None else None, _ptr(out), cap, C.byref(n), None))
         return out[:cap], offsets.astype(np.int64)
+
+    def saveMapPCDASCII(self, path, poses=None):
+        """pcl::io::savePCDFileASCII(path, map) of the map assembleMap(poses) returns (the map_save service, gbs.cpp:90-103,
+        369): assembled and formatted on the device, written chunk by chunk. Returns (points, file bytes). An empty map
+        raises with ERR_ARG and creates no file; a file that cannot be opened or written raises with ERR_IO."""
+        P = None
+        if poses is not None:
+            P = np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(self.numSubmaps(), 4, 4).transpose(0, 2, 1))
+        n, size = C.c_size_t(0), C.c_size_t(0)
+        self._check(self._lib.b200sm_save_map_pcd_ascii(self._h, _ptr(P) if P is not None else None, os.fsencode(path),
+                                                        C.byref(n), C.byref(size)))
+        return int(n.value), int(size.value)
 
     # ---- read-back ----
     def stats(self) -> dict:
