@@ -13,6 +13,8 @@ for f in grid_index voxel_map ndt_solver ndt_aux nn_grid voxelgrid gicp cloud_co
     # (20 iterations) amplifies that to centimetres on weakly constrained scenes. The NDT kernels spell their un-fused
     # arithmetic out with __fmul_rn / __fadd_rn where parity needs it.
     EXTRA=""; [ $f = gicp ] && EXTRA="-fmad=false"
+    # scanmatcher.cu: its host float arithmetic (csrc/sensor_frame.hpp) must match the un-fused device transform bit for bit
+    [ $f = scanmatcher ] && EXTRA="-Xcompiler -ffp-contract=off"
     $NVCC $FLAGS $EXTRA -Xptxas -v -c $f.cu -o $f.o 2> $f.ptxas.log || { cat $f.ptxas.log; exit 1; }
   fi
   OBJS="$OBJS $f.o"

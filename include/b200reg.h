@@ -312,6 +312,20 @@ int b200sm_update_map(b200sm_t s, b200reg_t reg, const float* final_T_colmajor16
  * pose7_out = position + quaternion after the frame; *map_updated = 1 if updateMap ran.                             */
 int b200sm_receive_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes,
                          long intensity_offset_bytes, double* pose7_out, float* final_T_colmajor16_out, int* map_updated);
+/* cloud_callback's tf2::doTransform(*msg, transformed_msg, transform) (sm.cpp:188-199): transform =
+ * lookupTransform(robot_frame_id_, msg->header.frame_id, stamp). Every later frame given to b200sm_set_scan /
+ * b200sm_receive_cloud is moved into the robot frame by the upload's unpack pass, before the de-skew, the range filter and
+ * both VoxelGrids, so the caller passes msg->data as it arrived. The matrix is tf2_sensor_msgs' Translation3f *
+ * Quaternionf(w, x, y, z) in float, the quaternion used as given (not normalised); each point is
+ * ((r0 x + r1 y) + r2 z) + t, intensity copied. A caller whose TF varies calls this before each frame. Both pointers
+ * NULL: off (the points are used as given). Non-finite values or a zero quaternion: B200REG_ERR_ARG.                 */
+int b200sm_set_sensor_transform(b200sm_t s, const double* translation3, const double* quat_xyzw);
+/* use_odom (sm.cpp:333-348) for the NEXT b200sm_receive_cloud: the odometry = lookupTransform(odom_frame_id_,
+ * robot_frame_id_, stamp). That frame's guess becomes sim_trans * previous_odom_mat_^-1 * odom_mat (all float; nothing
+ * changes while previous_odom_mat_ is exactly Identity, as on the first armed frame), then previous_odom_mat_ = odom_mat.
+ * A frame without an armed odometry keeps the current pose as its guess and leaves previous_odom_mat_ unchanged.
+ * Non-finite values or a zero quaternion: B200REG_ERR_ARG.                                                          */
+int b200sm_odom_next_scan(b200sm_t s, const double* translation3, const double* quat_xyzw);
 /* read-back (parity tests; the node's map / map_array publishers). Clouds are x, y, z, intensity floats. */
 int b200sm_num_submaps(b200sm_t s, size_t* out);
 int b200sm_get_targeted(b200sm_t s, float* out_xyzi, size_t capacity, size_t* n);

@@ -298,6 +298,15 @@ class ScanMatcherSession {
                             use_min_max_filter ? 1 : 0, scan_min_range, scan_max_range));
   }
   void setInitialPose(const double position[3], const double quat_xyzw[4]) { check(b200sm_set_initial_pose(s_.get(), position, quat_xyzw)); }
+  // cloud_callback's doTransform (sm.cpp:188-199): lookupTransform(robot_frame_id_, msg->header.frame_id, stamp), applied
+  // on the device to every later frame; (nullptr, nullptr) turns it off
+  void setSensorTransform(const double* translation3, const double* quat_xyzw) {
+    check(b200sm_set_sensor_transform(s_.get(), translation3, quat_xyzw));
+  }
+  // use_odom (sm.cpp:333-348): lookupTransform(odom_frame_id_, robot_frame_id_, stamp) for the next receiveCloud
+  void odomNextScan(const double translation3[3], const double quat_xyzw[4]) {
+    check(b200sm_odom_next_scan(s_.get(), translation3, quat_xyzw));
+  }
   // points: n structs of `stride` bytes with x, y, z floats first and the intensity float at `intensity_offset` (or -1)
   // pose7 = position + quaternion (x, y, z, w); final16 column-major like Eigen::Matrix4f::data()
   bool receiveCloud(b200reg_t reg, const float* points, size_t n, size_t stride, long intensity_offset, double pose7[7], float final16[16]) {

@@ -28,9 +28,13 @@ __global__ void unpack_points_kernel(const unsigned char* __restrict__ raw, size
   dst[i] = v;
 }
 // same + min/max of the finite points (the NDT voxel grid and the NN grid of a target are sized from them): one pass less
-// over the cloud and no separate round trip for the bounds
+// over the cloud and no separate round trip for the bounds.
+// kTransform: x, y, z go through T (transform_point) before the store, and the bounds are those of the transformed points
+// — tf2::doTransform of the frontend's cloud callback (scanmatcher_component.cpp:188-199) in the pass that reads the
+// records anyway. .w is copied untouched. The <false> instantiation has no transform code at all.
+template <bool kTransform>
 __global__ void unpack_points_bounds_kernel(const unsigned char* __restrict__ raw, size_t n, size_t stride, long w_off, float w_default,
-                                            float4* __restrict__ dst, unsigned* __restrict__ out6) {
+                                            float4* __restrict__ dst, unsigned* __restrict__ out6, Mat34f T) {
   const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
   if (i < n) {
@@ -41,6 +45,12 @@ __global__ void unpack_points_bounds_kernel(const unsigned char* __restrict__ ra
     v.y = f[1];
     v.z = f[2];
     v.w = w_off >= 0 ? *reinterpret_cast<const float*>(p + w_off) : w_default;
+    if (kTransform) {
+      const float3 r = transform_point(T.m, v);
+      v.x = r.x;
+      v.y = r.y;
+      v.z = r.z;
+    }
     dst[i] = v;
     if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) {
       mn[0] = mx[0] = v.x;
@@ -97,7 +107,7 @@ void staged_h2d(void* d_dst, const void* host, size_t bytes, bool pinned, unsign
 
 // upload + bounds: the result is valid after the caller has synchronised the stream (finish_bounds)
 void CloudUploader::upload_with_bounds(const void* host, size_t n, size_t stride, long w_off, float w_default, float4* dst,
-                                       cudaStream_t s) {
+                                       cudaStream_t s, const Mat34f* T) {
   if (n == 0) return;
   const size_t bytes = n * stride;
   raw.ensure(bytes);
@@ -109,7 +119,11 @@ void CloudUploader::upload_with_bounds(const void* host, size_t n, size_t stride
   std::memcpy(bounds_host.ptr, init, sizeof(init));
   B200_CUDA(cudaMemcpyAsync(bounds_dev.ptr, bounds_host.ptr, sizeof(init), cudaMemcpyHostToDevice, s));
   staged_h2d(raw.ptr, host, bytes, pinned, staging.ptr, s);
-  unpack_points_bounds_kernel<<<(int)((n + 255) / 256), 256, 0, s>>>(raw.ptr, n, stride, w_off, w_default, dst, bounds_dev.ptr);
+  const int blocks = (int)((n + 255) / 256);
+  if (T)
+    unpack_points_bounds_kernel<true><<<blocks, 256, 0, s>>>(raw.ptr, n, stride, w_off, w_default, dst, bounds_dev.ptr, *T);
+  else
+    unpack_points_bounds_kernel<false><<<blocks, 256, 0, s>>>(raw.ptr, n, stride, w_off, w_default, dst, bounds_dev.ptr, Mat34f{});
   B200_CUDA(cudaGetLastError());
   B200_CUDA(cudaMemcpyAsync(bounds_host.ptr, bounds_dev.ptr, sizeof(init), cudaMemcpyDeviceToHost, s));
   launches += 1;

@@ -105,10 +105,12 @@ struct CloudUploader {
   int launches = 0;
   // w_off >= 0: byte offset of the float that goes to .w (intensity); otherwise .w = w_default
   void upload(const void* host, size_t n, size_t stride, long w_off, float w_default, float4* dst, cudaStream_t s);
-  // upload + min/max of the finite points in the same pass; finish_bounds() is valid once the stream has been synchronised
+  // upload + min/max of the finite points in the same pass; finish_bounds() is valid once the stream has been synchronised.
+  // T (3x4 row-major, optional): every point's x, y, z is moved by T before the store and the bounds are the moved points'.
   DeviceBuffer<unsigned> bounds_dev;
   PinnedBuffer<unsigned> bounds_host;
-  void upload_with_bounds(const void* host, size_t n, size_t stride, long w_off, float w_default, float4* dst, cudaStream_t s);
+  void upload_with_bounds(const void* host, size_t n, size_t stride, long w_off, float w_default, float4* dst, cudaStream_t s,
+                          const Mat34f* T = nullptr);
   Bounds finish_bounds() const;
   // batched form (no synchronisation between clouds): reserve once, then upload_at per cloud at its byte offset
   void reserve(size_t raw_bytes, bool need_staging);

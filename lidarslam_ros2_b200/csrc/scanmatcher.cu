@@ -2,7 +2,9 @@
 // the callers either side of the registration hot path, built so that a frame costs ONE host-to-device copy.
 //
 // Replaces, in the reference's frontend node (scanmatcher/src/scanmatcher_component.cpp):
+//   cloud_callback tf2::doTransform into robot_frame_id_   :188-199   -> the upload's unpack pass (b200sm_set_sensor_transform)
 //   cloud_callback range filter                      :211-219   -> range_filter_kernel
+//   receiveCloud: use_odom initial guess             :333-348   -> b200sm_receive_cloud (b200sm_odom_next_scan)
 //   receiveCloud: VoxelGrid(vg_size_for_input) + setInputSource          :323-328   -> b200sm_set_scan
 //   initializeMap                                    :257-297   -> b200sm_update_map (first call)
 //   updateMap: VoxelGrid(vg_size_for_map), transformPointCloud(Matrix4f), concatenation of the last
@@ -28,6 +30,7 @@
 #include "deskew.hpp"
 #include "engine.hpp"
 #include "pose_graph.hpp"
+#include "sensor_frame.hpp"
 
 namespace b200 {
 namespace {
@@ -193,6 +196,13 @@ struct b200sm_session {
   ImuDeskew imu;
   bool deskew_armed = false;
   double deskew_scan_time = 0;
+  // cloud_callback's tf2::doTransform into robot_frame_id_ (sm.cpp:188-199), applied by the unpack pass of every frame
+  bool sensor_tf_set = false;
+  Mat34f sensor_tf{};
+  // use_odom (sm.cpp:333-348): the odometry armed for the next frame, and previous_odom_mat_ (row-major float)
+  bool odom_armed = false;
+  float odom_mat[16] = {};
+  float previous_odom_mat[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
 };
 
 namespace {
@@ -224,8 +234,10 @@ int sm_fail(b200sm_t s, int code, const char* msg) {
 
 void upload_frame(b200sm_t s, const float* points, size_t n, size_t stride, long intensity_off) {
   s->upload.ensure(n);
-  // one H2D copy per frame; the unpack pass also measures the scan's min/max (both VoxelGrids of the frame are sized from it)
-  s->uploader.upload_with_bounds(points, n, stride, intensity_off, 0.0f, s->upload.ptr, s->stream);
+  // one H2D copy per frame; the unpack pass also moves the points into the robot frame when a sensor transform is set, and
+  // measures the (moved) scan's min/max (both VoxelGrids of the frame are sized from it)
+  s->uploader.upload_with_bounds(points, n, stride, intensity_off, 0.0f, s->upload.ptr, s->stream,
+                                 s->sensor_tf_set ? &s->sensor_tf : nullptr);
   s->launches += 1;
   s->d_scan = s->upload.ptr;
   s->n_scan = n;
@@ -235,9 +247,20 @@ void upload_frame(b200sm_t s, const float* points, size_t n, size_t stride, long
     s->deskew_armed = false;
     deskewed = true;
     const char* b = reinterpret_cast<const char*>(points);
+    const float* first = reinterpret_cast<const float*>(b);
+    const float* last = reinterpret_cast<const float*>(b + (n - 1) * stride);
+    float first_t[3], last_t[3];
+    if (s->sensor_tf_set) {
+      // the de-skew's start / end azimuths are those of the robot-frame points: the first and last records are moved on
+      // the host with the kernel's un-fused float arithmetic (transform_point_f), bitwise what the unpack pass stores,
+      // so neither a read-back nor a synchronisation is added before the de-skew
+      transform_point_f(s->sensor_tf.m, first, first_t);
+      transform_point_f(s->sensor_tf.m, last, last_t);
+      first = first_t;
+      last = last_t;
+    }
     const int before = s->imu.launches;
-    s->imu.adjust_distortion(s->upload.ptr, n, reinterpret_cast<const float*>(b), reinterpret_cast<const float*>(b + (n - 1) * stride),
-                             s->deskew_scan_time, s->stream);
+    s->imu.adjust_distortion(s->upload.ptr, n, first, last, s->deskew_scan_time, s->stream);
     s->launches += s->imu.launches - before;
   }
   if (s->use_min_max_filter) {
@@ -456,6 +479,8 @@ int b200sm_receive_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t 
     return B200REG_ERR_ARG;
   return sm_guarded(s, [&]() {
     if (map_updated) *map_updated = 0;
+    const bool use_odom = s->odom_armed;  // armed for this frame only, like the de-skew
+    s->odom_armed = false;
     int kind = B200REG_NDT;
     b200reg_get_kind(reg, &kind);
     upload_frame(s, points, n, stride_bytes, intensity_offset_bytes);
@@ -484,6 +509,11 @@ int b200sm_receive_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t 
     rc = set_source_from_scan(s, reg);                // :323-328
     if (rc != B200REG_OK) return rc;
     sim_trans();
+    if (use_odom) {  // :333-348: sim_trans * previous_odom_mat_.inverse() * odom_mat, then previous_odom_mat_ = odom_mat
+      odom_guess_f(T_row, s->previous_odom_mat, s->odom_mat);
+      for (int r = 0; r < 4; r++)
+        for (int c = 0; c < 4; c++) sim_col[c * 4 + r] = T_row[r * 4 + c];
+    }
     float final_col[16];
     rc = b200reg_align(reg, sim_col, final_col);      // :350
     if (rc != B200REG_OK) {
@@ -953,6 +983,44 @@ int b200sm_deskew_next_scan(b200sm_t s, double scan_time) {
   if (!s) return B200REG_ERR_ARG;
   s->deskew_armed = true;
   s->deskew_scan_time = scan_time;
+  return B200REG_OK;
+}
+
+}  // extern "C"
+
+// ---- frame transforms of the cloud callback: doTransform into the robot frame (sm.cpp:188-199), use_odom (:333-348) ----
+namespace {
+bool valid_transform(const double* t3, const double* q_xyzw) {
+  for (int k = 0; k < 3; k++)
+    if (!std::isfinite(t3[k])) return false;
+  for (int k = 0; k < 4; k++)
+    if (!std::isfinite(q_xyzw[k])) return false;
+  return q_xyzw[0] != 0.0 || q_xyzw[1] != 0.0 || q_xyzw[2] != 0.0 || q_xyzw[3] != 0.0;
+}
+}  // namespace
+
+extern "C" {
+
+int b200sm_set_sensor_transform(b200sm_t s, const double* translation3, const double* quat_xyzw) {
+  if (!s) return B200REG_ERR_ARG;
+  if (!translation3 && !quat_xyzw) {
+    s->sensor_tf_set = false;
+    return B200REG_OK;
+  }
+  if (!translation3 || !quat_xyzw) return sm_fail(s, B200REG_ERR_ARG, "set_sensor_transform: one of translation / quaternion is NULL");
+  if (!valid_transform(translation3, quat_xyzw))
+    return sm_fail(s, B200REG_ERR_ARG, "set_sensor_transform: non-finite value or zero quaternion");
+  sensor_matrix_f(translation3, quat_xyzw, s->sensor_tf.m);
+  s->sensor_tf_set = true;
+  return B200REG_OK;
+}
+
+int b200sm_odom_next_scan(b200sm_t s, const double* translation3, const double* quat_xyzw) {
+  if (!s) return B200REG_ERR_ARG;
+  if (!translation3 || !quat_xyzw) return sm_fail(s, B200REG_ERR_ARG, "odom_next_scan: NULL translation or quaternion");
+  if (!valid_transform(translation3, quat_xyzw)) return sm_fail(s, B200REG_ERR_ARG, "odom_next_scan: non-finite value or zero quaternion");
+  odom_matrix_f(translation3, quat_xyzw, s->odom_mat);
+  s->odom_armed = true;
   return B200REG_OK;
 }
 

@@ -83,6 +83,24 @@ class ScanMatcher:
         """use_imu: de-skew the next frame on the device before the range filter (b200sm_deskew_next_scan)."""
         self._check(self._lib.b200sm_deskew_next_scan(self._h, float(scan_time)))
 
+    def setSensorTransform(self, position, quat_xyzw):
+        """cloud_callback's tf2::doTransform into the robot frame (sm.cpp:188-199), on the device for every later frame:
+        position / quat_xyzw are lookupTransform(robot_frame_id, cloud frame_id). setSensorTransform(None, None) turns it
+        off (b200sm_set_sensor_transform)."""
+        if position is None and quat_xyzw is None:
+            self._check(self._lib.b200sm_set_sensor_transform(self._h, None, None))
+            return
+        p = np.ascontiguousarray(position, dtype=np.float64).reshape(3)
+        q = np.ascontiguousarray(quat_xyzw, dtype=np.float64).reshape(4)
+        self._check(self._lib.b200sm_set_sensor_transform(self._h, _ptr(p), _ptr(q)))
+
+    def odomNextScan(self, position, quat_xyzw):
+        """use_odom: the odometry lookupTransform(odom_frame_id, robot_frame_id) for the next receiveCloud, whose guess
+        becomes pose * previous_odom^-1 * odom (sm.cpp:333-348; b200sm_odom_next_scan)."""
+        p = np.ascontiguousarray(position, dtype=np.float64).reshape(3)
+        q = np.ascontiguousarray(quat_xyzw, dtype=np.float64).reshape(4)
+        self._check(self._lib.b200sm_odom_next_scan(self._h, _ptr(p), _ptr(q)))
+
     def updateMap(self, final_transformation, position, quat_xyzw, adopt_now: bool = True):
         T = np.ascontiguousarray(np.asarray(final_transformation, dtype=np.float32).T).reshape(16)
         p = np.ascontiguousarray(position, dtype=np.float64)
