@@ -364,6 +364,13 @@ int b200sm_imu_adjust_distortion(b200sm_t s, float* points, size_t n, size_t str
 /* read-back for the parity tests: imu_ptr_front_, imu_ptr_last_, imu_ptr_last_iter_; one ring entry                */
 int b200sm_imu_get_state(b200sm_t s, int* ptr_front, int* ptr_last, int* ptr_last_iter);
 int b200sm_imu_get_sample(b200sm_t s, int index, double* stamp, float* rpy3, float* shift3, float* velo3);
+/* read-back of the last adjustDistortion's per-point scratch for the de-skew tests: copies min(capacity, n) entries of
+ * rel_time (float), t = scan_time + rel_time (double), imu_ptr_front_ after the walk (ring index) and the skip flag
+ * (1: the point was `continue`d), and sets *n to the number of points; k_first is the first index that set half_passed
+ * (n if none), rounds the passes of the skipped-set fix point (0 when the clock stepped back and the walk ran
+ * literally). *n is 0 when no kernel ran (an empty cloud, or imu_ptr_last_ <= 0). Any output pointer may be NULL.    */
+int b200sm_imu_get_trace(b200sm_t s, size_t capacity, size_t* n, float* rel_time, double* t, int* front,
+                         unsigned char* skip, int* k_first, int* rounds);
 
 /* A backend in its OWN process gets the submaps as lidarslam_msgs/SubMap (voxel-filtered cloud in the sensor frame, pose,
  * travelled distance; gbs.cpp:91-101): append one to the session (uploaded once, then device-resident like the

@@ -41,7 +41,7 @@ SYMBOLS = [
     "b200sm_set_scan", "b200sm_update_map", "b200sm_receive_cloud", "b200sm_num_submaps", "b200sm_get_targeted",
     "b200sm_get_submap", "b200sm_get_filtered_scan", "b200sm_get_stats", "b200sm_search_loop", "b200sm_search_loop_all", "b200sm_import_submap",
     "b200sm_imu_set_scan_period", "b200sm_imu_push", "b200sm_deskew_next_scan", "b200sm_imu_adjust_distortion",
-    "b200sm_imu_get_state", "b200sm_imu_get_sample", "b200sm_pose_adjust", "b200sm_assemble_map",
+    "b200sm_imu_get_state", "b200sm_imu_get_sample", "b200sm_imu_get_trace", "b200sm_pose_adjust", "b200sm_assemble_map",
     "b200sm_save_map_pcd_ascii", "b200reg_encode_pcd_ascii", "b200sm_set_sensor_transform", "b200sm_odom_next_scan",
     # include/b200comm.h
     "b200comm_unique_id", "b200comm_create", "b200comm_destroy", "b200comm_all_gather_rows", "b200comm_rank", "b200comm_last_error",
@@ -187,6 +187,7 @@ def lib() -> C.CDLL:
     L.b200sm_imu_adjust_distortion.argtypes = [vp, vp, sz, sz, C.c_long, d]
     L.b200sm_imu_get_state.argtypes = [vp, C.POINTER(i), C.POINTER(i), C.POINTER(i)]
     L.b200sm_imu_get_sample.argtypes = [vp, i, C.POINTER(d), vp, vp, vp]
+    L.b200sm_imu_get_trace.argtypes = [vp, sz, C.POINTER(sz), vp, vp, vp, vp, C.POINTER(i), C.POINTER(i)]
     L.b200sm_pose_adjust.argtypes = [vp, i, vp, i, i, vp, C.POINTER(SmPoseAdjustResult)]
     L.b200sm_assemble_map.argtypes = [vp, vp, vp, sz, C.POINTER(sz), vp]
     L.b200sm_save_map_pcd_ascii.argtypes = [vp, vp, C.c_char_p, C.POINTER(sz), C.POINTER(sz)]

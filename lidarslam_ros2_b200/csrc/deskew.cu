@@ -7,7 +7,10 @@
 //   * half_passed is set by the FIRST point whose pre-half-turn azimuth is more than pi past the start  -> atomicMin;
 //   * the carried pointer is the running maximum, over the previous NON-skipped points, of an independent per-point
 //     lower bound into the ring (first sample later than the point's time stamp)  -> exclusive prefix-max scan, repeated
-//     until the set of skipped points is stable (one pass when the IMU covers the scan);
+//     until the set of skipped points is stable (one pass when the IMU covers the scan). The lower bound uses the
+//     walk's own test `t < time`, so a NaN time (a NaN ray) carries the newest sample as in the reference. The form is
+//     exact only while the stamps of the ring window never decrease; when the IMU clock steps back inside the window
+//     (checked on the host) one thread of deskew_scan runs the walk literally instead;
 //   * interpolation of roll/pitch/yaw/shift/velocity and the rigid correction are independent per point.
 // Kernels: deskew_orient (azimuth, first-index reduction) -> deskew_time (relative time, ring lower bound) ->
 // deskew_scan (one CTA: prefix-max fix point, carried pointers, start pose) -> deskew_apply (per-point correction).
@@ -28,7 +31,8 @@ constexpr double PI_D = 3.14159265358979323846;  // M_PI
 struct DeskewParams {
   float start_ori, end_ori, ori_diff;
   double scan_period, scan_time;
-  int base, span;  // ring positions 0..span map to ring indices (base + pos) % IMU_QUE, chronological
+  int base, span;  // ring positions 0..span map to ring indices (base + pos) % IMU_QUE, in the walk's order
+  int monotone;    // the stamps at positions 0..span never decrease (the binary search and the fix point are exact)
 };
 
 struct DeskewShared {  // small device-side block shared by the kernels of one call
@@ -36,9 +40,11 @@ struct DeskewShared {  // small device-side block shared by the kernels of one c
   int ptr_front_pos;    // ring position of imu_ptr_front_ after the last point
   int ptr_iter_pos;     // ring position carried past the last non-skipped point (-1: none)
   int ok0;              // point 0 was not skipped: the start pose below is valid
+  int rounds;           // passes of the fix point (0: the literal walk ran instead)
   float r_s_i[9];       // r_c.inverse() of the first point (row-major)
   float shift0[3], velo0[3];
 };
+constexpr int DESKEW_SHARED_INTS = 5;  // the leading int fields, initialised and read back by the host
 
 __device__ __forceinline__ float neg_atan2_f(float y, float x) { return -(float)atan2((double)y, (double)x); }
 
@@ -78,11 +84,12 @@ __global__ void deskew_time_kernel(int n, DeskewParams P, const ImuSample* __res
   // float rel_time = (ori_h - start_ori) / ori_diff * scan_period_   (:149): float quotient, double product, float store
   const float rel = (float)((double)__fdiv_rn(__fsub_rn(oh, P.start_ori), P.ori_diff) * P.scan_period);
   const double t = P.scan_time + (double)rel;
-  // first ring position whose stamp is later than t (the walk :153-158 stops there), clamped to the newest sample
+  // first ring position whose stamp is later than t (the walk :153-158 stops there), clamped to the newest sample. The
+  // walk's own test `t < time` decides, so a NaN t (a NaN ray) runs to the newest sample like in the reference.
   int lo = 0, hi = P.span + 1;
   while (lo < hi) {
     const int mid = (lo + hi) >> 1;
-    if (times[mid] <= t) lo = mid + 1;
+    if (!(t < times[mid])) lo = mid + 1;
     else hi = mid;
   }
   rel_out[i] = rel;
@@ -151,6 +158,7 @@ __device__ __forceinline__ void rot_zyx(float roll, float pitch, float yaw, floa
 // One CTA: fix point of   skipped_i = |t_i - time[max(carried_i, lb_i)]| > scan_period,
 //                         carried_i = max(0, max_{j < i, !skipped_j} lb_j)                    (exclusive prefix max)
 // Thread q owns the contiguous chunk [q * per, (q + 1) * per). Converges in one pass when the IMU covers the scan.
+// Stamps that step back (P.monotone == 0): thread 0 walks the points literally instead and no fix point runs.
 constexpr int SCAN_THREADS = 1024;
 __global__ void __launch_bounds__(SCAN_THREADS) deskew_scan_kernel(int n, DeskewParams P, const ImuSample* __restrict__ ring,
                                                                    const double* __restrict__ t, const int* __restrict__ lb,
@@ -166,8 +174,26 @@ __global__ void __launch_bounds__(SCAN_THREADS) deskew_scan_kernel(int n, Deskew
   const int c0 = min(n, tid * per), c1 = min(n, c0 + per);
   for (int i = c0; i < c1; i++) skip2[i] = 0;
   __syncthreads();
-  int cur = 0;
-  for (int iter = 0; iter <= n; iter++) {
+  int cur = 0, rounds = 0;
+  if (!P.monotone) {
+    // The stamps step back inside the window (a replayed bag, a restamping driver): the lower bounds of deskew_time do
+    // not describe the walk, so thread 0 runs it literally (:152-158, :223) from the carried pointer, position 0.
+    if (tid == 0) {
+      int carried_pos = 0;
+      for (int i = 0; i < n; i++) {
+        const double ti = t[i];
+        int fp = carried_pos;
+        while (fp != P.span && !(ti < times[fp])) fp++;
+        const bool s = fabs(ti - times[fp]) > P.scan_period;
+        front[i] = fp;
+        skip2[i] = s ? 1 : 0;
+        if (!s) carried_pos = fp;
+      }
+    }
+    __syncthreads();
+  }
+  for (int iter = 0; P.monotone && iter <= n; iter++) {
+    rounds++;
     const unsigned char* sk = skip2 + (size_t)cur * n;
     unsigned char* sk_new = skip2 + (size_t)(cur ^ 1) * n;
     if (tid == 0) changed = 0;
@@ -230,6 +256,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) deskew_scan_kernel(int n, Deskew
     sh->ptr_front_pos = front[n - 1];            // assigned before the skip test, for every point (:152-158)
     sh->ptr_iter_pos = best >= 0 ? front[best] : -1;  // carried only past non-skipped points (:223)
     sh->ok0 = sk[0] ? 0 : 1;
+    sh->rounds = rounds;
     if (!sk[0]) {
       float rpy[3], shift[3], velo[3], R[9];
       imu_interp(ring, (P.base + front[0]) % IMU_QUE, t[0], rpy, shift, velo);
@@ -310,6 +337,7 @@ void ImuDeskew::get_imu(const float* w, const float* acc_in, const float* q, dou
 void ImuDeskew::adjust_distortion(float4* d_cloud, size_t n_sz, const float* first_xy, const float* last_xy, double scan_time,
                                   cudaStream_t s) {
   const int n = (int)n_sz;
+  trace_n = 0;
   if (n == 0) return;
   if (ptr_last <= 0) {  // `if (imu_ptr_last_ > 0)` (:151) is false: no point is touched; the carry at :223 still runs
     ptr_last_iter = ptr_front;
@@ -345,14 +373,17 @@ void ImuDeskew::adjust_distortion(float4* d_cloud, size_t n_sz, const float* fir
     }
     e.pad = 0.f;
   }
+  P.monotone = 1;  // the walk's order; NaN stamps also take the literal walk
+  for (int j = 0; j < P.span; j++)
+    if (!(time[(P.base + j + 1) % IMU_QUE] >= time[(P.base + j) % IMU_QUE])) P.monotone = 0;
   ImuSample* d_ring = reinterpret_cast<ImuSample*>(d_small.ptr);
   DeskewShared* d_sh = reinterpret_cast<DeskewShared*>(d_small.ptr + ring_bytes);
   DeskewShared init{};
   init.k_first = n;
   init.ptr_iter_pos = -1;
-  std::memcpy(h_out.ptr + 8, &init, sizeof(int) * 4);
+  std::memcpy(h_out.ptr + 8, &init, sizeof(int) * DESKEW_SHARED_INTS);
   B200_CUDA(cudaMemcpyAsync(d_ring, h_ring, ring_bytes, cudaMemcpyHostToDevice, s));
-  B200_CUDA(cudaMemcpyAsync(d_sh, h_out.ptr + 8, sizeof(int) * 4, cudaMemcpyHostToDevice, s));
+  B200_CUDA(cudaMemcpyAsync(d_sh, h_out.ptr + 8, sizeof(int) * DESKEW_SHARED_INTS, cudaMemcpyHostToDevice, s));
   const int blocks = (n + 255) / 256;
   deskew_orient_kernel<<<blocks, 256, 0, s>>>(d_cloud, n, P, d_ori.ptr, d_a.ptr, d_sh);
   deskew_time_kernel<<<blocks, 256, 0, s>>>(n, P, d_ring, d_ori.ptr, d_a.ptr, d_sh, d_rel.ptr, d_t.ptr, d_lb.ptr);
@@ -360,11 +391,32 @@ void ImuDeskew::adjust_distortion(float4* d_cloud, size_t n_sz, const float* fir
   deskew_apply_kernel<<<blocks, 256, 0, s>>>(d_cloud, n, P, d_ring, d_t.ptr, d_rel.ptr, d_front.ptr, d_skip.ptr, d_sh);
   B200_CUDA(cudaGetLastError());
   launches += 4;
-  B200_CUDA(cudaMemcpyAsync(h_out.ptr, d_sh, sizeof(int) * 4, cudaMemcpyDeviceToHost, s));
+  B200_CUDA(cudaMemcpyAsync(h_out.ptr, d_sh, sizeof(int) * DESKEW_SHARED_INTS, cudaMemcpyDeviceToHost, s));
   B200_CUDA(cudaStreamSynchronize(s));
   // imu_ptr_front_ / imu_ptr_last_iter_ after the loop
   ptr_front = (P.base + h_out.ptr[1]) % IMU_QUE;
   if (h_out.ptr[2] >= 0) ptr_last_iter = (P.base + h_out.ptr[2]) % IMU_QUE;
+  trace_n = n;
+  trace_base = P.base;
+  trace_k_first = h_out.ptr[0];
+  trace_rounds = h_out.ptr[4];
+}
+
+// ---- read-back of the last adjust_distortion's per-point scratch (tests) -----------------------------------------
+size_t ImuDeskew::get_trace(size_t capacity, float* rel_time, double* t, int* front, unsigned char* skip, int* k_first,
+                            int* rounds, cudaStream_t s) {
+  const size_t n = trace_n, m = capacity < n ? capacity : n;
+  if (k_first) *k_first = trace_k_first;
+  if (rounds) *rounds = trace_rounds;
+  if (m == 0) return n;
+  if (rel_time) B200_CUDA(cudaMemcpyAsync(rel_time, d_rel.ptr, m * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if (t) B200_CUDA(cudaMemcpyAsync(t, d_t.ptr, m * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (front) B200_CUDA(cudaMemcpyAsync(front, d_front.ptr, m * sizeof(int), cudaMemcpyDeviceToHost, s));
+  if (skip) B200_CUDA(cudaMemcpyAsync(skip, d_skip.ptr, m, cudaMemcpyDeviceToHost, s));  // the stable half
+  B200_CUDA(cudaStreamSynchronize(s));
+  if (front)
+    for (size_t i = 0; i < m; i++) front[i] = (trace_base + front[i]) % IMU_QUE;  // ring positions -> ring indices
+  return n;
 }
 
 }  // namespace b200

@@ -34,8 +34,14 @@ class ImuDeskew {
   // first_xy / last_xy: x, y of the first and the last point (the host has them: it uploaded the scan).
   // Synchronises the stream (the carried ring pointers come back to the host).
   void adjust_distortion(float4* d_cloud, size_t n, const float* first_xy, const float* last_xy, double scan_time, cudaStream_t s);
+  // The last adjust_distortion's per-point scratch: relative time, time stamp, imu_ptr_front_ (ring index) and the
+  // stable skip flag of min(capacity, n) points, the half-turn index and the fix-point passes. Returns n (0 when the
+  // kernels did not run). Synchronises the stream.
+  size_t get_trace(size_t capacity, float* rel_time, double* t, int* front, unsigned char* skip, int* k_first, int* rounds,
+                   cudaStream_t s);
 
  private:
+  int trace_n = 0, trace_base = 0, trace_k_first = 0, trace_rounds = 0;
   DeviceBuffer<float> d_ori, d_a, d_rel;
   DeviceBuffer<double> d_t;
   DeviceBuffer<int> d_lb, d_front;

@@ -1073,4 +1073,13 @@ int b200sm_imu_get_sample(b200sm_t s, int index, double* stamp, float* rpy3, flo
   return B200REG_OK;
 }
 
+int b200sm_imu_get_trace(b200sm_t s, size_t capacity, size_t* n, float* rel_time, double* t, int* front, unsigned char* skip,
+                         int* k_first, int* rounds) {
+  if (!s || !n) return B200REG_ERR_ARG;
+  return sm_guarded(s, [&]() {
+    *n = s->imu.get_trace(capacity, rel_time, t, front, skip, k_first, rounds, s->stream);
+    return (int)B200REG_OK;
+  });
+}
+
 }  // extern "C"

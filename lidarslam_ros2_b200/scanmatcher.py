@@ -313,3 +313,19 @@ class LidarUndistortion:
         rpy, sh, ve = (np.zeros(3, dtype=np.float32) for _ in range(3))
         self._check(self._lib.b200sm_imu_get_sample(self._s, int(index), C.byref(t), rpy.ctypes.data, sh.ctypes.data, ve.ctypes.data))
         return t.value, rpy, sh, ve
+
+    def trace(self) -> dict:
+        """The last adjustDistortion's per-point scratch (b200sm_imu_get_trace): rel_time (float32), t (float64), front
+        (ring index after the walk), skip (bool), k_first (first index that set half_passed, n if none) and rounds
+        (passes of the skipped-set fix point, 0 after a literal walk). n = 0 when no kernel ran."""
+        C = self._C
+        n, k, r = C.c_size_t(0), C.c_int(0), C.c_int(0)
+        self._check(self._lib.b200sm_imu_get_trace(self._s, 0, C.byref(n), None, None, None, None, C.byref(k), C.byref(r)))
+        m = n.value
+        rel, t = np.zeros(m, dtype=np.float32), np.zeros(m, dtype=np.float64)
+        front, skip = np.zeros(m, dtype=np.int32), np.zeros(m, dtype=np.uint8)
+        if m:
+            self._check(self._lib.b200sm_imu_get_trace(self._s, m, C.byref(n), rel.ctypes.data, t.ctypes.data,
+                                                       front.ctypes.data, skip.ctypes.data, None, None))
+        return {"n": m, "rel_time": rel, "t": t, "front": front, "skip": skip.astype(bool), "k_first": k.value,
+                "rounds": r.value}

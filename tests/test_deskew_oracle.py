@@ -69,3 +69,19 @@ def test_no_imu_means_no_change():
     cloud = _spinning_scan(400)
     np.testing.assert_array_equal(u.adjust_distortion(cloud, 1.0), cloud)
     np.testing.assert_array_equal(u.adjust_distortion_parallel(cloud, 1.0), cloud)
+
+
+@pytest.mark.parametrize("scan_time_offset", [0.20, 0.95])  # mid coverage, running off the end
+def test_parallel_form_equals_sequential_with_nan_ray(scan_time_offset):
+    """A NaN ray (fromROSMsg of an organised cloud keeps them): the walk runs to the newest sample for it and carries
+    that pointer; the parallel form's lower bound (searchsorted sorts NaN last) does the same."""
+    u = deskew.LidarUndistortion(scan_period=0.1)
+    _imu_stream(u, t0=100.0, n=100)
+    v = copy.deepcopy(u)
+    cloud = _spinning_scan()
+    cloud[700, :3] = np.nan
+    for rep in range(2):
+        a = u.adjust_distortion(cloud, 100.0 + scan_time_offset + 0.1 * rep)
+        b = v.adjust_distortion_parallel(cloud, 100.0 + scan_time_offset + 0.1 * rep)
+        np.testing.assert_array_equal(a, b)
+        assert (u.ptr_front, u.ptr_last_iter) == (v.ptr_front, v.ptr_last_iter)
