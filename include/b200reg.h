@@ -44,7 +44,8 @@ enum b200reg_status {
   B200REG_ERR_CUDA = -4,      /* CUDA runtime error, or no device                                      */
   B200REG_ERR_TIMEOUT = -5,   /* device-side watchdog fired inside the persistent solver               */
   B200REG_ERR_GRID = -6,      /* voxel grid would overflow int32 (voxel_grid_covariance_omp_impl.hpp:79) */
-  B200REG_ERR_IO = -7         /* a file could not be opened or written                                 */
+  B200REG_ERR_IO = -7,        /* a file could not be opened, read or written                           */
+  B200REG_ERR_FORMAT = -8     /* a PCD file the reader does not accept (b200reg_load_pcd)              */
 };
 
 /* ---- lifetime --------------------------------------------------------------------------------------- */
@@ -434,6 +435,40 @@ int b200sm_save_map_pcd_ascii(b200sm_t s, const double* poses_colmajor16, const 
  * is not a multiple of 4. */
 int b200reg_encode_pcd_ascii(int device, const float* base, size_t n, size_t stride_bytes, long intensity_offset_bytes,
                              char* out, size_t capacity, size_t* n_bytes);
+
+/* ---- pcl::io::loadPCDFile (apps/align.cpp:54-61; a localisation or resume node reading the map.pcd saved above) ---
+ * The header is parsed on the host, PCD v0.7 as PCL reads it: '#' comment lines, VERSION, FIELDS, SIZE, TYPE, COUNT,
+ * WIDTH, HEIGHT, VIEWPOINT, POINTS, DATA (COUNT may be absent: 1 each; WIDTH * HEIGHT must equal POINTS). Organised clouds
+ * (HEIGHT > 1) come out flat, WIDTH * HEIGHT points. Fields x, y, z are required and intensity is optional, each TYPE F,
+ * SIZE 4, COUNT 1; every other field is skipped whatever its type and count. Output rows are float4 (x, y, z, intensity),
+ * intensity 0 when the file has none (the PointXYZI default).
+ * DATA ascii, as PCDReader::readBodyASCII / copyStringValue<float> of PCL 1.12: lines from getline, empty lines skipped,
+ * tokens split on ' ', '\t' and '\r' with runs of separators compressed; a token equal to "nan" in any case is quiet_NaN,
+ * every other token reads as `istringstream >> float` in the classic locale (glibc strtof, correctly rounded, subnormals,
+ * overflow to +-inf), and the signed nan and inf / infinity spellings take the value of PCL's atof fallback. Reading
+ * stops after POINTS points (the file is read at most one piece further). The text is parsed on the device, piece by piece (B200REG_PCD_LOAD_PIECE_BYTES of the body at
+ * a time, each ending at its last '\n', read into two pinned buffers in turn while the device parses the previous one).
+ * B200REG_ERR_FORMAT: a POINTS the body cannot hold (checked against the file size before anything is allocated), fewer
+ * data lines than POINTS, a line whose token count is not the sum of COUNT (a line of
+ * separators only included), an x / y / z / intensity token outside the grammar [+-](digits[.[digits]] | .digits)
+ * [(e|E)[+-]digits] | [+-](nan | inf | infinity), a line longer than a piece before the POINTS-th line. Deliberate divergences from PCL: PCL takes
+ * atof's value of a malformed token silently, and its handling of a bad token count differs between releases.
+ * DATA binary: POINTS records of sum(SIZE * COUNT) bytes, unpacked on the device by the upload path of set_input_*; x, y,
+ * z must be consecutive, intensity (if any) after x, the record size and the offsets multiples of 4; a body shorter than
+ * the header says is B200REG_ERR_FORMAT. DATA binary_compressed (one sequential LZF block) is B200REG_ERR_FORMAT. */
+#define B200REG_PCD_LOAD_PIECE_BYTES ((size_t)64 << 20)
+/* The file's points into out_xyzi (4 floats per point): *n_points = POINTS, min(POINTS, capacity) rows copied; capacity 0
+ * is a size query from the header alone. B200REG_ERR_IO when the file cannot be opened or read. */
+int b200reg_load_pcd(int device, const char* path, float* out_xyzi, size_t capacity, size_t* n_points);
+/* setInputTarget(cloud) of a loadPCDFile(path, cloud): the file is parsed into device scratch and handed over device to
+ * device as b200reg_set_input_target_device does; no point of it exists as floats on the host, and the scratch copy of
+ * the cloud is freed after the hand-over. On B200REG_ERR_IO, B200REG_ERR_FORMAT, B200REG_ERR_ARG (no points) and, for
+ * NDT, B200REG_ERR_GRID (the new map's voxel grid would overflow int32 at the current resolution; checked before the
+ * hand-over) the handle's previous target is unchanged, and b200reg_last_error names the reason (and the line of the
+ * file, for a bad line). After B200REG_ERR_CUDA the handle has no valid target. The handle keeps the reader's fixed-size
+ * buffers for later calls: two pinned pieces of B200REG_PCD_LOAD_PIECE_BYTES and one device piece; a binary file also
+ * keeps a pinned and a device buffer of its body's size. n_points (may be NULL) = points of the new target. */
+int b200reg_set_input_target_pcd(b200reg_t h, const char* path, size_t* n_points);
 
 typedef struct b200sm_stats {
   size_t n_scan, n_filtered, n_targeted, n_submaps;

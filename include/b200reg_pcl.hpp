@@ -12,6 +12,7 @@
 //    with identical method names, which is what tests/cpp/adapter_smoke.cpp exercises.
 // Header-only; link with -lb200reg. Matrices are column-major float[16] == Eigen::Matrix4f::data().
 #pragma once
+#include <algorithm>
 #include <array>
 #include <cfloat>
 #include <cstdio>
@@ -90,6 +91,13 @@ class Registration {
     if (rc != B200REG_OK && rc != B200REG_ERR_NO_TARGET && rc != B200REG_ERR_NO_SOURCE) check(rc);
     output.points.resize(n_source_);
     if (rc == B200REG_OK && n_source_) check(b200reg_get_aligned(h_.get(), &output.points[0].x, sizeof(PointXYZI)));
+  }
+  // setInputTarget(cloud) of loadPCDFile(path, cloud), the file parsed on the device (b200reg_set_input_target_pcd);
+  // throws on a file the reader refuses, keeping the previous target. Returns the number of points.
+  size_t setInputTargetPCD(const std::string& path) {
+    size_t n = 0;
+    check(b200reg_set_input_target_pcd(h_.get(), path.c_str(), &n));
+    return n;
   }
   Matrix4f getFinalTransformation() const { return final_; }
   bool hasConverged() const {
@@ -181,6 +189,17 @@ class RegistrationBase : public pcl::Registration<PointSource, PointTarget> {
       return;
     }
     source_ok_ = report(b200reg_set_input_source(h_.get(), &cloud->points[0].x, cloud->size(), sizeof(PointSource)), "setInputSource");
+  }
+  // setInputTarget(cloud) of loadPCDFile(path, cloud) with the file parsed on the device (b200reg_set_input_target_pcd):
+  // no host copy of the map exists, so PCL's own target_ is an empty cloud (align() only needs it to be set). On a file
+  // the reader refuses the error is reported, the previous target stays, and 0 is returned.
+  size_t setInputTargetPCD(const std::string& path) {
+    size_t n = 0;
+    if (!report(b200reg_set_input_target_pcd(h_.get(), path.c_str(), &n), "setInputTargetPCD")) return 0;
+    this->target_.reset(new pcl::PointCloud<PointTarget>());
+    this->target_cloud_updated_ = false;
+    target_ok_ = true;
+    return n;
   }
   void setKeepHostSearchTree(bool keep) { keep_host_tree_ = keep; }
   // align() fills `output` with the transformed source (a device-to-host copy of the whole scan per call). Both nodes
@@ -280,6 +299,31 @@ class GeneralizedIterativeClosestPoint : public RegistrationBase<PointSource, Po
 };
 
 #endif  // B200REG_WITH_PCL
+
+// pcl::io::loadPCDFile(path, cloud) for a PointXYZI cloud, the text parsed on the device (b200reg_load_pcd): x, y, z and
+// intensity of every point, WIDTH * HEIGHT points as one flat row. Returns 0, or the negative B200REG_ERR_* code (PCL: -1).
+template <typename Cloud>
+int loadPCDFile(const std::string& path, Cloud& cloud, int device = 0) {
+  size_t n = 0;
+  int rc = b200reg_load_pcd(device, path.c_str(), nullptr, 0, &n);
+  if (rc != B200REG_OK) return rc;
+  std::vector<float> xyzi(4 * n);
+  const size_t capacity = n;
+  if (n && (rc = b200reg_load_pcd(device, path.c_str(), xyzi.data(), capacity, &n)) != B200REG_OK) return rc;
+  n = std::min(n, capacity);  // the file may have changed between the two calls
+  cloud.points.resize(n);
+  for (size_t i = 0; i < n; i++) {
+    cloud.points[i].x = xyzi[4 * i];
+    cloud.points[i].y = xyzi[4 * i + 1];
+    cloud.points[i].z = xyzi[4 * i + 2];
+    cloud.points[i].intensity = xyzi[4 * i + 3];
+  }
+#ifdef B200REG_WITH_PCL
+  cloud.width = static_cast<decltype(cloud.width)>(n);
+  cloud.height = 1;
+#endif
+  return B200REG_OK;
+}
 
 // ---- frontend session: device-resident map maintenance (b200sm_*, include/b200reg.h) -------------------------------
 // What ScanMatcherComponent keeps per node instead of targeted_cloud_ / map_array_msg_.submaps[i].cloud on the host:

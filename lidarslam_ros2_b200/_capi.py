@@ -10,7 +10,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 REPO_ROOT = os.path.dirname(_HERE)
 LIB_PATH = os.path.join(_HERE, "csrc", os.environ.get("B200REG_LIB_VARIANT", "libb200reg.so"))  # variant: developer A/B builds
 
-OK, ERR_ARG, ERR_NO_TARGET, ERR_NO_SOURCE, ERR_CUDA, ERR_TIMEOUT, ERR_GRID, ERR_IO = 0, -1, -2, -3, -4, -5, -6, -7
+OK, ERR_ARG, ERR_NO_TARGET, ERR_NO_SOURCE, ERR_CUDA, ERR_TIMEOUT, ERR_GRID, ERR_IO, ERR_FORMAT = 0, -1, -2, -3, -4, -5, -6, -7, -8
+PCD_LOAD_PIECE_BYTES = 64 << 20  # B200REG_PCD_LOAD_PIECE_BYTES
 NDT, GICP = 0, 1
 KDTREE, DIRECT26, DIRECT7, DIRECT1 = 0, 1, 2, 3
 
@@ -43,6 +44,7 @@ SYMBOLS = [
     "b200sm_imu_set_scan_period", "b200sm_imu_push", "b200sm_deskew_next_scan", "b200sm_imu_adjust_distortion",
     "b200sm_imu_get_state", "b200sm_imu_get_sample", "b200sm_imu_get_trace", "b200sm_pose_adjust", "b200sm_assemble_map",
     "b200sm_save_map_pcd_ascii", "b200reg_encode_pcd_ascii", "b200sm_set_sensor_transform", "b200sm_odom_next_scan",
+    "b200reg_load_pcd", "b200reg_set_input_target_pcd",
     # include/b200comm.h
     "b200comm_unique_id", "b200comm_create", "b200comm_destroy", "b200comm_all_gather_rows", "b200comm_rank", "b200comm_last_error",
     "b200comm_board_create", "b200comm_board_destroy", "b200comm_board_info",
@@ -193,6 +195,8 @@ def lib() -> C.CDLL:
     L.b200sm_save_map_pcd_ascii.argtypes = [vp, vp, C.c_char_p, C.POINTER(sz), C.POINTER(sz)]
     L.b200reg_encode_pcd_ascii.argtypes = [i, vp, sz, sz, C.c_long, vp, sz, C.POINTER(sz)]
     L.b200sm_set_sensor_transform.argtypes = [vp, vp, vp]
+    L.b200reg_load_pcd.argtypes = [i, C.c_char_p, vp, sz, C.POINTER(sz)]
+    L.b200reg_set_input_target_pcd.argtypes = [vp, C.c_char_p, C.POINTER(sz)]
     L.b200sm_odom_next_scan.argtypes = [vp, vp, vp]
     L.b200comm_unique_id.argtypes = [vp]
     L.b200comm_create.argtypes = [vp, i, i, i, C.POINTER(vp)]

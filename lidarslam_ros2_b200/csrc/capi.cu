@@ -61,6 +61,8 @@ struct b200reg_engine {
   DeviceBuffer<double> scratch_d;   // >= 64 doubles
   DeviceBuffer<float> scratch_f;    // >= 16 floats
   DeviceBuffer<float4> query_buf;
+  PcdLoader pcd;                   // b200reg_set_input_target_pcd: the file is parsed into pcd_points, then handed over
+  DeviceBuffer<float4> pcd_points;
 
   // results of the last align (row-major)
   float final_T[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
@@ -482,6 +484,32 @@ int b200reg_set_input_target_device(b200reg_t h, const void* dev, size_t n) {
 }
 int b200reg_set_input_source_device(b200reg_t h, const void* dev, size_t n) {
   return guarded(h, [&]() { return set_cloud(h, false, nullptr, n, 16, dev); });
+}
+int b200reg_set_input_target_pcd(b200reg_t h, const char* path, size_t* n_points) {
+  if (!h || !path) return B200REG_ERR_ARG;
+  return guarded(h, [&]() {
+    size_t n = 0;
+    std::string why;
+    const int rc = h->pcd.load(path, h->pcd_points, &n, why, h->stream);  // the current target is not touched
+    if (rc != B200REG_OK) return fail(h, rc, (std::string("setInputTargetPCD: ") + path + ": " + why).c_str());
+    struct Release {  // the map-sized copy is not kept once it has been handed over
+      DeviceBuffer<float4>& b;
+      ~Release() { b.release(); }
+    } release{h->pcd_points};
+    if (n == 0) return fail(h, B200REG_ERR_ARG, "setInputTargetPCD: the file has no points (empty input cloud ignored)");
+    if (h->kind == B200REG_NDT) {  // a map whose voxel grid would overflow int32 does not replace the current target
+      h->scratch_bounds.ensure(8);
+      const Bounds b = cloud_bounds(h->pcd_points.ptr, n, h->scratch_bounds.ptr, h->stream);
+      h->other_launches += 1;
+      GridGeom g{};
+      if (b.any && !make_grid_geom(b, h->ndt.resolution, g))
+        return fail(h, B200REG_ERR_GRID, (std::string("setInputTargetPCD: ") + path +
+                                          ": the voxel grid would overflow int32 at this resolution; the target is unchanged").c_str());
+    }
+    const int r = set_cloud(h, true, nullptr, n, 16, h->pcd_points.ptr);
+    if (r == B200REG_OK && n_points) *n_points = n;
+    return r;
+  });
 }
 // Library-internal (not in include/b200reg.h): the frontend session hands over its voxel-filtered scan WITHOUT a copy — the
 // buffer stays valid and untouched until the session's next frame, and the session has synchronised its own stream.

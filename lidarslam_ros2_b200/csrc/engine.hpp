@@ -3,6 +3,7 @@
 #include <algorithm>
 #include <cuda_runtime.h>
 
+#include <cstdio>
 #include <cstring>
 #include <mutex>
 #include <string>
@@ -11,6 +12,7 @@
 #include "../../include/b200reg.h"
 #include "common.cuh"
 #include "ndt_math.cuh"
+#include "pcd_parse.cuh"
 
 namespace b200 {
 
@@ -366,6 +368,23 @@ struct PcdEncoder {
   void measure(const float4* pts, size_t n, cudaStream_t s);
   // pass 2: the text of chunk c into `text` (enqueue only; the offsets are those of the last measure() of the same cloud)
   void encode_chunk(const float4* pts, size_t n, size_t c, cudaStream_t s);
+};
+
+// ---- PCD file -> float4 (x, y, z, intensity) on the device (pcd_load.cu; the contract is b200reg_load_pcd's) ---------
+// the header of an open file, read up to and including its DATA line: B200REG_OK, B200REG_ERR_IO or B200REG_ERR_FORMAT
+int read_pcd_header(FILE* fp, PcdHeader& h, std::string& err);
+struct PcdLoader {
+  PinnedBuffer<char> pieces[2];            // the ASCII body, B200REG_PCD_LOAD_PIECE_BYTES at a time
+  DeviceBuffer<char> text;                 // one piece, plus the parse kernel's staging slack
+  DeviceBuffer<unsigned> counts, scan_tmp; // non-empty lines per tile, scanned in place into tile offsets
+  DeviceBuffer<unsigned long long> state;  // [0] non-empty lines so far, [1] first failing line: file offset << 2 | kind
+  PinnedBuffer<unsigned long long> h_state;
+  PinnedBuffer<unsigned char> body;        // a binary body, read whole
+  CloudUploader uploader;
+  int launches = 0;
+  // The points of `path` into dst (grown to POINTS rows); *n = POINTS. B200REG_OK, B200REG_ERR_IO or B200REG_ERR_FORMAT
+  // (reason in err); CUDA errors throw. The stream is synchronised on return.
+  int load(const char* path, DeviceBuffer<float4>& dst, size_t* n, std::string& err, cudaStream_t s);
 };
 
 }  // namespace b200

@@ -65,4 +65,27 @@ __device__ __forceinline__ void block_bounds_merge(float (&mn)[3], float (&mx)[3
   }
 }
 
+// exclusive prefix of v over the block's kThreads threads; total = the block's sum (the ASCII PCD encode and parse tiles)
+template <int kThreads>
+__device__ __forceinline__ unsigned block_exclusive_scan(unsigned v, unsigned& total) {
+  __shared__ unsigned warp_tot[kThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned incl = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const unsigned t = __shfl_up_sync(0xffffffffu, incl, d);
+    if (lane >= d) incl += t;
+  }
+  if (lane == 31) warp_tot[warp] = incl;
+  __syncthreads();
+  unsigned off = 0, tot = 0;
+#pragma unroll
+  for (int w = 0; w < kThreads / 32; w++) {
+    if (w < warp) off += warp_tot[w];
+    tot += warp_tot[w];
+  }
+  total = tot;
+  return off + incl - v;
+}
+
 }  // namespace b200

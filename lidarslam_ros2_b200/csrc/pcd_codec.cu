@@ -10,6 +10,7 @@
 #include <string>
 
 #include "engine.hpp"
+#include "grid_index.cuh"
 #include "pcd_format.cuh"
 
 namespace b200 {
@@ -20,28 +21,6 @@ constexpr int PCD_TILE = 256;  // points (= threads) per tile
 constexpr size_t PCD_TILES_PER_CHUNK = PCD_CHUNK_POINTS / PCD_TILE;
 static_assert(PCD_CHUNK_POINTS % PCD_TILE == 0, "a chunk is whole tiles");
 static_assert(PCD_CHUNK_POINTS * PCD_LINE_MAX_CHARS < ((size_t)1 << 32), "offsets inside a chunk are unsigned");
-
-// exclusive prefix of v over the block's PCD_TILE threads; total = the block's sum
-__device__ __forceinline__ unsigned block_exclusive_scan(unsigned v, unsigned& total) {
-  __shared__ unsigned warp_tot[PCD_TILE / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  unsigned incl = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const unsigned t = __shfl_up_sync(0xffffffffu, incl, d);
-    if (lane >= d) incl += t;
-  }
-  if (lane == 31) warp_tot[warp] = incl;
-  __syncthreads();
-  unsigned off = 0, tot = 0;
-#pragma unroll
-  for (int w = 0; w < PCD_TILE / 32; w++) {
-    if (w < warp) off += warp_tot[w];
-    tot += warp_tot[w];
-  }
-  total = tot;
-  return off + incl - v;
-}
 
 // counts of chunk c start at c * (PCD_TILES_PER_CHUNK + 1): each chunk's scan leaves its total right after its tiles
 __global__ void __launch_bounds__(PCD_TILE) pcd_measure_kernel(const float4* __restrict__ pts, size_t n, unsigned* __restrict__ counts) {
@@ -54,7 +33,7 @@ __global__ void __launch_bounds__(PCD_TILE) pcd_measure_kernel(const float4* __r
     len = (unsigned)pcd_format_line(p.x, p.y, p.z, p.w, line);
   }
   unsigned total;
-  block_exclusive_scan(len, total);
+  block_exclusive_scan<PCD_TILE>(len, total);
   if (threadIdx.x == 0) counts[(tile / PCD_TILES_PER_CHUNK) * (PCD_TILES_PER_CHUNK + 1) + tile % PCD_TILES_PER_CHUNK] = total;
 }
 
@@ -70,7 +49,7 @@ __global__ void __launch_bounds__(PCD_TILE) pcd_encode_kernel(const float4* __re
     len = (unsigned)pcd_format_line(p.x, p.y, p.z, p.w, line);
   }
   unsigned total;
-  const unsigned pos = block_exclusive_scan(len, total);
+  const unsigned pos = block_exclusive_scan<PCD_TILE>(len, total);
   const unsigned off = tile_off[blockIdx.x], end = off + total;
   // output byte g sits at buf byte g - (off & ~15): the shared copy has the output's alignment
   const unsigned shift = off & ~15u;

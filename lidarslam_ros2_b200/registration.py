@@ -11,6 +11,7 @@ fallback; constructing an engine without a CUDA device raises.
 from __future__ import annotations
 
 import ctypes as C
+import os
 
 import numpy as np
 
@@ -91,6 +92,14 @@ class _Registration:
     def setInputTargetDevice(self, dev_ptr: int, n: int):
         """Target already resident in HBM as n float4 (e.g. a torch CUDA tensor's data_ptr())."""
         self._check(self._lib.b200reg_set_input_target_device(self._h, C.c_void_p(dev_ptr), n))
+
+    def setInputTargetPCD(self, path: str) -> int:
+        """setInputTarget of loadPCDFile(path): the file is parsed on the device and becomes the target without its points
+        passing through host floats (b200reg_set_input_target_pcd). On error the previous target stays. Returns the
+        number of points."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200reg_set_input_target_pcd(self._h, os.fsencode(path), C.byref(n)))
+        return n.value
 
     def setInputSourceDevice(self, dev_ptr: int, n: int):
         self._n_source = n
