@@ -132,7 +132,9 @@ struct Accum {
   bool first;  // no point applied yet this evaluation: store instead of read-modify-write
   double score;
   int hits;
-  __device__ __forceinline__ void add(int slot, float v) { s[slot][tid] = first ? v : s[slot][tid] + v; }
+  // FIRST: the thread's first point with hits (a plain store, no load); the caller branches on `first` once per point
+  template <bool FIRST>
+  __device__ __forceinline__ void add(int slot, float v) { s[slot][tid] = FIRST ? v : s[slot][tid] + v; }
 };
 
 struct PairSums {  // sums over the voxels hit by one point
@@ -190,7 +192,7 @@ __device__ __forceinline__ void accumulate_pair(const Rec& R, bool valid, float3
 }
 
 // per-POINT application of J (point gradient, :396-412) and H_E (:414-436) to the pair sums
-template <bool HESS>
+template <bool HESS, bool FIRST>
 __device__ __forceinline__ void apply_point(const float4 p, const PairSums& ps, const NdtControl& c, float gd2, Accum& a) {
   const float x = p.x, y = p.y, z = p.z;
   // the 24 + 45 table floats are read as 16-byte shared-memory vectors (NdtControl: jang at byte 48, hang at 144)
@@ -207,12 +209,12 @@ __device__ __forceinline__ void apply_point(const float4 p, const PairSums& ps, 
   const float j7 = ja5.y * x + ja5.z * y + ja5.w * z;
   a.score += (double)ps.score;
   a.hits += ps.hits;
-  a.add(0, ps.S0);
-  a.add(1, ps.S1);
-  a.add(2, ps.S2);
-  a.add(3, j0 * ps.S1 + j1 * ps.S2);
-  a.add(4, j2 * ps.S0 + j3 * ps.S1 + j4 * ps.S2);
-  a.add(5, j5 * ps.S0 + j6 * ps.S1 + j7 * ps.S2);
+  a.add<FIRST>(0, ps.S0);
+  a.add<FIRST>(1, ps.S1);
+  a.add<FIRST>(2, ps.S2);
+  a.add<FIRST>(3, j0 * ps.S1 + j1 * ps.S2);
+  a.add<FIRST>(4, j2 * ps.S0 + j3 * ps.S1 + j4 * ps.S2);
+  a.add<FIRST>(5, j5 * ps.S0 + j6 * ps.S1 + j7 * ps.S2);
   if (HESS) {
     // W = sum e (C - d2 s s^T)
     const float W00 = ps.M00 - gd2 * ps.Q00, W01 = ps.M01 - gd2 * ps.Q01, W02 = ps.M02 - gd2 * ps.Q02;
@@ -234,15 +236,17 @@ __device__ __forceinline__ void apply_point(const float4 p, const PairSums& ps, 
     const float hF1 = h9.x * x + h9.y * y + h9.z * z, hF2 = h9.w * x + h10.x * y + h10.y * z,
                 hF3 = h10.z * x + h10.w * y + h44 * z;
     // upper triangle, row-major: (0,0..5) (1,1..5) (2,2..5) (3,3..5) (4,4..5) (5,5)
-    a.add(6 + 0, W00); a.add(6 + 1, W01); a.add(6 + 2, W02); a.add(6 + 3, a0); a.add(6 + 4, b0); a.add(6 + 5, c0);
-    a.add(6 + 6, W11); a.add(6 + 7, W12); a.add(6 + 8, a1); a.add(6 + 9, b1); a.add(6 + 10, c1);
-    a.add(6 + 11, W22); a.add(6 + 12, a2); a.add(6 + 13, b2); a.add(6 + 14, c2);
-    a.add(6 + 15, (j0 * a1 + j1 * a2) + (hA2 * ps.S1 + hA3 * ps.S2));
-    a.add(6 + 16, (j0 * b1 + j1 * b2) + (hB2 * ps.S1 + hB3 * ps.S2));
-    a.add(6 + 17, (j0 * c1 + j1 * c2) + (hC2 * ps.S1 + hC3 * ps.S2));
-    a.add(6 + 18, (j2 * b0 + j3 * b1 + j4 * b2) + (hD1 * ps.S0 + hD2 * ps.S1 + hD3 * ps.S2));
-    a.add(6 + 19, (j2 * c0 + j3 * c1 + j4 * c2) + (hE1 * ps.S0 + hE2 * ps.S1 + hE3 * ps.S2));
-    a.add(6 + 20, (j5 * c0 + j6 * c1 + j7 * c2) + (hF1 * ps.S0 + hF2 * ps.S1 + hF3 * ps.S2));
+    a.add<FIRST>(6 + 0, W00); a.add<FIRST>(6 + 1, W01); a.add<FIRST>(6 + 2, W02);
+    a.add<FIRST>(6 + 3, a0); a.add<FIRST>(6 + 4, b0); a.add<FIRST>(6 + 5, c0);
+    a.add<FIRST>(6 + 6, W11); a.add<FIRST>(6 + 7, W12); a.add<FIRST>(6 + 8, a1); a.add<FIRST>(6 + 9, b1);
+    a.add<FIRST>(6 + 10, c1);
+    a.add<FIRST>(6 + 11, W22); a.add<FIRST>(6 + 12, a2); a.add<FIRST>(6 + 13, b2); a.add<FIRST>(6 + 14, c2);
+    a.add<FIRST>(6 + 15, (j0 * a1 + j1 * a2) + (hA2 * ps.S1 + hA3 * ps.S2));
+    a.add<FIRST>(6 + 16, (j0 * b1 + j1 * b2) + (hB2 * ps.S1 + hB3 * ps.S2));
+    a.add<FIRST>(6 + 17, (j0 * c1 + j1 * c2) + (hC2 * ps.S1 + hC3 * ps.S2));
+    a.add<FIRST>(6 + 18, (j2 * b0 + j3 * b1 + j4 * b2) + (hD1 * ps.S0 + hD2 * ps.S1 + hD3 * ps.S2));
+    a.add<FIRST>(6 + 19, (j2 * c0 + j3 * c1 + j4 * c2) + (hE1 * ps.S0 + hE2 * ps.S1 + hE3 * ps.S2));
+    a.add<FIRST>(6 + 20, (j5 * c0 + j6 * c1 + j7 * c2) + (hF1 * ps.S0 + hF2 * ps.S1 + hF3 * ps.S2));
   }
 }
 
@@ -310,7 +314,8 @@ __device__ __forceinline__ void process_point(const NdtLaunch& L, const NdtContr
         }
   }
   if (ps.hits) {
-    apply_point<HESS>(p, ps, c, gd2, acc);
+    if (acc.first) apply_point<HESS, true>(p, ps, c, gd2, acc);
+    else apply_point<HESS, false>(p, ps, c, gd2, acc);
     acc.first = false;
   }
 }
