@@ -470,6 +470,66 @@ int b200reg_load_pcd(int device, const char* path, float* out_xyzi, size_t capac
  * keeps a pinned and a device buffer of its body's size. n_points (may be NULL) = points of the new target. */
 int b200reg_set_input_target_pcd(b200reg_t h, const char* path, size_t* n_points);
 
+/* ---- localisation in a prior map: drive in the map.pcd saved above ---------------------------------------------------
+ * The reference has no localisation mode; this is the session's own contract. The prior map stays on the device as float4
+ * (x, y, z, intensity) and is never modified. The registration target of a frame is a CUT of it: the rows with
+ *   dx = (double)x - cx, dy = (double)y - cy, dx * dx + dy * dy <= crop_radius * crop_radius
+ * (cx, cy the session's position when the cut is made; every operation one IEEE double operation, nothing fused; NaN
+ * coordinates fail; z is not tested — a cylinder, like the range filter), in MAP ORDER: bitwise map[mask] of that boolean
+ * mask. The cut is a two-pass stream compaction (per-tile counts, scan, write at tile offset + rank), so target indices
+ * (GICP's correspondences, its "lower index wins a tie") mean rows of the map in order. Each cut reads the map twice and
+ * writes the kept rows once: 32 * n_map + 16 * n_cut bytes. At most 2^32 - 1 points; larger maps are B200REG_ERR_ARG.
+ *
+ * b200sm_set_prior_map_pcd reads the file with the reader of b200reg_load_pcd (the session keeps that reader's fixed-size
+ * buffers); on B200REG_ERR_IO / B200REG_ERR_FORMAT / B200REG_ERR_ARG (no points) the previous prior map and cut stay and
+ * b200sm_last_error names the reason. *n_points (may be NULL) = POINTS of the file; non-finite rows stay in the map and
+ * are never kept by a cut. b200sm_set_prior_map takes host records as b200sm_import_submap does (no intensity field:
+ * intensity 0). Both replace the previous map, return with the session's stream synchronised and make the current cut
+ * stale: the next frame cuts anew. */
+int b200sm_set_prior_map_pcd(b200sm_t s, const char* path, size_t* n_points);
+int b200sm_set_prior_map(b200sm_t s, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes);
+/* crop_radius: horizontal radius (metres, finite, > 0) of the cut; recrop_distance (finite, >= 0): the target is cut again
+ * once the pose is this far (horizontally) from the centre of the current cut. Defaults 120 and 20. The caller keeps
+ * crop_radius >= scan_max_range + recrop_distance, so that a scan never reaches past the edge of its target; this is not
+ * enforced. Makes the current cut stale. Anything else: B200REG_ERR_ARG, nothing changes. */
+int b200sm_set_localization_params(b200sm_t s, double crop_radius, double recrop_distance);
+typedef struct b200sm_localize_stats {
+  size_t n_map, n_cut, n_target;     /* prior map, current cut, what the engine was given (GICP: after VoxelGrid) */
+  double cut_centre[2];              /* x, y the current cut was made around                                   */
+  double dist_from_centre;           /* horizontal distance of the pose from the cut's centre as the last frame compared it
+                                        with recrop_distance (before any re-cut that frame made)              */
+  int n_cuts;                        /* cuts made since the prior map was set                                   */
+  int cut_pending;                   /* a new cut waits to become the target at the next frame                  */
+} b200sm_localize_stats;
+/* One frame of a localising frontend: b200sm_receive_cloud without a map of its own. (1) The frame is uploaded exactly as
+ * there (sensor transform, armed de-skew, range filter). (2) If there is no cut yet or it is stale (new prior map, new
+ * parameters, b200sm_set_initial_pose since), the map is cut around the current position now; a pending cut then becomes
+ * the engine's target (NDT: the cut; GICP: VoxelGrid(vg_size_for_input) of it, as for the targeted cloud). (3)
+ * VoxelGrid(vg_size_for_input) + setInputSource, guess = current pose (or the armed use_odom guess), align, and the pose of
+ * publishMapAndPose. No submap is made and latest_distance does not move. (4) dist_from_centre = sqrt(dx * dx + dy * dy)
+ * in double from the new position to cut_centre; when dist_from_centre >= recrop_distance the map is cut again around the
+ * new position at once, *target_recut = 1, and that cut becomes the target at the start of the next frame.
+ * B200REG_ERR_NO_TARGET: no prior map, or the cut of step 2 keeps no row (the pose is outside the map; the message gives
+ * centre and radius) — the pose, the previous cut and the engine's target are unchanged. A re-cut of step 4 that keeps no
+ * row does not fail the frame: *target_recut = 0, the old cut and target stay, the next frame tries again.
+ * B200REG_ERR_GRID (NDT): the cut's voxel grid would overflow int32 at the engine's resolution; the engine's target is
+ * unchanged and the cut stays pending. Frames of b200sm_receive_cloud and of this call may be mixed on one session: each
+ * uses its own buffers (the targeted cloud there, the cut here). */
+int b200sm_localize_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes,
+                          long intensity_offset_bytes, double* pose7_out, float* final_T_colmajor16_out, int* target_recut);
+/* The initial pose from several hypotheses (NDT only; a GICP handle is B200REG_ERR_ARG). Steps 1 and 2 as above (the cut
+ * is made around the current position, e.g. a rough b200sm_set_initial_pose), then the filtered scan is registered from
+ * `count` >= 1 initial guesses (16 * count floats, column-major) in ONE b200reg_ndt_align_batch_device call, the scan read
+ * in place `count` times. Every results[k] is bitwise what b200reg_align gives for that scan, target and guess. The
+ * converged row with the highest trans_probability (the lowest index on a tie) becomes the session's pose; *best = its
+ * index, or -1 when none converged (pose unchanged, B200REG_OK). An armed use_odom guess is left for the next frame. */
+int b200sm_localize_init(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes,
+                         long intensity_offset_bytes, const float* guesses, int count, b200reg_batch_result* results,
+                         int* best);
+int b200sm_get_localize_stats(b200sm_t s, b200sm_localize_stats* out);
+/* read-back of the current cut (the newest one, pending or adopted), like b200sm_get_targeted */
+int b200sm_get_cut(b200sm_t s, float* out_xyzi, size_t capacity, size_t* n);
+
 typedef struct b200sm_stats {
   size_t n_scan, n_filtered, n_targeted, n_submaps;
   int kernel_launches;

@@ -396,6 +396,46 @@ class ScanMatcherSession {
     check(b200sm_save_map_pcd_ascii(s_.get(), poses_colmajor16, path.c_str(), &n, &bytes));
     return bytes;
   }
+  // ---- localisation in a prior map (b200sm_set_prior_map*, b200sm_localize_*): the map stays on the device, each frame is
+  // registered against a cut of it around the pose. Returns the map's points.
+  size_t setPriorMapPCD(const std::string& path) {
+    size_t n = 0;
+    check(b200sm_set_prior_map_pcd(s_.get(), path.c_str(), &n));
+    return n;
+  }
+  void setPriorMap(const float* points, size_t n, size_t stride, long intensity_offset) {
+    check(b200sm_set_prior_map(s_.get(), points, n, stride, intensity_offset));
+  }
+  // keep crop_radius >= scan_max_range + recrop_distance
+  void setLocalizationParams(double crop_radius, double recrop_distance) {
+    check(b200sm_set_localization_params(s_.get(), crop_radius, recrop_distance));
+  }
+  // one frame; returns true when the target was cut again (the new cut is the target from the next frame on)
+  bool localizeCloud(b200reg_t reg, const float* points, size_t n, size_t stride, long intensity_offset, double pose7[7], float final16[16]) {
+    int recut = 0;
+    check(b200sm_localize_cloud(s_.get(), reg, points, n, stride, intensity_offset, pose7, final16, &recut));
+    return recut != 0;
+  }
+  // NDT: the initial pose from guesses.size() / 16 hypotheses (column-major 4x4 each) in one batch launch; returns the index
+  // of the adopted one or -1, rows = one result per guess
+  int localizeInit(b200reg_t reg, const float* points, size_t n, size_t stride, long intensity_offset, const std::vector<float>& guesses,
+                   std::vector<b200reg_batch_result>& rows) {
+    int best = -1;
+    rows.resize(guesses.size() / 16);
+    check(b200sm_localize_init(s_.get(), reg, points, n, stride, intensity_offset, guesses.data(), (int)rows.size(), rows.data(), &best));
+    return best;
+  }
+  b200sm_localize_stats localizeStats() const {
+    b200sm_localize_stats st{};
+    check(b200sm_get_localize_stats(s_.get(), &st));
+    return st;
+  }
+  void cutCloud(std::vector<float>& xyzi) {
+    size_t n = 0;
+    check(b200sm_get_cut(s_.get(), nullptr, 0, &n));
+    xyzi.resize(4 * n);
+    check(b200sm_get_cut(s_.get(), xyzi.data(), n, &n));
+  }
   b200sm_t handle() const { return s_.get(); }
 
  private:

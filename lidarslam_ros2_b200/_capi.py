@@ -45,6 +45,8 @@ SYMBOLS = [
     "b200sm_imu_get_state", "b200sm_imu_get_sample", "b200sm_imu_get_trace", "b200sm_pose_adjust", "b200sm_assemble_map",
     "b200sm_save_map_pcd_ascii", "b200reg_encode_pcd_ascii", "b200sm_set_sensor_transform", "b200sm_odom_next_scan",
     "b200reg_load_pcd", "b200reg_set_input_target_pcd",
+    "b200sm_set_prior_map_pcd", "b200sm_set_prior_map", "b200sm_set_localization_params", "b200sm_localize_cloud",
+    "b200sm_localize_init", "b200sm_get_localize_stats", "b200sm_get_cut",
     # include/b200comm.h
     "b200comm_unique_id", "b200comm_create", "b200comm_destroy", "b200comm_all_gather_rows", "b200comm_rank", "b200comm_last_error",
     "b200comm_board_create", "b200comm_board_destroy", "b200comm_board_info",
@@ -69,6 +71,11 @@ class SmPoseAdjustResult(C.Structure):
 class SmStats(C.Structure):
     _fields_ = [("n_scan", C.c_size_t), ("n_filtered", C.c_size_t), ("n_targeted", C.c_size_t), ("n_submaps", C.c_size_t),
                 ("kernel_launches", C.c_int), ("trans", C.c_double), ("latest_distance", C.c_double)]
+
+
+class SmLocalizeStats(C.Structure):
+    _fields_ = [("n_map", C.c_size_t), ("n_cut", C.c_size_t), ("n_target", C.c_size_t), ("cut_centre", C.c_double * 2),
+                ("dist_from_centre", C.c_double), ("n_cuts", C.c_int), ("cut_pending", C.c_int)]
 
 
 class BatchResult(C.Structure):
@@ -198,6 +205,13 @@ def lib() -> C.CDLL:
     L.b200reg_load_pcd.argtypes = [i, C.c_char_p, vp, sz, C.POINTER(sz)]
     L.b200reg_set_input_target_pcd.argtypes = [vp, C.c_char_p, C.POINTER(sz)]
     L.b200sm_odom_next_scan.argtypes = [vp, vp, vp]
+    L.b200sm_set_prior_map_pcd.argtypes = [vp, C.c_char_p, C.POINTER(sz)]
+    L.b200sm_set_prior_map.argtypes = [vp, vp, sz, sz, C.c_long]
+    L.b200sm_set_localization_params.argtypes = [vp, d, d]
+    L.b200sm_localize_cloud.argtypes = [vp, vp, vp, sz, sz, C.c_long, vp, vp, C.POINTER(i)]
+    L.b200sm_localize_init.argtypes = [vp, vp, vp, sz, sz, C.c_long, vp, i, vp, C.POINTER(i)]
+    L.b200sm_get_localize_stats.argtypes = [vp, C.POINTER(SmLocalizeStats)]
+    L.b200sm_get_cut.argtypes = [vp, vp, sz, C.POINTER(sz)]
     L.b200comm_unique_id.argtypes = [vp]
     L.b200comm_create.argtypes = [vp, i, i, i, C.POINTER(vp)]
     L.b200comm_destroy.argtypes = [vp]

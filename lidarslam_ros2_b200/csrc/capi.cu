@@ -319,6 +319,17 @@ int set_cloud(b200reg_t h, bool target, const float* base, size_t n, size_t stri
   return B200REG_OK;
 }
 
+// false when an NDT handle could not grid this device cloud at its resolution (voxel_grid_covariance_omp_impl.hpp:79-84);
+// measured on the handle's stream, which is synchronised on return
+bool target_grid_fits(b200reg_t h, const float4* pts, size_t n) {
+  if (h->kind != B200REG_NDT) return true;
+  h->scratch_bounds.ensure(8);
+  const Bounds b = cloud_bounds(pts, n, h->scratch_bounds.ptr, h->stream);
+  h->other_launches += 1;
+  GridGeom g{};
+  return !b.any || make_grid_geom(b, h->ndt.resolution, g);
+}
+
 }  // namespace
 
 extern "C" {
@@ -497,18 +508,21 @@ int b200reg_set_input_target_pcd(b200reg_t h, const char* path, size_t* n_points
       ~Release() { b.release(); }
     } release{h->pcd_points};
     if (n == 0) return fail(h, B200REG_ERR_ARG, "setInputTargetPCD: the file has no points (empty input cloud ignored)");
-    if (h->kind == B200REG_NDT) {  // a map whose voxel grid would overflow int32 does not replace the current target
-      h->scratch_bounds.ensure(8);
-      const Bounds b = cloud_bounds(h->pcd_points.ptr, n, h->scratch_bounds.ptr, h->stream);
-      h->other_launches += 1;
-      GridGeom g{};
-      if (b.any && !make_grid_geom(b, h->ndt.resolution, g))
-        return fail(h, B200REG_ERR_GRID, (std::string("setInputTargetPCD: ") + path +
-                                          ": the voxel grid would overflow int32 at this resolution; the target is unchanged").c_str());
-    }
+    if (!target_grid_fits(h, h->pcd_points.ptr, n))  // such a map does not replace the current target
+      return fail(h, B200REG_ERR_GRID, (std::string("setInputTargetPCD: ") + path +
+                                        ": the voxel grid would overflow int32 at this resolution; the target is unchanged").c_str());
     const int r = set_cloud(h, true, nullptr, n, 16, h->pcd_points.ptr);
     if (r == B200REG_OK && n_points) *n_points = n;
     return r;
+  });
+}
+// Library-internal (not in include/b200reg.h): would setInputTarget of this device cloud succeed? B200REG_ERR_GRID when its
+// voxel grid would overflow int32 at the handle's resolution (NDT); the handle's target is not touched either way.
+int b200reg_check_target_grid_device(b200reg_t h, const void* dev, size_t n) {
+  if (!h || !dev || n == 0) return B200REG_ERR_ARG;
+  return guarded(h, [&]() {
+    if (target_grid_fits(h, static_cast<const float4*>(dev), n)) return (int)B200REG_OK;
+    return fail(h, B200REG_ERR_GRID, "the target's voxel grid would overflow int32 at this resolution; the target is unchanged");
   });
 }
 // Library-internal (not in include/b200reg.h): the frontend session hands over its voxel-filtered scan WITHOUT a copy — the

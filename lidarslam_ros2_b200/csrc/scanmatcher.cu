@@ -16,6 +16,8 @@
 //   doPoseAdjustment: g2o pose graph + LM (host, pose_graph.hpp)                            :262-319   -> b200sm_pose_adjust
 //   doPoseAdjustment: modified_map / modified_map_array                                     :321-368   -> b200sm_assemble_map
 //   doPoseAdjustment: savePCDFileASCII("map.pcd", modified_map)                             :369       -> b200sm_save_map_pcd_ascii
+// Localising in a saved map has no counterpart in the reference: b200sm_set_prior_map* keep the map on the device and
+// b200sm_localize_cloud registers each frame against a stable cut of it around the pose (csrc/map_cut.hpp).
 // The submaps (sensor-frame, voxel-filtered) and the targeted cloud never leave the GPU; read-back entry points exist for
 // the parity tests and for the node's publishers.
 #include <cerrno>
@@ -29,6 +31,7 @@
 #include "../../include/b200reg.h"
 #include "deskew.hpp"
 #include "engine.hpp"
+#include "map_cut.hpp"
 #include "pose_graph.hpp"
 #include "sensor_frame.hpp"
 
@@ -54,6 +57,71 @@ __global__ void range_filter_kernel(const float4* __restrict__ in, size_t n, dou
   if (lane == __ffs(mask) - 1) base = atomicAdd(count, (unsigned)__popc(mask));
   base = __shfl_sync(0xffffffffu, base, __ffs(mask) - 1);
   if (keep) out[base + __popc(mask & ((1u << lane) - 1u))] = p;
+}
+
+// The cut of the prior map, pass 1: counts[tile] = rows of the tile that cut_keep keeps. A tile's eight 32-row rounds per
+// warp are all loaded before the first ballot.
+__device__ __forceinline__ void cut_round_masks(const float4* __restrict__ map, size_t n, size_t tile, int warp, int lane, double cx,
+                                                double cy, double r2, float4 (&p)[CUT_ROUNDS], unsigned (&mask)[CUT_ROUNDS]) {
+#pragma unroll
+  for (int k = 0; k < CUT_ROUNDS; k++) {
+    const size_t i = cut_row(tile, warp, k, lane);
+    p[k] = i < n ? map[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+#pragma unroll
+  for (int k = 0; k < CUT_ROUNDS; k++) {
+    const size_t i = cut_row(tile, warp, k, lane);
+    mask[k] = __ballot_sync(0xffffffffu, i < n && cut_keep(p[k].x, p[k].y, cx, cy, r2));
+  }
+}
+
+__global__ void __launch_bounds__(CUT_THREADS) cut_count_kernel(const float4* __restrict__ map, size_t n, double cx, double cy, double r2,
+                                                                unsigned* __restrict__ counts) {
+  __shared__ unsigned warp_count[CUT_WARPS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float4 p[CUT_ROUNDS];
+  unsigned mask[CUT_ROUNDS];
+  cut_round_masks(map, n, blockIdx.x, warp, lane, cx, cy, r2, p, mask);
+  unsigned c = 0;
+#pragma unroll
+  for (int k = 0; k < CUT_ROUNDS; k++) c += (unsigned)__popc(mask[k]);
+  if (lane == 0) warp_count[warp] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned t = 0;
+#pragma unroll
+    for (int w = 0; w < CUT_WARPS; w++) t += warp_count[w];
+    counts[blockIdx.x] = t;
+  }
+}
+
+// Pass 2: the same predicate on the same (never modified) map; a kept row goes to tile offset + kept rows of the earlier
+// warps of the tile + of the warp's earlier rounds + its rank in the round, i.e. map order. `out` has exactly `total`
+// rows, the count the host read back after pass 1: a destination outside it is not stored, *tripped is raised instead.
+__global__ void __launch_bounds__(CUT_THREADS) cut_write_kernel(const float4* __restrict__ map, size_t n, double cx, double cy, double r2,
+                                                                const unsigned* __restrict__ tile_offsets, unsigned total,
+                                                                float4* __restrict__ out, unsigned* __restrict__ tripped) {
+  __shared__ unsigned warp_count[CUT_WARPS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float4 p[CUT_ROUNDS];
+  unsigned mask[CUT_ROUNDS];
+  cut_round_masks(map, n, blockIdx.x, warp, lane, cx, cy, r2, p, mask);
+  unsigned c = 0;
+#pragma unroll
+  for (int k = 0; k < CUT_ROUNDS; k++) c += (unsigned)__popc(mask[k]);
+  if (lane == 0) warp_count[warp] = c;
+  __syncthreads();
+  unsigned base = tile_offsets[blockIdx.x];
+  for (int w = 0; w < warp; w++) base += warp_count[w];
+#pragma unroll
+  for (int k = 0; k < CUT_ROUNDS; k++) {
+    if ((mask[k] >> lane) & 1u) {
+      const unsigned dst = base + cut_rank_in_round(mask[k], lane);
+      if (dst < total) out[dst] = p[k];
+      else atomicOr(tripped, 1u);
+    }
+    base += (unsigned)__popc(mask[k]);
+  }
 }
 
 struct Mat34d {
@@ -203,6 +271,17 @@ struct b200sm_session {
   bool odom_armed = false;
   float odom_mat[16] = {};
   float previous_odom_mat[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  // localisation in a prior map (b200sm_set_prior_map*, b200sm_localize_cloud)
+  PcdLoader pcd_loader;
+  DeviceBuffer<float4> prior_map, prior_incoming;  // the map; a new one is loaded beside it and swapped in once complete
+  size_t n_prior = 0;
+  double crop_radius = 120.0, recrop_distance = 20.0;  // >= the default scan_max_range + recrop_distance
+  DeviceBuffer<float4> cut;             // the current cut, map order; the engine holds its own copy of its target
+  DeviceBuffer<unsigned> cut_counts, cut_scan_tmp;  // per-tile counts -> offsets, [tiles] total, [tiles + 1] tripwire flag
+  size_t n_cut = 0, n_cut_target = 0;
+  double cut_centre[2] = {0, 0}, dist_from_centre = 0;
+  int n_cuts = 0;
+  bool have_cut = false, cut_stale = true, cut_pending = false;
 };
 
 namespace {
@@ -353,21 +432,78 @@ int update_map(b200sm_t s, const float* final_T, const double* position, const d
   return B200REG_OK;
 }
 
+// setInputTarget(cloud) from a session buffer (GICP: VoxelGrid(vg_size_for_input) of it first, sm.cpp:311-317); *n_given =
+// the points the engine received. The engine copies, so `cloud` may be rebuilt as soon as this returns.
+int hand_over_target(b200sm_t s, b200reg_t reg, int is_gicp, const float4* cloud, size_t n, const char* empty_msg, size_t* n_given) {
+  const float4* t = cloud;
+  if (is_gicp) t = filter_on_device(s, s->vg_target, cloud, n, s->vg_size_for_input, &n);
+  if (n == 0) return sm_fail(s, B200REG_ERR_NO_TARGET, empty_msg);
+  B200_CUDA(cudaStreamSynchronize(s->stream));
+  const int rc = b200reg_set_input_target_device(reg, t, n);
+  if (rc != B200REG_OK) s->err = std::string("setInputTarget: ") + b200reg_last_error(reg);
+  else if (n_given) *n_given = n;
+  return rc;
+}
+
 // receiveCloud :300-322: the rebuilt targeted cloud becomes the registration target
 int adopt_target(b200sm_t s, b200reg_t reg, int is_gicp) {
   if (!s->target_pending) return B200REG_OK;
-  const float4* t = s->targeted.ptr;
-  size_t n = s->n_targeted;
-  if (is_gicp) t = filter_on_device(s, s->vg_target, s->targeted.ptr, s->n_targeted, s->vg_size_for_input, &n);
-  if (n == 0) return sm_fail(s, B200REG_ERR_NO_TARGET, "targeted cloud is empty");
-  B200_CUDA(cudaStreamSynchronize(s->stream));
-  const int rc = b200reg_set_input_target_device(reg, t, n);
+  const int rc = hand_over_target(s, reg, is_gicp, s->targeted.ptr, s->n_targeted, "targeted cloud is empty", nullptr);
+  if (rc == B200REG_OK) s->target_pending = false;
+  return rc;
+}
+
+// sim_trans = getTransformation(corrent_pose_stamped_.pose): Affine3d matrix cast to float (:493-499), row- and column-major
+void sim_trans(b200sm_t s, float* T_row, float* sim_col) {
+  double M[16];
+  pose_to_matrix_d(s->position, s->quat, M);
+  for (int r = 0; r < 4; r++)
+    for (int c = 0; c < 4; c++) {
+      T_row[r * 4 + c] = (float)M[r * 4 + c];
+      sim_col[c * 4 + r] = (float)M[r * 4 + c];
+    }
+}
+
+// publishMapAndPose's pose (:391-398): position and quaternion of a column-major float final transformation
+void adopt_pose(b200sm_t s, const float* final_col) {
+  double R[9];
+  for (int r = 0; r < 3; r++) {
+    for (int c = 0; c < 3; c++) R[r * 3 + c] = (double)final_col[c * 4 + r];
+    s->position[r] = (double)final_col[12 + r];
+  }
+  matrix_to_quat_d(R, s->quat);
+}
+
+// The part of a frame the mapping and the localising frontend share, once the engine has its target: VoxelGrid +
+// setInputSource (:323-328), guess = current pose or the use_odom guess (:333-348), align (:350), the new pose (:391-398).
+int register_frame(b200sm_t s, b200reg_t reg, bool use_odom, float* final_col) {
+  int rc = set_source_from_scan(s, reg);
+  if (rc != B200REG_OK) return rc;
+  float sim_col[16], T_row[16];
+  sim_trans(s, T_row, sim_col);
+  if (use_odom) {  // sim_trans * previous_odom_mat_.inverse() * odom_mat, then previous_odom_mat_ = odom_mat
+    odom_guess_f(T_row, s->previous_odom_mat, s->odom_mat);
+    for (int r = 0; r < 4; r++)
+      for (int c = 0; c < 4; c++) sim_col[c * 4 + r] = T_row[r * 4 + c];
+  }
+  rc = b200reg_align(reg, sim_col, final_col);
   if (rc != B200REG_OK) {
-    s->err = std::string("setInputTarget: ") + b200reg_last_error(reg);
+    s->err = std::string("align: ") + b200reg_last_error(reg);
     return rc;
   }
-  s->target_pending = false;
+  adopt_pose(s, final_col);
   return B200REG_OK;
+}
+
+void write_pose(b200sm_t s, double* pose7_out) {
+  if (!pose7_out) return;
+  for (int k = 0; k < 3; k++) pose7_out[k] = s->position[k];
+  for (int k = 0; k < 4; k++) pose7_out[3 + k] = s->quat[k];
+}
+
+bool valid_frame_args(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes) {
+  return s && reg && points && n != 0 && stride_bytes >= 12 && (stride_bytes % 4) == 0 &&
+         (intensity_offset_bytes < 0 || (intensity_offset_bytes % 4) == 0);
 }
 
 int read_back(b200sm_t s, const float4* d, size_t n, float* out, size_t cap, size_t* n_out) {
@@ -432,6 +568,7 @@ int b200sm_set_initial_pose(b200sm_t s, const double* position3, const double* q
   if (!s || !position3 || !quat_xyzw) return B200REG_ERR_ARG;
   for (int k = 0; k < 3; k++) s->position[k] = s->previous_position[k] = position3[k];
   for (int k = 0; k < 4; k++) s->quat[k] = quat_xyzw[k];
+  s->cut_stale = true;  // a localising session cuts its target around the new position at the next frame
   return B200REG_OK;
 }
 
@@ -474,9 +611,7 @@ int b200sm_update_map(b200sm_t s, b200reg_t reg, const float* final_T_colmajor16
 
 int b200sm_receive_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes,
                          double* pose7_out, float* final_T_colmajor16_out, int* map_updated) {
-  if (!s || !reg || !points || n == 0 || stride_bytes < 12 || (stride_bytes % 4) != 0 ||
-      (intensity_offset_bytes >= 0 && (intensity_offset_bytes % 4) != 0))
-    return B200REG_ERR_ARG;
+  if (!valid_frame_args(s, reg, points, n, stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
   return sm_guarded(s, [&]() {
     if (map_updated) *map_updated = 0;
     const bool use_odom = s->odom_armed;  // armed for this frame only, like the de-skew
@@ -484,21 +619,11 @@ int b200sm_receive_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t 
     int kind = B200REG_NDT;
     b200reg_get_kind(reg, &kind);
     upload_frame(s, points, n, stride_bytes, intensity_offset_bytes);
-    // sim_trans = getTransformation(corrent_pose_stamped_.pose): Affine3d matrix cast to float (:493-499)
-    double M[16];
-    float sim_col[16], T_row[16];
-    auto sim_trans = [&]() {
-      pose_to_matrix_d(s->position, s->quat, M);
-      for (int r = 0; r < 4; r++)
-        for (int c = 0; c < 4; c++) {
-          T_row[r * 4 + c] = (float)M[r * 4 + c];
-          sim_col[c * 4 + r] = (float)M[r * 4 + c];
-        }
-    };
     int rc;
     if (!s->initial_cloud_received) {  // initializeMap (:257-297): the first scan, at the initial pose, is the map
       s->initial_cloud_received = true;
-      sim_trans();
+      float sim_col[16], T_row[16];
+      sim_trans(s, T_row, sim_col);
       rc = update_map(s, T_row, s->position, s->quat);
       if (rc != B200REG_OK) return rc;
       rc = adopt_target(s, reg, /*is_gicp=*/0);  // initializeMap hands the transformed cloud over unfiltered
@@ -506,28 +631,11 @@ int b200sm_receive_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t 
     }
     rc = adopt_target(s, reg, kind == B200REG_GICP);  // :300-322
     if (rc != B200REG_OK) return rc;
-    rc = set_source_from_scan(s, reg);                // :323-328
-    if (rc != B200REG_OK) return rc;
-    sim_trans();
-    if (use_odom) {  // :333-348: sim_trans * previous_odom_mat_.inverse() * odom_mat, then previous_odom_mat_ = odom_mat
-      odom_guess_f(T_row, s->previous_odom_mat, s->odom_mat);
-      for (int r = 0; r < 4; r++)
-        for (int c = 0; c < 4; c++) sim_col[c * 4 + r] = T_row[r * 4 + c];
-    }
     float final_col[16];
-    rc = b200reg_align(reg, sim_col, final_col);      // :350
-    if (rc != B200REG_OK) {
-      s->err = std::string("align: ") + b200reg_last_error(reg);
-      return rc;
-    }
-    // publishMapAndPose (:391-434)
-    double R[9], pos[3];
-    for (int r = 0; r < 3; r++) {
-      for (int c = 0; c < 3; c++) R[r * 3 + c] = (double)final_col[c * 4 + r];
-      pos[r] = (double)final_col[12 + r];
-    }
-    matrix_to_quat_d(R, s->quat);
-    for (int k = 0; k < 3; k++) s->position[k] = pos[k];
+    rc = register_frame(s, reg, use_odom, final_col);  // :323-353, 391-398
+    if (rc != B200REG_OK) return rc;
+    // publishMapAndPose (:399-434)
+    const double* pos = s->position;
     const double dx = pos[0] - s->previous_position[0], dy = pos[1] - s->previous_position[1], dz = pos[2] - s->previous_position[2];
     s->trans = std::sqrt(dx * dx + dy * dy + dz * dz);
     if (s->trans >= s->trans_for_mapupdate) {
@@ -540,10 +648,7 @@ int b200sm_receive_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t 
       if (rc != B200REG_OK) return rc;
       if (map_updated) *map_updated = 1;
     }
-    if (pose7_out) {
-      for (int k = 0; k < 3; k++) pose7_out[k] = s->position[k];
-      for (int k = 0; k < 4; k++) pose7_out[3 + k] = s->quat[k];
-    }
+    write_pose(s, pose7_out);
     if (final_T_colmajor16_out) std::memcpy(final_T_colmajor16_out, final_col, sizeof(final_col));
     return (int)B200REG_OK;
   });
@@ -1080,6 +1185,230 @@ int b200sm_imu_get_trace(b200sm_t s, size_t capacity, size_t* n, float* rel_time
     *n = s->imu.get_trace(capacity, rel_time, t, front, skip, k_first, rounds, s->stream);
     return (int)B200REG_OK;
   });
+}
+
+}  // extern "C"
+
+// ---- localisation in a prior map: the map resident on the device, the registration target a stable cut around the pose ----
+extern "C" int b200reg_check_target_grid_device(b200reg_t h, const void* dev, size_t n);  // capi.cu (library-internal)
+
+namespace {
+
+// the freshly loaded map replaces the previous one (whose memory is freed); the next frame cuts anew
+int install_prior_map(b200sm_t s, size_t n) {
+  std::swap(s->prior_map.ptr, s->prior_incoming.ptr);
+  std::swap(s->prior_map.cap, s->prior_incoming.cap);
+  s->prior_incoming.release();
+  s->n_prior = n;
+  s->cut_stale = true;
+  s->cut_pending = false;
+  s->n_cuts = 0;
+  return B200REG_OK;
+}
+
+// The rows of the prior map within crop_radius (horizontally) of (cx, cy), in map order, into s->cut: count per tile, scan,
+// read the total, size the output, write. Returns with the stream synchronised. B200REG_ERR_NO_TARGET when no row is kept:
+// nothing is written then and the previous cut stays as it is.
+int make_cut(b200sm_t s, double cx, double cy) {
+  const size_t tiles = cut_tiles(s->n_prior);
+  const double r2 = s->crop_radius * s->crop_radius;
+  s->cut_counts.ensure(tiles + 2);
+  cut_count_kernel<<<(unsigned)tiles, CUT_THREADS, 0, s->stream>>>(s->prior_map.ptr, s->n_prior, cx, cy, r2, s->cut_counts.ptr);
+  B200_CUDA(cudaGetLastError());
+  counter_scan_async(s->cut_counts.ptr, tiles, s->cut_scan_tmp, s->stream);
+  B200_CUDA(cudaGetLastError());
+  unsigned total = 0;
+  B200_CUDA(cudaMemcpyAsync(&total, s->cut_counts.ptr + tiles, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+  B200_CUDA(cudaStreamSynchronize(s->stream));
+  s->launches += 4;
+  if (total == 0) {
+    char msg[200];
+    std::snprintf(msg, sizeof(msg), "localize: no point of the prior map within %.3f m of (%.3f, %.3f)", s->crop_radius, cx, cy);
+    return sm_fail(s, B200REG_ERR_NO_TARGET, msg);
+  }
+  s->have_cut = false;  // until the rows are in place
+  s->cut.ensure(total);  // may free: the stream is idle and the engine keeps its own copy of its target
+  unsigned* tripped = s->cut_counts.ptr + tiles + 1;
+  B200_CUDA(cudaMemsetAsync(tripped, 0, sizeof(unsigned), s->stream));
+  cut_write_kernel<<<(unsigned)tiles, CUT_THREADS, 0, s->stream>>>(s->prior_map.ptr, s->n_prior, cx, cy, r2, s->cut_counts.ptr, total,
+                                                                   s->cut.ptr, tripped);
+  B200_CUDA(cudaGetLastError());
+  unsigned flag = 0;
+  B200_CUDA(cudaMemcpyAsync(&flag, tripped, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+  B200_CUDA(cudaStreamSynchronize(s->stream));
+  s->launches += 1;
+  if (flag) {
+    s->cut_stale = true;
+    return sm_fail(s, B200REG_ERR_CUDA, "localize: the cut's write pass met a row beyond the counted total (nothing was stored there)");
+  }
+  s->n_cut = total;
+  s->cut_centre[0] = cx;
+  s->cut_centre[1] = cy;
+  s->n_cuts += 1;
+  s->have_cut = true;
+  s->cut_stale = false;
+  s->cut_pending = true;
+  return B200REG_OK;
+}
+
+// step 2 of a localising frame: a cut around the current position if there is none or it is stale, then a pending cut
+// becomes the engine's target. An NDT cut whose voxel grid would overflow int32 is not handed over (it stays pending).
+int ensure_cut_target(b200sm_t s, b200reg_t reg, int kind) {
+  if (!s->have_cut || s->cut_stale) {
+    const int rc = make_cut(s, s->position[0], s->position[1]);
+    if (rc != B200REG_OK) return rc;
+  }
+  if (!s->cut_pending) return B200REG_OK;
+  if (kind == B200REG_NDT) {
+    const int rc = b200reg_check_target_grid_device(reg, s->cut.ptr, s->n_cut);
+    if (rc != B200REG_OK) {
+      s->err = std::string("localize: ") + b200reg_last_error(reg);
+      return rc;
+    }
+  }
+  const int rc = hand_over_target(s, reg, kind == B200REG_GICP, s->cut.ptr, s->n_cut, "localize: the cut is empty after VoxelGrid",
+                                  &s->n_cut_target);
+  if (rc == B200REG_OK) s->cut_pending = false;
+  return rc;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b200sm_set_prior_map_pcd(b200sm_t s, const char* path, size_t* n_points) {
+  if (!s || !path) return B200REG_ERR_ARG;
+  return sm_guarded(s, [&]() {
+    size_t n = 0;
+    std::string why;
+    const int before = s->pcd_loader.launches;
+    const int rc = s->pcd_loader.load(path, s->prior_incoming, &n, why, s->stream);  // the current map is not touched
+    s->launches += s->pcd_loader.launches - before;
+    if (rc == B200REG_OK && n != 0 && n <= CUT_MAX_POINTS) {
+      if (n_points) *n_points = n;
+      return install_prior_map(s, n);
+    }
+    s->prior_incoming.release();
+    s->err = std::string("set_prior_map_pcd: ") + path + ": ";
+    if (rc != B200REG_OK) {
+      s->err += why;
+      return rc;
+    }
+    s->err += n == 0 ? "the file has no points" : "more than 2^32 - 1 points";
+    return (int)B200REG_ERR_ARG;
+  });
+}
+
+int b200sm_set_prior_map(b200sm_t s, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes) {
+  if (!s || !points || n == 0 || stride_bytes < 12 || (stride_bytes % 4) != 0 ||
+      (intensity_offset_bytes >= 0 && (intensity_offset_bytes % 4) != 0))
+    return B200REG_ERR_ARG;
+  if (n > CUT_MAX_POINTS) return sm_fail(s, B200REG_ERR_ARG, "set_prior_map: more than 2^32 - 1 points");
+  return sm_guarded(s, [&]() {
+    s->prior_incoming.ensure(n);
+    // an uploader of its own, gone on return: the session's would keep a device (and, for pageable input, a pinned host)
+    // copy of the map's raw records for the rest of its life
+    CloudUploader once;
+    once.upload(points, n, stride_bytes, intensity_offset_bytes, 0.0f, s->prior_incoming.ptr, s->stream);
+    B200_CUDA(cudaStreamSynchronize(s->stream));  // the caller may reuse its buffer
+    s->launches += 1;
+    return install_prior_map(s, n);
+  });
+}
+
+int b200sm_set_localization_params(b200sm_t s, double crop_radius, double recrop_distance) {
+  if (!s) return B200REG_ERR_ARG;
+  if (!std::isfinite(crop_radius) || !std::isfinite(recrop_distance) || !(crop_radius > 0) || !(recrop_distance >= 0))
+    return sm_fail(s, B200REG_ERR_ARG, "set_localization_params: crop_radius must be finite and > 0, recrop_distance finite and >= 0");
+  s->crop_radius = crop_radius;
+  s->recrop_distance = recrop_distance;
+  s->cut_stale = true;
+  return B200REG_OK;
+}
+
+int b200sm_localize_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes,
+                          double* pose7_out, float* final_T_colmajor16_out, int* target_recut) {
+  if (!valid_frame_args(s, reg, points, n, stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
+  return sm_guarded(s, [&]() {
+    if (target_recut) *target_recut = 0;
+    if (s->n_prior == 0) return sm_fail(s, B200REG_ERR_NO_TARGET, "localize_cloud: no prior map");
+    const bool use_odom = s->odom_armed;  // armed for this frame only, like the de-skew
+    s->odom_armed = false;
+    int kind = B200REG_NDT;
+    b200reg_get_kind(reg, &kind);
+    upload_frame(s, points, n, stride_bytes, intensity_offset_bytes);
+    int rc = ensure_cut_target(s, reg, kind);
+    if (rc != B200REG_OK) return rc;
+    float final_col[16];
+    rc = register_frame(s, reg, use_odom, final_col);
+    if (rc != B200REG_OK) return rc;
+    // the target follows the pose: once it is recrop_distance from the centre of the cut, cut again around it now; the
+    // new cut becomes the target at the start of the next frame
+    const double dx = s->position[0] - s->cut_centre[0], dy = s->position[1] - s->cut_centre[1];
+    s->dist_from_centre = std::sqrt(dx * dx + dy * dy);
+    if (s->dist_from_centre >= s->recrop_distance) {
+      rc = make_cut(s, s->position[0], s->position[1]);
+      if (rc == B200REG_OK) {
+        if (target_recut) *target_recut = 1;
+      } else if (rc != B200REG_ERR_NO_TARGET) {
+        return rc;
+      }  // an empty re-cut: the frame stands, the old cut and target stay, the next frame tries again
+    }
+    write_pose(s, pose7_out);
+    if (final_T_colmajor16_out) std::memcpy(final_T_colmajor16_out, final_col, sizeof(final_col));
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_localize_init(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes,
+                         const float* guesses, int count, b200reg_batch_result* results, int* best) {
+  if (!valid_frame_args(s, reg, points, n, stride_bytes, intensity_offset_bytes) || !guesses || count < 1 || !results)
+    return B200REG_ERR_ARG;
+  int kind = B200REG_NDT;
+  b200reg_get_kind(reg, &kind);
+  if (kind != B200REG_NDT) return sm_fail(s, B200REG_ERR_ARG, "localize_init: the batch solver is NDT's");
+  return sm_guarded(s, [&]() {
+    if (best) *best = -1;
+    if (s->n_prior == 0) return sm_fail(s, B200REG_ERR_NO_TARGET, "localize_init: no prior map");
+    upload_frame(s, points, n, stride_bytes, intensity_offset_bytes);
+    int rc = ensure_cut_target(s, reg, kind);
+    if (rc != B200REG_OK) return rc;
+    rc = set_source_from_scan(s, reg);
+    if (rc != B200REG_OK) return rc;
+    std::vector<const void*> sources((size_t)count, s->d_filtered);  // every hypothesis reads the one filtered scan in place
+    std::vector<size_t> sizes((size_t)count, s->n_filtered);
+    rc = b200reg_ndt_align_batch_device(reg, count, sources.data(), sizes.data(), guesses, results);
+    if (rc != B200REG_OK) {
+      s->err = std::string("localize_init: ") + b200reg_last_error(reg);
+      return rc;
+    }
+    int pick = -1;
+    for (int k = 0; k < count; k++)
+      if (results[k].status == B200REG_OK && results[k].converged &&
+          (pick < 0 || results[k].trans_probability > results[pick].trans_probability))
+        pick = k;
+    if (pick >= 0) adopt_pose(s, results[pick].final_T);
+    if (best) *best = pick;
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_localize_stats(b200sm_t s, b200sm_localize_stats* out) {
+  if (!s || !out) return B200REG_ERR_ARG;
+  out->n_map = s->n_prior;
+  out->n_cut = s->have_cut ? s->n_cut : 0;
+  out->n_target = s->n_cut_target;
+  out->cut_centre[0] = s->cut_centre[0];
+  out->cut_centre[1] = s->cut_centre[1];
+  out->dist_from_centre = s->dist_from_centre;
+  out->n_cuts = s->n_cuts;
+  out->cut_pending = s->cut_pending ? 1 : 0;
+  return B200REG_OK;
+}
+
+int b200sm_get_cut(b200sm_t s, float* out_xyzi, size_t capacity, size_t* n) {
+  if (!s) return B200REG_ERR_ARG;
+  return sm_guarded(s, [&]() { return read_back(s, s->cut.ptr, s->have_cut ? s->n_cut : 0, out_xyzi, capacity, n); });
 }
 
 }  // extern "C"

@@ -71,6 +71,69 @@ class ScanMatcher:
                                                    _ptr(pose), _ptr(fin), C.byref(upd)))
         return pose, fin.reshape(4, 4).T.copy(), bool(upd.value)
 
+    # ---- localisation in a prior map (b200sm_set_prior_map*, b200sm_localize_*) ----
+    def setPriorMap(self, cloud) -> int:
+        """The map to localise in, from host rows (x, y, z[, intensity]); it stays on the device. Returns its points."""
+        p = _as_cloud(cloud)
+        n, w = p.shape
+        self._check(self._lib.b200sm_set_prior_map(self._h, _ptr(p), n, 4 * w, 12 if w >= 4 else -1))
+        return n
+
+    def setPriorMapPCD(self, path) -> int:
+        """The map to localise in, from a PCD file (e.g. the one saveMapPCDASCII wrote), parsed onto the device. Returns
+        POINTS. A file that cannot be read or parsed raises with ERR_IO / ERR_FORMAT and leaves the previous map."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_set_prior_map_pcd(self._h, os.fsencode(path), C.byref(n)))
+        return int(n.value)
+
+    def setLocalizationParams(self, crop_radius: float, recrop_distance: float):
+        """Horizontal radius of the target cut around the pose, and how far the pose may move from the cut's centre before
+        the target is cut again. Keep crop_radius >= scan_max_range + recrop_distance."""
+        self._check(self._lib.b200sm_set_localization_params(self._h, float(crop_radius), float(recrop_distance)))
+
+    def localizeCloud(self, points):
+        """One frame registered against the cut of the prior map around the pose (b200sm_localize_cloud). Returns
+        (pose7 = position + quaternion xyzw, final 4x4, target_recut)."""
+        p = _as_cloud(points)
+        n, w = p.shape
+        pose = np.zeros(7, dtype=np.float64)
+        fin = np.zeros(16, dtype=np.float32)
+        recut = C.c_int(0)
+        self._check(self._lib.b200sm_localize_cloud(self._h, self.registration._h, _ptr(p), n, 4 * w, 12 if w >= 4 else -1,
+                                                    _ptr(pose), _ptr(fin), C.byref(recut)))
+        return pose, fin.reshape(4, 4).T.copy(), bool(recut.value)
+
+    def localizeInit(self, points, guesses):
+        """The initial pose from several hypotheses (NDT): `guesses` (K, 4, 4) registered in one batch launch against the
+        cut around the current position; the converged one with the highest transformation probability becomes the pose.
+        Returns (best index or -1, list of per-guess dicts: final, trans_probability, converged, iterations, status)."""
+        p = _as_cloud(points)
+        n, w = p.shape
+        G = np.ascontiguousarray(np.asarray(guesses, dtype=np.float32).reshape(-1, 4, 4).transpose(0, 2, 1))
+        res = (_capi.BatchResult * len(G))()
+        best = C.c_int(-1)
+        self._check(self._lib.b200sm_localize_init(self._h, self.registration._h, _ptr(p), n, 4 * w, 12 if w >= 4 else -1,
+                                                   _ptr(G), len(G), res, C.byref(best)))
+        rows = [{"final": np.array(r.final_T, dtype=np.float32).reshape(4, 4).T.copy(),
+                 "trans_probability": float(r.trans_probability), "converged": bool(r.converged),
+                 "iterations": int(r.iterations), "status": int(r.status)} for r in res]
+        return int(best.value), rows
+
+    def localizeStats(self) -> dict:
+        st = _capi.SmLocalizeStats()
+        self._check(self._lib.b200sm_get_localize_stats(self._h, C.byref(st)))
+        out = {k: getattr(st, k) for k, _ in _capi.SmLocalizeStats._fields_}
+        out["cut_centre"] = (float(st.cut_centre[0]), float(st.cut_centre[1]))
+        return out
+
+    def cutCloud(self) -> np.ndarray:
+        """The current cut of the prior map, in map order (the newest cut: pending or already the target)."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_get_cut(self._h, None, 0, C.byref(n)))
+        out = np.empty((n.value, 4), dtype=np.float32)
+        self._check(self._lib.b200sm_get_cut(self._h, _ptr(out), n.value, C.byref(n)))
+        return out
+
     # ---- the pieces, for callers that drive the steps themselves ----
     def setScan(self, points) -> int:
         p = _as_cloud(points)
