@@ -167,4 +167,49 @@ __device__ __forceinline__ int lookup_cell_fast(float x, float leaf, float inv_l
   return (int)floorf(q);
 }
 
+// Radius neighbourhood (VoxelGridCovariance::radiusSearch, voxel_grid_covariance_omp.h:470-499: every voxel centroid c
+// with un-fused f32 |c - x|^2 < f32(res^2)). The cells to probe on one axis are derived from the BUILD rule, not from
+// the query's lookup cell: floor(x / leaf) and the builder's floor(x * inv_leaf) disagree near a cell face, so a hit
+// can lie two lookup cells away from the query. A centroid that passes the test is within res (1 + 2^-22) of x on each
+// axis; the voxel's points (whose build cell names the voxel) are within a few ulp of their f32 centroid, so within
+// reach = res (1 + 2^-20) + 2^-21 |x| of x. floor(fl(y * inv_leaf)) is non-decreasing in y, so the voxel's cell on
+// this axis lies in [build(x - reach) rounded down, build(x + reach) rounded up]: three cells, four near a face.
+// Returns false (no neighbour on any axis) when the range misses the grid or x is not finite; the float clamps
+// before the int conversion keep huge coordinates from overflowing it.
+__device__ __forceinline__ bool radius_cell_range(float x, float res, float inv_leaf, int min_b, int max_b, int& lo, int& hi) {
+  const float reach = __fmaf_ru(fabsf(x), 0x1p-21f, __fmul_ru(res, 1.0f + 0x1p-20f));
+  float fl = floorf(__fmul_rn(__fsub_rd(x, reach), inv_leaf));
+  float fh = floorf(__fmul_rn(__fadd_ru(x, reach), inv_leaf));
+  if (!(fh >= (float)min_b && fl <= (float)max_b)) return false;  // also false for NaN and +-inf
+  lo = max((int)fmaxf(fl, (float)min_b), min_b);
+  hi = min((int)fminf(fh, (float)max_b), max_b);
+  return lo <= hi;
+}
+
+// Visits the record index of every voxel whose f32 centroid passes the radius test of xt (f(r)), z-y-x ascending.
+template <bool STAGED, typename F>
+__device__ __forceinline__ void for_radius_voxels(const GridGeom& g, const RankWord* __restrict__ idx, const float4* centroids,
+                                                  float res, float radius2, float3 xt, F&& f) {
+  int lo[3], hi[3];
+  if (!radius_cell_range(xt.x, res, g.inv_leaf, g.min_b[0], g.max_b[0], lo[0], hi[0]) ||
+      !radius_cell_range(xt.y, res, g.inv_leaf, g.min_b[1], g.max_b[1], lo[1], hi[1]) ||
+      !radius_cell_range(xt.z, res, g.inv_leaf, g.min_b[2], g.max_b[2], lo[2], hi[2]))
+    return;
+  for (int k = lo[2]; k <= hi[2]; k++)
+    for (int j = lo[1]; j <= hi[1]; j++)
+      for (int i = lo[0]; i <= hi[0]; i++) {
+        const int lin = (i - g.min_b[0]) + (j - g.min_b[1]) * g.mul[1] + (k - g.min_b[2]) * g.mul[2];
+        uint2 w;
+        if (STAGED) w = *reinterpret_cast<const uint2*>(idx + (lin >> 5));
+        else w = __ldg(reinterpret_cast<const uint2*>(idx + (lin >> 5)));
+        unsigned r;
+        if (!rank_probe(w, lin & 31, r)) continue;
+        const float4 c = __ldg(centroids + r);
+        const float ex = __fsub_rn(xt.x, c.x), ey = __fsub_rn(xt.y, c.y), ez = __fsub_rn(xt.z, c.z);
+        const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez));
+        if (!(d2 < radius2)) continue;
+        f((int)r);
+      }
+}
+
 }  // namespace b200

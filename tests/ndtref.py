@@ -8,9 +8,10 @@ What is computed
   * transformed point: the solver's f32 transform, ((T0 x + T1 y) + T2 z) + T3 un-fused. The reference transforms in float
     too (pcl::transformPointCloud), so this is ground truth, not an approximation; cells and hits follow from it exactly.
   * neighbourhood: the cell floor(f32(x) / f32(leaf)) (gridref.lookup_ref), then DIRECT7: centre plus the six face
-    neighbours, DIRECT1: centre, DIRECT26: the 26 cells around the centre without it, KDTREE: the 27 cells, keeping a voxel
-    when the un-fused f32 squared distance to its centroid is below f32(res^2). Every neighbour is tested against the grid
-    bounds per axis.
+    neighbours, DIRECT1: centre, DIRECT26: the 26 cells around the centre without it; every neighbour is tested against
+    the grid bounds per axis. KDTREE has no cells: every voxel whose centroid's un-fused f32 squared distance is below
+    f32(res^2) (radiusref.neighbours). It is not confined to the 27 cells around the lookup cell: the builder's cell
+    floor(x * inv_leaf) and the lookup's floor(x / leaf) disagree near a face, so a hit can lie two lookup cells away.
   * each pair in float64: x' = f64(x_t) - mean, C = f64(f32(icov)), s = C x', q = x'^T s, ex = exp(-d2 q / 2),
     e2 = d2 ex, score increment -d1 ex, the pair dropped (score included) when e2 > 1, e2 < 0 or NaN, e = d1 e2;
     gradient e s^T J_k, Hessian e (-d2 (s^T J_i)(s^T J_j) + s^T H_ij + J_i^T C J_j). d1 is float64, d2 the float32 value
@@ -34,8 +35,8 @@ The bound
       with d1 rounded to float: 8 + 2 |d2 q / 2|.
     * the angle tables: the f32 table values are the definition of the live path (both sides multiply with them), so they
       add nothing beyond the f32 products J x and H_ij x, which are counted in gamma.
-  gamma, the depth of the f32 sums an entry passes through: the pairs of a point (up to 27: DIRECT7 7, DIRECT1 1, DIRECT26 26,
-  KDTREE 27), the per-point J / H_E products (j = table . x, three terms, W = M - d2 Q, W J, J^T W J, s^T H_ij: 10), the
+  gamma, the depth of the f32 sums an entry passes through: the pairs of a point (DIRECT7 7, DIRECT1 1, DIRECT26 26,
+  KDTREE 27 or the most any point of the scan has), the per-point J / H_E products (j = table . x, three terms, W = M - d2 Q, W J, J^T W J, s^T H_ij: 10), the
   points one thread accumulates (one per 768 staged points, more than one above the staging capacity), and the 4-term
   f32 pre-sum of the warp reduction (2). Everything after that is float64, fixed order, and a few 2^-53 at most.
   The oracle (one f32 contribution per pair, summed in float64) stays inside the same bound: its per-pair product depth
@@ -151,9 +152,12 @@ def points_per_thread(n_src, n_sms):
 
 def _pairs(xt, g, res, method, vidx, centroid):
     """(point, voxel) candidate pairs of the neighbourhood rule; near: pairs within 4 ulp of the KDTREE radius."""
+    if method == KDTREE:  # every centroid, no cells (radiusref.neighbours)
+        import radiusref
+
+        return radiusref.neighbours(xt, res, dict(idx=vidx, centroid=centroid))
     ijk = np.stack([R.lookup_ref(xt[:, a], res) for a in range(3)], axis=1) - g["min_b"]
-    r2 = F32(float(F32(res)) ** 2)
-    P, V, near = [], [], 0
+    P, V = [], []
     for o in offsets(method):
         c = ijk + np.array(o)
         inside = ((c >= 0) & (c < g["div_b"])).all(axis=1)
@@ -161,16 +165,9 @@ def _pairs(xt, g, res, method, vidx, centroid):
         lin = c[pi, 0] + c[pi, 1] * g["mul"][1] + c[pi, 2] * g["mul"][2]
         k = np.minimum(np.searchsorted(vidx, lin), len(vidx) - 1)
         hit = vidx[k] == lin
-        pi, vi = pi[hit], k[hit]
-        if method == KDTREE:
-            d = xt[pi] - centroid[vi]
-            d2 = (d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2]
-            near += int((np.abs(d2.astype(np.float64) - float(r2)) <= 4 * float(np.spacing(r2))).sum())
-            keep = d2 < r2
-            pi, vi = pi[keep], vi[keep]
-        P.append(pi)
-        V.append(vi)
-    return np.concatenate(P), np.concatenate(V), near
+        P.append(pi[hit])
+        V.append(k[hit])
+    return np.concatenate(P), np.concatenate(V), 0
 
 
 def derivatives(src, T, p6, res, voxels, geom, method=DIRECT7, outlier_ratio=0.55, compute_hessian=True,
@@ -186,7 +183,12 @@ def derivatives(src, T, p6, res, voxels, geom, method=DIRECT7, outlier_ratio=0.5
     mean = np.asarray(voxels["mean"], dtype=np.float64)
     C_all = np.asarray(voxels["icov"], dtype=np.float64).astype(F32).astype(np.float64)
     cen = np.asarray(voxels["centroid"], dtype=F32)
-    gamma = MAX_PAIRS[method] + JH_DEPTH + points_per_thread(len(src), n_sms) + PRESUM_DEPTH
+    max_pairs = MAX_PAIRS[method]
+    if method == KDTREE and len(vidx):  # a radius neighbourhood can exceed 27 voxels (it spans up to 4 cells per axis)
+        for lo in range(0, len(src), chunk):
+            pi = _pairs(transform_points(T, src[lo:lo + chunk]), geom, res, method, vidx, cen)[0]
+            max_pairs = max(max_pairs, int(np.bincount(pi).max()) if len(pi) else 0)
+    gamma = max_pairs + JH_DEPTH + points_per_thread(len(src), n_sms) + PRESUM_DEPTH
     out = dict(score=0.0, g=np.zeros(6), H=np.zeros((6, 6)), hits=0, near_threshold=0, tol_score=0.0,
                tol_g=np.zeros(6), tol_H=np.zeros((6, 6)))
     if len(vidx) == 0:

@@ -134,3 +134,19 @@ def test_ladder_sizes_hit_their_edges():
             assert np.bincount(rank * 768 + tid).max() == per_thread[n]
         assert N.point_owner(128 * n_eval, sms)[2] == n_eval and N.point_owner(128 * (n_eval - 1), sms)[2] == n_eval - 1
         assert 33 % 32 and (cap + 33) % 32  # ragged last units
+
+
+def test_kdtree_reaches_a_voxel_two_lookup_cells_away(oracle_mod):
+    """KDTREE is a radius search over every centroid: on an escape fixture (a wall on a build-cell face, the query two
+    lookup cells below it, inside the radius) the reference and the oracle both score the wall voxel."""
+    import radiusref as RR
+
+    for axis in range(3):
+        tgt, q, *_ = RR.escape_fixture(0.3, axis, 1)
+        o = _oracle_ndt(oracle_mod, q, tgt, 0.3, N.KDTREE)
+        v, geom = o.voxels(), R.leaf_geometry(tgt, 0.3)
+        eye = np.eye(4, dtype=F32)
+        ref = N.derivatives(q, eye[:3], np.zeros(6), 0.3, v, geom, N.KDTREE)
+        assert ref["hits"] == 1 and ref["near_threshold"] == 0, axis
+        assert N.within(o.derivatives(eye, np.zeros(6), True), ref, scale=2.0)["max"] <= 1.0, axis
+        assert ref["score"] != 0
