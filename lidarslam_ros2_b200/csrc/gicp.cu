@@ -53,12 +53,22 @@ __device__ __forceinline__ void sym_eig_smallest(const double* c6, double* u3) {
     B200_ROT(a11, a22, a12, a01, a02, 1, 2)
 #undef B200_ROT
   }
-  // JacobiSVD orders singular values (= |eigenvalues|) descending; the last column of U belongs to the smallest
-  const double e0 = fabs(a00), e1 = fabs(a11), e2 = fabs(a22);
-  int m = 0;
-  double em = e0;
-  if (e1 < em) { em = e1; m = 1; }
-  if (e2 < em) { em = e2; m = 2; }
+  // JacobiSVD orders singular values (= |eigenvalues|) descending; the last column of U belongs to the smallest. Its
+  // selection sort takes the first maximum of the remaining values, swaps only when that is not already in place and
+  // stops at a zero maximum; at exact ties (an unrotated diagonal, zero included) that decides which column is last.
+  double s[3] = {fabs(a00), fabs(a11), fabs(a22)};
+  int col[3] = {0, 1, 2};
+  for (int i = 0; i < 2; i++) {
+    int p = i;
+    for (int j = i + 1; j < 3; j++)
+      if (s[j] > s[p]) p = j;
+    if (s[p] == 0.0) break;
+    if (p != i) {
+      const double ts = s[i]; s[i] = s[p]; s[p] = ts;
+      const int tc = col[i]; col[i] = col[p]; col[p] = tc;
+    }
+  }
+  const int m = col[2];
   u3[0] = v[0 * 3 + m];
   u3[1] = v[1 * 3 + m];
   u3[2] = v[2 * 3 + m];
@@ -121,8 +131,7 @@ __global__ void __launch_bounds__(128) gicp_cov_kernel(NnView V, const float4* _
           if (bd[s] > worst || (bd[s] == worst && bi[s] > worst_idx)) { worst = bd[s]; worst_idx = bi[s]; worst_slot = s; }
       }
     });
-    const float bound = (float)r * g.h;
-    if (cnt == k && worst <= bound * bound * 0.99999f) break;
+    if (cnt == k && worst <= nn_ring_b2(g, r)) break;
   }
   // mean / covariance of the k neighbours in f64 (gicp_omp_impl.hpp:82-107); the sum order follows ascending
   // (d2, index) like nearestKSearch's sorted result

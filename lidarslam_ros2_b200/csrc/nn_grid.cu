@@ -4,7 +4,8 @@
 // apps/align.cpp:37) and by GICP's searchForNeighbors (gicp_omp.h:340-347).
 //
 // Exactness: cells are visited in Chebyshev rings around the query's cell; after ring r every unvisited point is at
-// least r*h away, so the search stops as soon as best_d2 <= (r*h)^2 (with a conservative float margin). Squared
+// least (r - delta)*h away, delta covering the f32 cell assignment, so the search stops as soon as best_d2 is within that
+// radius (nn_ring_b2 in nn_search.cuh, with a conservative float margin). Squared
 // distances are accumulated in f32 exactly like FLANN's L2_Simple, ((dx*dx + dy*dy) + dz*dz), un-fused; ties go to
 // the lower point index.
 #include <cfloat>

@@ -36,6 +36,20 @@ __device__ __forceinline__ int nn_cell_coord(float v, float o, float inv_h, int 
   return max(0, min(dim - 1, c));
 }
 
+// The squared radius a ring search may trust after ring r: every point in a cell outside ring r is farther than it, and
+// its f32 d2 is larger. Cells come from floor(fl(fl(v - o) * inv_h)), whose cell coordinate s' differs from the exact
+// (v - o) / h by at most 3 * 2^-24 * |s| (three roundings). A point two rings out is only r - e_p - e_q cells away,
+// with e_p <= 3 * 2^-24 * D for a grid point (s <= D, the largest dimension) and the same for the query: a query
+// clamped into the grid is farther than its clamped cell says, and one inside has |s| <= D. So after ring r every
+// unvisited point is at least (r - delta) h away with delta = D * 2^-20 (> 6 * 2^-24 D with room for the second-order
+// terms). The factor 0.99999 keeps the bound below the f32 d2 of such a point, which rounds at most 5 * 2^-24 low.
+// (r h)^2 alone is wrong on long axes: at cell 513 of a 1 130-cell grid a point two cells away can be closer than h.
+__device__ __forceinline__ float nn_ring_b2(const NnGeom& g, int r) {
+  const float delta = (float)max(g.dims[0], max(g.dims[1], g.dims[2])) * 0x1p-20f;
+  const float bound = fmaxf((float)r - delta, 0.f) * g.h;
+  return bound * bound * 0.99999f;
+}
+
 // FLANN L2_Simple: ((dx*dx + dy*dy) + dz*dz) in f32, un-fused
 __device__ __forceinline__ float nn_dist2(float qx, float qy, float qz, float4 t) {
   const float dx = __fsub_rn(qx, t.x), dy = __fsub_rn(qy, t.y), dz = __fsub_rn(qz, t.z);
@@ -111,9 +125,7 @@ __device__ __forceinline__ bool nn1_search(const NnView& V, float qx, float qy, 
         }
       }
     }
-    // after ring r every unvisited point is >= r*h away from the query
-    const float bound = (float)r * g.h;
-    const float b2 = bound * bound * 0.99999f;
+    const float b2 = nn_ring_b2(g, r);  // every unvisited point has a larger d2
     if (best_i >= 0 && best <= b2) return true;
     if (b2 > max_d2) return true;  // nothing within the caller's radius remains unvisited
   }

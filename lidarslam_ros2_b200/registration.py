@@ -422,6 +422,10 @@ class GeneralizedIterativeClosestPoint(_Registration):
     def setMaximumOptimizerIterations(self, n: int):
         self._check(self._lib.b200reg_gicp_set_maximum_optimizer_iterations(self._h, int(n)))
 
+    def setEpsilon(self, eps: float):
+        """gicp_epsilon_ (gicp.h:110): the value the smallest singular value of every point covariance is replaced by."""
+        self._check(self._lib.b200reg_gicp_set_epsilon(self._h, float(eps)))
+
     # ---- parity hooks ----
     def covariances(self, which: str) -> np.ndarray:
         w = 1 if which == "target" else 0

@@ -48,13 +48,17 @@ def test_gicp_covariances_parity(b200, oracle_mod):
     o.set_target(tgt)
     o.set_source(src)
     o.align()
-    for which in ("source", "target"):
+    import covref as CR
+
+    for which, cloud in (("source", src), ("target", tgt)):
         cg, co = g.covariances(which), o.covariances(which)
         assert cg.shape == co.shape
-        err = np.abs(cg - co).max(axis=(1, 2))
-        # exact kNN on both sides; a handful of points have a tie at the k-th neighbour or a nearly isotropic
-        # neighbourhood (the smallest-variance direction is then ill-defined)
-        assert np.mean(err < 1e-6) > 0.995, (which, np.mean(err < 1e-6))
+        # every point: within the per-point bound of the float64 reference where the smallest-variance direction is
+        # determined by the moments, by the projector invariants where it is not (tests/covref.py); the oracle likewise
+        ref, info = CR.reference(cloud, 20)
+        for what, got in (("gpu", cg), ("oracle", co)):
+            bad, _, _ = CR.check(got, ref, info)
+            assert not bad.any(), (which, what, int(bad.sum()), np.flatnonzero(bad)[:5])
 
 
 def test_gicp_align_parity(b200, oracle_mod):
