@@ -191,6 +191,19 @@ int b200reg_get_stats(b200reg_t h, b200reg_stats* out);
  * tables taken at p6[3..5]; out: score, g[6], H[36] row-major. */
 int b200reg_ndt_derivatives(b200reg_t h, const float* T, const double* p6, int compute_hessian, double* score,
                             double* g6, double* H36);
+/* NDT score of `count` rigid poses of the handle's current source against its current target, in one launch.
+ * scores[k] = the score of computeDerivatives (ndt_omp_impl.hpp:179-284) at poses[k] (16 floats, column-major): over the
+ * source points and the voxels of their neighbourhood (the handle's search method: KDTREE, DIRECT26, DIRECT7, DIRECT1), the
+ * sum of -d1 * exp(-d2 * q / 2), with a pair dropped, score included, by the test of :504-505. hits[k] (may be NULL) =
+ * pairs kept. The per-pair arithmetic is the solver's; each point's pairs are summed in f32 in probe order and added to an
+ * f64 sum, so scores[k] agrees with b200reg_ndt_derivatives' score to rounding and hits[k] equals its hit count.
+ * Deterministic: scores[k] and hits[k] depend bit for bit only on poses[k], the two clouds, the resolution, the outlier
+ * ratio and the search method — not on count, on k or on the other poses.
+ * count == 0: B200REG_OK, nothing launched. A GICP handle, count < 0 or a non-finite pose entry: B200REG_ERR_ARG (checked
+ * before anything is launched). No target / no source: B200REG_ERR_NO_TARGET / B200REG_ERR_NO_SOURCE. A target with no
+ * valid voxel: every score and hit count is 0. An ordinary (not cooperative) launch on the handle's stream. The handle
+ * keeps device buffers for the largest count it has scored (80 bytes per pose, grown geometrically) until it is destroyed. */
+int b200reg_ndt_score_poses(b200reg_t h, int count, const float* poses_colmajor16, double* scores, long long* hits);
 /* Hessian-only pass over the radius neighbourhood in f64 (ndt_omp_impl.hpp:538-629) */
 int b200reg_ndt_hessian_radius(b200reg_t h, const float* T, const double* p6, double* H36);
 /* voxel map read-back, voxels with >= 6 points in ascending leaf index (voxel_grid_covariance_omp_impl.hpp:
@@ -526,6 +539,42 @@ int b200sm_localize_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t
 int b200sm_localize_init(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes,
                          long intensity_offset_bytes, const float* guesses, int count, b200reg_batch_result* results,
                          int* best);
+/* Global localisation: the pose found in the prior map without a precise guess (NDT only; a GICP handle is
+ * B200REG_ERR_ARG). (1) The frame is uploaded and the map cut around the current position as in b200sm_localize_init
+ * (upload, cut, VoxelGrid + setInputSource). (2) A grid of (x, y, yaw) hypotheses is built on the host around the current
+ * pose: with K = floor(radius / step), positions (i, j) for j = -K-1 .. K+1 (outer) and i = -K-1 .. K+1 (inner) are kept
+ * when a * a + b * b <= radius * radius (a = (double)i * step, b = (double)j * step, every operation rounded on its own);
+ * hypothesis k = position_index * yaw_steps + m has translation (cx + a, cy + b, z0) (the current position), rotation
+ * Rz(2 pi m / yaw_steps) * R0 (R0: the rotation of the current pose, as sim_trans builds it in double; std::cos / std::sin,
+ * products summed left to right in double), cast to float. z, roll and pitch are not searched: they come from the current
+ * pose and the refinement corrects what remains. (3) Every hypothesis is scored by b200reg_ndt_score_poses on the filtered
+ * scan. (4) The top_k highest scores, in descending score and the lower index first on equal scores, are refined in ONE
+ * batch launch exactly as b200sm_localize_init refines its guesses: candidates[r] = the hypothesis of row r, results[r] =
+ * bitwise what b200sm_localize_init returns for that guess (both arrays need min(top_k, n_hypotheses) rows). The converged
+ * row with the highest trans_probability (the lowest row on a tie) becomes the session's pose; out->best = that row, or -1
+ * (pose unchanged, B200REG_OK). out may be NULL. The caller keeps crop_radius >= radius + scan_max_range (not enforced).
+ * An invalid spec, floor(radius / step) > 4096 or more than 2^24 hypotheses: B200REG_ERR_ARG before anything changes. No
+ * prior map: B200REG_ERR_NO_TARGET. A node with no initial pose, or one that has lost track, calls this once and then
+ * b200sm_localize_cloud frame by frame. */
+typedef struct b200sm_global_search {
+  double radius;   /* finite, >= 0: positions within this horizontal distance of the current position          */
+  double step;     /* finite, > 0: grid spacing                                                                */
+  int yaw_steps;   /* 1..4096: yaw offsets 2*pi*m / yaw_steps, m = 0..yaw_steps-1                              */
+  int top_k;       /* 1..1024: best-scored hypotheses refined in one batch launch                              */
+} b200sm_global_search;
+typedef struct b200sm_global_result {
+  long long n_hypotheses, hits_total;
+  int n_refined;   /* min(top_k, n_hypotheses)                                                                 */
+  int best;        /* refined row adopted as the session's pose, -1 when none converged (pose unchanged)        */
+  float score_ms;  /* device time of the scoring launch (CUDA events around it on the engine's stream)         */
+} b200sm_global_result;
+int b200sm_localize_global(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes,
+                           long intensity_offset_bytes, const b200sm_global_search* spec, int* candidates,
+                           b200reg_batch_result* results, b200sm_global_result* out);
+/* the grid of the last b200sm_localize_global that reached its scoring: *n = its hypotheses; min(capacity, n) rows of poses
+ * (16 floats, column-major), scores and hits; any pointer may be NULL. The session keeps this grid in host memory (80 bytes per
+ * hypothesis, about 1.3 GB at the 2^24 cap) until the next such call or until it is destroyed. */
+int b200sm_get_global_search(b200sm_t s, size_t capacity, size_t* n, float* poses_colmajor16, double* scores, long long* hits);
 int b200sm_get_localize_stats(b200sm_t s, b200sm_localize_stats* out);
 /* read-back of the current cut (the newest one, pending or adopted), like b200sm_get_targeted */
 int b200sm_get_cut(b200sm_t s, float* out_xyzi, size_t capacity, size_t* n);

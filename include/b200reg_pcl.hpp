@@ -140,6 +140,13 @@ class NormalDistributionsTransform : public Registration {
     b200reg_ndt_get_final_num_iteration(h_.get(), &v);
     return v;
   }
+  // NDT score of the current source at poses.size() / 16 poses (column-major 4x4 each) against the current target, in one
+  // launch (b200reg_ndt_score_poses); scores and hits get one entry per pose
+  void scorePoses(const std::vector<float>& poses, std::vector<double>& scores, std::vector<long long>& hits) {
+    scores.resize(poses.size() / 16);
+    hits.resize(scores.size());
+    check(b200reg_ndt_score_poses(h_.get(), (int)scores.size(), poses.data(), scores.data(), hits.data()));
+  }
 };
 
 class GeneralizedIterativeClosestPoint : public Registration {
@@ -279,6 +286,13 @@ class NormalDistributionsTransform : public RegistrationBase<PointSource, PointT
     int v = 0;
     b200reg_ndt_get_final_num_iteration(this->h_.get(), &v);
     return v;
+  }
+  // b200reg_ndt_score_poses, as in the stand-alone class; false (reported on stderr) when the call is refused
+  bool scorePoses(const std::vector<float>& poses, std::vector<double>& scores, std::vector<long long>& hits) {
+    scores.resize(poses.size() / 16);
+    hits.resize(scores.size());
+    return this->report(b200reg_ndt_score_poses(this->h_.get(), (int)scores.size(), poses.data(), scores.data(), hits.data()),
+                        "scorePoses");
   }
 };
 
@@ -424,6 +438,30 @@ class ScanMatcherSession {
     rows.resize(guesses.size() / 16);
     check(b200sm_localize_init(s_.get(), reg, points, n, stride, intensity_offset, guesses.data(), (int)rows.size(), rows.data(), &best));
     return best;
+  }
+  // NDT: the pose without a precise guess (b200sm_localize_global): the (x, y, yaw) grid of `spec` around the current pose
+  // scored in one launch, the best spec.top_k refined in one batch launch; returns the adopted row or -1. candidates[r] = the
+  // hypothesis of row r, rows = one result per refined hypothesis (as localizeInit's), info (optional) = the search's counts
+  int localizeGlobal(b200reg_t reg, const float* points, size_t n, size_t stride, long intensity_offset, const b200sm_global_search& spec,
+                     std::vector<int>& candidates, std::vector<b200reg_batch_result>& rows, b200sm_global_result* info = nullptr) {
+    const size_t k = spec.top_k > 0 ? (size_t)spec.top_k : 1;
+    candidates.assign(k, -1);
+    rows.resize(k);
+    b200sm_global_result r{};
+    check(b200sm_localize_global(s_.get(), reg, points, n, stride, intensity_offset, &spec, candidates.data(), rows.data(), &r));
+    candidates.resize((size_t)r.n_refined);
+    rows.resize((size_t)r.n_refined);
+    if (info) *info = r;
+    return r.best;
+  }
+  // the grid of the last localizeGlobal: 16 floats per hypothesis (column-major), its score and its kept pairs
+  void globalSearch(std::vector<float>& poses, std::vector<double>& scores, std::vector<long long>& hits) {
+    size_t n = 0;
+    check(b200sm_get_global_search(s_.get(), 0, &n, nullptr, nullptr, nullptr));
+    poses.resize(16 * n);
+    scores.resize(n);
+    hits.resize(n);
+    check(b200sm_get_global_search(s_.get(), n, &n, poses.data(), scores.data(), hits.data()));
   }
   b200sm_localize_stats localizeStats() const {
     b200sm_localize_stats st{};

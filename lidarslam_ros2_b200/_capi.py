@@ -46,7 +46,8 @@ SYMBOLS = [
     "b200sm_save_map_pcd_ascii", "b200reg_encode_pcd_ascii", "b200sm_set_sensor_transform", "b200sm_odom_next_scan",
     "b200reg_load_pcd", "b200reg_set_input_target_pcd",
     "b200sm_set_prior_map_pcd", "b200sm_set_prior_map", "b200sm_set_localization_params", "b200sm_localize_cloud",
-    "b200sm_localize_init", "b200sm_get_localize_stats", "b200sm_get_cut",
+    "b200sm_localize_init", "b200sm_get_localize_stats", "b200sm_get_cut", "b200reg_ndt_score_poses",
+    "b200sm_localize_global", "b200sm_get_global_search",
     # include/b200comm.h
     "b200comm_unique_id", "b200comm_create", "b200comm_destroy", "b200comm_all_gather_rows", "b200comm_rank", "b200comm_last_error",
     "b200comm_board_create", "b200comm_board_destroy", "b200comm_board_info",
@@ -81,6 +82,15 @@ class SmLocalizeStats(C.Structure):
 class BatchResult(C.Structure):
     _fields_ = [("final_T", C.c_float * 16), ("trans_probability", C.c_double), ("converged", C.c_int), ("iterations", C.c_int),
                 ("evaluations", C.c_int), ("status", C.c_int), ("hits_total", C.c_longlong)]
+
+
+class SmGlobalSearch(C.Structure):
+    _fields_ = [("radius", C.c_double), ("step", C.c_double), ("yaw_steps", C.c_int), ("top_k", C.c_int)]
+
+
+class SmGlobalResult(C.Structure):
+    _fields_ = [("n_hypotheses", C.c_longlong), ("hits_total", C.c_longlong), ("n_refined", C.c_int), ("best", C.c_int),
+                ("score_ms", C.c_float)]
 
 
 class SweepResult(C.Structure):
@@ -212,6 +222,9 @@ def lib() -> C.CDLL:
     L.b200sm_localize_init.argtypes = [vp, vp, vp, sz, sz, C.c_long, vp, i, vp, C.POINTER(i)]
     L.b200sm_get_localize_stats.argtypes = [vp, C.POINTER(SmLocalizeStats)]
     L.b200sm_get_cut.argtypes = [vp, vp, sz, C.POINTER(sz)]
+    L.b200reg_ndt_score_poses.argtypes = [vp, i, vp, vp, vp]
+    L.b200sm_localize_global.argtypes = [vp, vp, vp, sz, sz, C.c_long, C.POINTER(SmGlobalSearch), vp, vp, C.POINTER(SmGlobalResult)]
+    L.b200sm_get_global_search.argtypes = [vp, sz, C.POINTER(sz), vp, vp, vp]
     L.b200comm_unique_id.argtypes = [vp]
     L.b200comm_create.argtypes = [vp, i, i, i, C.POINTER(vp)]
     L.b200comm_destroy.argtypes = [vp]

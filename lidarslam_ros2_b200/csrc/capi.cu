@@ -88,6 +88,12 @@ struct b200reg_engine {
   unsigned batch_tag = 0;                // value the flags take for the current call
   b200reg_engine* siblings[3] = {nullptr, nullptr, nullptr};  // further engines of b200reg_ndt_sweep (own stream and buffers each)
   int sweep_engines = 4;  // engines (host threads) the sweep pipelines over (developer switch: B200REG_SWEEP_ENGINES)
+
+  // b200reg_ndt_score_poses
+  DeviceBuffer<float> d_poses;
+  DeviceBuffer<double> d_pose_scores;
+  DeviceBuffer<long long> d_pose_hits;
+  float score_ms = 0;  // device time of the last scoring launch
 };
 
 namespace {
@@ -760,6 +766,44 @@ int b200reg_ndt_derivatives(b200reg_t h, const float* T, const double* p6, int c
     return (int)B200REG_OK;
   });
 }
+
+int b200reg_ndt_score_poses(b200reg_t h, int count, const float* poses_colmajor16, double* scores, long long* hits) {
+  if (!h || h->kind != B200REG_NDT || count < 0) return B200REG_ERR_ARG;
+  if (count == 0) return B200REG_OK;
+  if (!poses_colmajor16 || !scores) return B200REG_ERR_ARG;
+  for (size_t i = 0; i < (size_t)count * 16; i++)
+    if (!std::isfinite(poses_colmajor16[i])) return fail(h, B200REG_ERR_ARG, "score_poses: a pose entry is not finite");
+  return guarded(h, [&]() {
+    if (!h->have_target) return fail(h, B200REG_ERR_NO_TARGET, "no input target");
+    if (!h->have_source) return fail(h, B200REG_ERR_NO_SOURCE, "no input source");
+    ensure_map(h);
+    h->score_ms = 0;
+    if (h->map.n_voxels == 0) {
+      std::memset(scores, 0, (size_t)count * sizeof(double));
+      if (hits) std::memset(hits, 0, (size_t)count * sizeof(long long));
+      return (int)B200REG_OK;
+    }
+    h->d_poses.ensure((size_t)count * 16);
+    h->d_pose_scores.ensure((size_t)count);
+    h->d_pose_hits.ensure((size_t)count);
+    B200_CUDA(cudaMemcpyAsync(h->d_poses.ptr, poses_colmajor16, (size_t)count * 16 * sizeof(float), cudaMemcpyHostToDevice,
+                              h->stream));
+    B200_CUDA(cudaEventRecord(h->ev0, h->stream));
+    ndt_score_poses(h->map, h->src_view, h->n_source, h->ndt, h->d_poses.ptr, count, h->d_pose_scores.ptr, h->d_pose_hits.ptr,
+                    h->stream);
+    B200_CUDA(cudaEventRecord(h->ev1, h->stream));
+    h->other_launches += 1;
+    B200_CUDA(cudaMemcpyAsync(scores, h->d_pose_scores.ptr, (size_t)count * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    if (hits)
+      B200_CUDA(cudaMemcpyAsync(hits, h->d_pose_hits.ptr, (size_t)count * sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
+    B200_CUDA(cudaStreamSynchronize(h->stream));
+    B200_CUDA(cudaEventElapsedTime(&h->score_ms, h->ev0, h->ev1));
+    return (int)B200REG_OK;
+  });
+}
+
+// library-internal (the scan-matcher session's b200sm_global_result::score_ms): device time of the last scoring launch
+extern "C" float b200reg_last_score_ms(b200reg_t h) { return h ? h->score_ms : 0.0f; }
 
 int b200reg_ndt_hessian_radius(b200reg_t h, const float* T, const double* p6, double* H36) {
   if (!h || h->kind != B200REG_NDT || !T || !p6 || !H36) return B200REG_ERR_ARG;

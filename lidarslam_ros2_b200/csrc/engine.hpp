@@ -325,6 +325,10 @@ void ndt_hessian_radius(const VoxelMap& map, const float4* src, size_t n, const 
                         const double* d_jd, const double* d_hd, double* d_out21, cudaStream_t s);
 void ndt_hessian_into_state(const double* d_upper21, NdtSolverWork* work, cudaStream_t s);
 void ndt_score(const VoxelMap& map, const float4* cloud, size_t n, const NdtConfig& cfg, double* d_out1, cudaStream_t s);
+// K12 (ndt_score.cu): d_scores[k] / d_hits[k] = NDT score and kept pairs of `count` column-major poses (d_poses, 16 floats
+// each, device memory) of src against map; enqueue only. The map must hold at least one voxel.
+void ndt_score_poses(const VoxelMap& map, const float4* src, size_t n_src, const NdtConfig& cfg, const float* d_poses, int count,
+                     double* d_scores, long long* d_hits, cudaStream_t s);
 // out = T * in, xyz in f32 (transform_point), w copied
 void transform_cloud_device(const float4* in, size_t n, float4* out, const Mat34f& T, cudaStream_t s);
 

@@ -1,4 +1,4 @@
-// Device-side structures shared by the NDT solver kernels (ndt_solver.cu, ndt_aux.cu).
+// Device-side structures and per-pair helpers shared by the NDT kernels (ndt_solver.cu, ndt_aux.cu, ndt_score.cu).
 #pragma once
 #include "../../include/b200reg.h"
 #include "common.cuh"
@@ -154,6 +154,68 @@ __device__ __forceinline__ int probe_cell(const GridGeom& g, const RankWord* __r
   unsigned r;
   if (!rank_probe(w, lin & 31, r)) return -1;
   return (int)r;
+}
+
+// rank-index probe of a leaf index known to be inside the grid
+// (idx points either at the shared-memory copy staged by TMA or at the global table)
+__device__ __forceinline__ int probe_lin(const RankWord* __restrict__ idx, int lin) {
+  unsigned r;
+  if (!rank_probe(*reinterpret_cast<const uint2*>(idx + (lin >> 5)), lin & 31, r)) return -1;
+  return (int)r;
+}
+
+struct PairSums {  // sums over the voxels hit by one point
+  float S0, S1, S2;                    // sum e * s,           s = C x'
+  float M00, M01, M02, M11, M12, M22;  // sum e * C
+  float Q00, Q01, Q02, Q11, Q12, Q22;  // sum e * s s^T
+  float score;                         // sum of the f32 score increments of this point
+  int hits;
+};
+
+struct Rec {
+  float4 a, b, c;
+};
+__device__ __forceinline__ Rec load_record(const VoxelRecord* __restrict__ rec) {
+  Rec r;
+  const float4* p = reinterpret_cast<const float4*>(rec);
+  r.a = __ldg(p);
+  r.b = __ldg(p + 1);
+  r.c = __ldg(p + 2);
+  return r;
+}
+
+// one (point, voxel) pair — updateDerivatives (ndt_omp_impl.hpp:482-535) reduced to its per-pair core.
+// Branch-free: a probe that missed reads record 0 and is masked out, so that the compiler may keep the loads and
+// the arithmetic of several pairs in flight. All f32: the reference forms score_inc = float(-d1 * e) and
+// e' = float(e * d1) through a double product (:499, :508); multiplying by float(d1) instead differs by at most one
+// f32 ulp (6e-8 relative), far below the f32 noise of the per-pair products themselves.
+template <bool HESS>
+__device__ __forceinline__ void accumulate_pair(const Rec& R, bool valid, float3 xt, float d1f, float gd2, PairSums& ps) {
+  const float c00 = R.b.z, c01 = R.b.w, c02 = R.c.x, c11 = R.c.y, c12 = R.c.z, c22 = R.c.w;
+  // x' = x_trans - mean (float-float mean: within one ulp of the reference's f64 subtraction + cast, :259-262, :490)
+  const float x0 = __fsub_rn(__fsub_rn(xt.x, R.a.x), R.a.w);
+  const float x1 = __fsub_rn(__fsub_rn(xt.y, R.a.y), R.b.x);
+  const float x2 = __fsub_rn(__fsub_rn(xt.z, R.a.z), R.b.y);
+  const float s0 = c00 * x0 + c01 * x1 + c02 * x2;
+  const float s1 = c01 * x0 + c11 * x1 + c12 * x2;
+  const float s2 = c02 * x0 + c12 * x1 + c22 * x2;
+  const float q = x0 * s0 + x1 * s1 + x2 * s2;
+  const float ex = expf(-gd2 * q * 0.5f);  // :497
+  const float e2 = gd2 * ex;               // :501
+  const bool ok = valid && !(e2 > 1.0f || e2 < 0.0f || e2 != e2);  // :504-505 (the score increment is dropped too)
+  const float e = ok ? e2 * d1f : 0.0f;    // :508
+  ps.score += ok ? -d1f * ex : 0.0f;       // :499
+  ps.hits += ok ? 1 : 0;
+  ps.S0 += e * s0;
+  ps.S1 += e * s1;
+  ps.S2 += e * s2;
+  if (HESS) {
+    ps.M00 += e * c00; ps.M01 += e * c01; ps.M02 += e * c02;
+    ps.M11 += e * c11; ps.M12 += e * c12; ps.M22 += e * c22;
+    const float es0 = e * s0, es1 = e * s1, es2 = e * s2;
+    ps.Q00 += es0 * s0; ps.Q01 += es0 * s1; ps.Q02 += es0 * s2;
+    ps.Q11 += es1 * s1; ps.Q12 += es1 * s2; ps.Q22 += es2 * s2;
+  }
 }
 
 // lookup cell of a transformed point: floor(x / leaf) with an IEEE division (impl.hpp:379-381)

@@ -31,6 +31,7 @@
 #include "../../include/b200reg.h"
 #include "deskew.hpp"
 #include "engine.hpp"
+#include "global_grid.hpp"
 #include "map_cut.hpp"
 #include "pose_graph.hpp"
 #include "sensor_frame.hpp"
@@ -222,6 +223,7 @@ __global__ void __launch_bounds__(ASSEMBLE_THREADS) assemble_map_kernel(const As
 using namespace b200;
 
 extern "C" int b200reg_adopt_source_device(b200reg_t h, const void* dev, size_t n);  // capi.cu (library-internal)
+extern "C" float b200reg_last_score_ms(b200reg_t h);                                 // capi.cu (library-internal)
 
 struct b200sm_session {
   int device = 0;
@@ -282,6 +284,10 @@ struct b200sm_session {
   double cut_centre[2] = {0, 0}, dist_from_centre = 0;
   int n_cuts = 0;
   bool have_cut = false, cut_stale = true, cut_pending = false;
+  // the grid of the last b200sm_localize_global: poses (16 floats each, column-major), scores, hits
+  std::vector<float> global_poses;
+  std::vector<double> global_scores;
+  std::vector<long long> global_hits;
 };
 
 namespace {
@@ -1272,6 +1278,28 @@ int ensure_cut_target(b200sm_t s, b200reg_t reg, int kind) {
   return rc;
 }
 
+// step 3 of b200sm_localize_init / b200sm_localize_global: the filtered scan registered from `count` guesses in one batch
+// launch (the scan read in place `count` times); the converged row with the highest trans_probability, the lowest index on
+// a tie, becomes the pose. *best = its index, or -1 when none converged (pose unchanged).
+int refine_hypotheses(b200sm_t s, b200reg_t reg, const float* guesses, int count, b200reg_batch_result* results, int* best,
+                      const char* who) {
+  std::vector<const void*> sources((size_t)count, s->d_filtered);
+  std::vector<size_t> sizes((size_t)count, s->n_filtered);
+  const int rc = b200reg_ndt_align_batch_device(reg, count, sources.data(), sizes.data(), guesses, results);
+  if (rc != B200REG_OK) {
+    s->err = std::string(who) + b200reg_last_error(reg);
+    return rc;
+  }
+  int pick = -1;
+  for (int k = 0; k < count; k++)
+    if (results[k].status == B200REG_OK && results[k].converged &&
+        (pick < 0 || results[k].trans_probability > results[pick].trans_probability))
+      pick = k;
+  if (pick >= 0) adopt_pose(s, results[pick].final_T);
+  if (best) *best = pick;
+  return (int)B200REG_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1375,22 +1403,76 @@ int b200sm_localize_init(b200sm_t s, b200reg_t reg, const float* points, size_t 
     if (rc != B200REG_OK) return rc;
     rc = set_source_from_scan(s, reg);
     if (rc != B200REG_OK) return rc;
-    std::vector<const void*> sources((size_t)count, s->d_filtered);  // every hypothesis reads the one filtered scan in place
-    std::vector<size_t> sizes((size_t)count, s->n_filtered);
-    rc = b200reg_ndt_align_batch_device(reg, count, sources.data(), sizes.data(), guesses, results);
+    return refine_hypotheses(s, reg, guesses, count, results, best, "localize_init: ");
+  });
+}
+
+int b200sm_localize_global(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes,
+                           long intensity_offset_bytes, const b200sm_global_search* spec, int* candidates,
+                           b200reg_batch_result* results, b200sm_global_result* out) {
+  if (!valid_frame_args(s, reg, points, n, stride_bytes, intensity_offset_bytes) || !spec || !candidates || !results)
+    return B200REG_ERR_ARG;
+  int kind = B200REG_NDT;
+  b200reg_get_kind(reg, &kind);
+  if (kind != B200REG_NDT) return sm_fail(s, B200REG_ERR_ARG, "localize_global: the batch solver is NDT's");
+  const long long n_hyp = global_grid_count(spec->radius, spec->step, spec->yaw_steps, spec->top_k);
+  if (n_hyp < 0)
+    return sm_fail(s, B200REG_ERR_ARG, "localize_global: radius must be finite and >= 0, step finite and > 0, yaw_steps in "
+                                       "1..4096, top_k in 1..1024, floor(radius / step) <= 4096 and at most 2^24 hypotheses");
+  return sm_guarded(s, [&]() {
+    if (out) {
+      std::memset(out, 0, sizeof(*out));
+      out->best = -1;
+    }
+    if (s->n_prior == 0) return sm_fail(s, B200REG_ERR_NO_TARGET, "localize_global: no prior map");
+    upload_frame(s, points, n, stride_bytes, intensity_offset_bytes);
+    int rc = ensure_cut_target(s, reg, B200REG_NDT);
+    if (rc != B200REG_OK) return rc;
+    rc = set_source_from_scan(s, reg);
+    if (rc != B200REG_OK) return rc;
+    std::vector<float> poses;
+    global_grid_build(s->position, s->quat, spec->radius, spec->step, spec->yaw_steps, poses);
+    std::vector<double> scores((size_t)n_hyp);
+    std::vector<long long> hits((size_t)n_hyp);
+    rc = b200reg_ndt_score_poses(reg, (int)n_hyp, poses.data(), scores.data(), hits.data());
     if (rc != B200REG_OK) {
-      s->err = std::string("localize_init: ") + b200reg_last_error(reg);
+      s->err = std::string("localize_global: ") + b200reg_last_error(reg);
       return rc;
     }
-    int pick = -1;
-    for (int k = 0; k < count; k++)
-      if (results[k].status == B200REG_OK && results[k].converged &&
-          (pick < 0 || results[k].trans_probability > results[pick].trans_probability))
-        pick = k;
-    if (pick >= 0) adopt_pose(s, results[pick].final_T);
-    if (best) *best = pick;
-    return (int)B200REG_OK;
+    const float score_ms = b200reg_last_score_ms(reg);
+    const std::vector<int> top = global_select_top_k(scores.data(), n_hyp, spec->top_k);
+    const int k = (int)top.size();
+    std::vector<float> guesses((size_t)k * 16);
+    for (int r = 0; r < k; r++) {
+      candidates[r] = top[r];
+      std::memcpy(guesses.data() + (size_t)r * 16, poses.data() + (size_t)top[r] * 16, 16 * sizeof(float));
+    }
+    long long hits_total = 0;
+    for (long long h : hits) hits_total += h;
+    s->global_poses.swap(poses);
+    s->global_scores.swap(scores);
+    s->global_hits.swap(hits);
+    int best = -1;
+    rc = refine_hypotheses(s, reg, guesses.data(), k, results, &best, "localize_global: ");
+    if (out) {
+      out->n_hypotheses = n_hyp;
+      out->hits_total = hits_total;
+      out->n_refined = k;
+      out->best = best;
+      out->score_ms = score_ms;
+    }
+    return rc;
   });
+}
+
+int b200sm_get_global_search(b200sm_t s, size_t capacity, size_t* n, float* poses_colmajor16, double* scores, long long* hits) {
+  if (!s) return B200REG_ERR_ARG;
+  const size_t total = s->global_scores.size(), m = std::min(capacity, total);
+  if (n) *n = total;
+  if (poses_colmajor16 && m) std::memcpy(poses_colmajor16, s->global_poses.data(), m * 16 * sizeof(float));
+  if (scores && m) std::memcpy(scores, s->global_scores.data(), m * sizeof(double));
+  if (hits && m) std::memcpy(hits, s->global_hits.data(), m * sizeof(long long));
+  return B200REG_OK;
 }
 
 int b200sm_get_localize_stats(b200sm_t s, b200sm_localize_stats* out) {

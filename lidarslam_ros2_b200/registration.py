@@ -363,6 +363,17 @@ class NormalDistributionsTransform(_Registration):
                                                       _ptr(g), _ptr(H)))
         return s.value, g, H
 
+    def scorePoses(self, poses):
+        """NDT score of the current source at each of `poses` ((K, 4, 4)) against the current target, in one launch
+        (b200reg_ndt_score_poses): the score computeDerivatives would give there, and the pairs it kept. Returns (scores
+        float64 (K,), hits int64 (K,)); each entry depends only on its own pose."""
+        P = np.asarray(poses, dtype=np.float32).reshape(-1, 4, 4)
+        G = np.ascontiguousarray(P.transpose(0, 2, 1))
+        scores = np.zeros(len(G), dtype=np.float64)
+        hits = np.zeros(len(G), dtype=np.int64)
+        self._check(self._lib.b200reg_ndt_score_poses(self._h, len(G), _ptr(G), _ptr(scores), _ptr(hits)))
+        return scores, hits
+
     def hessian_radius(self, T, p6) -> np.ndarray:
         Tc = _colmajor(T)
         p = np.ascontiguousarray(p6, dtype=np.float64)

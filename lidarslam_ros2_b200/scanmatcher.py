@@ -119,6 +119,40 @@ class ScanMatcher:
                  "iterations": int(r.iterations), "status": int(r.status)} for r in res]
         return int(best.value), rows
 
+    def localizeGlobal(self, points, radius: float, step: float, yaw_steps: int, top_k: int):
+        """The pose without a precise guess (NDT, b200sm_localize_global): an (x, y, yaw) grid around the current pose —
+        positions within `radius` at spacing `step`, `yaw_steps` headings each — scored on the device in one launch, the
+        `top_k` best refined in one batch launch; the converged one with the highest transformation probability becomes the
+        pose. Returns (best row or -1, candidates (hypothesis index per row), rows as localizeInit's, info dict:
+        n_hypotheses, hits_total, n_refined, score_ms)."""
+        p = _as_cloud(points)
+        n, w = p.shape
+        spec = _capi.SmGlobalSearch(float(radius), float(step), int(yaw_steps), int(top_k))
+        k = max(int(top_k), 1)
+        cand = np.full(k, -1, dtype=np.int32)
+        res = (_capi.BatchResult * k)()
+        out = _capi.SmGlobalResult()
+        self._check(self._lib.b200sm_localize_global(self._h, self.registration._h, _ptr(p), n, 4 * w, 12 if w >= 4 else -1,
+                                                     C.byref(spec), _ptr(cand), res, C.byref(out)))
+        m = out.n_refined
+        rows = [{"final": np.array(r.final_T, dtype=np.float32).reshape(4, 4).T.copy(),
+                 "trans_probability": float(r.trans_probability), "converged": bool(r.converged),
+                 "iterations": int(r.iterations), "status": int(r.status)} for r in res[:m]]
+        info = dict(n_hypotheses=int(out.n_hypotheses), hits_total=int(out.hits_total), n_refined=int(m),
+                    score_ms=float(out.score_ms))
+        return int(out.best), cand[:m].copy(), rows, info
+
+    def globalSearch(self):
+        """The grid of the last localizeGlobal: (poses (H, 4, 4) float32, scores float64 (H,), hits int64 (H,))."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_get_global_search(self._h, 0, C.byref(n), None, None, None))
+        H = n.value
+        poses = np.empty((H, 16), dtype=np.float32)
+        scores = np.empty(H, dtype=np.float64)
+        hits = np.empty(H, dtype=np.int64)
+        self._check(self._lib.b200sm_get_global_search(self._h, H, C.byref(n), _ptr(poses), _ptr(scores), _ptr(hits)))
+        return poses.reshape(H, 4, 4).transpose(0, 2, 1).copy(), scores, hits
+
     def localizeStats(self) -> dict:
         st = _capi.SmLocalizeStats()
         self._check(self._lib.b200sm_get_localize_stats(self._h, C.byref(st)))
