@@ -403,6 +403,48 @@ int b200sm_search_loop_all(b200sm_t s, b200reg_t reg, float voxel_leaf_size, dou
                            int shard_rank, int shard_world, b200sm_loop_result* out, size_t capacity, size_t* n_out,
                            size_t* n_candidates_total);
 
+/* ---- place recognition: a loop search that does not trust the drifted poses (Scan Context, Kim & Kim, IROS 2018) ------
+ * Each submap's cloud (sensor frame) is described by a num_rings x num_sectors grid of the horizontal plane around the
+ * sensor out to max_radius: bin (ring, sector) holds the largest z + lidar_height of its points, 0 when it has none. The
+ * newest descriptor is compared with every older submap's at every column shift, so a revisit is found however far the
+ * odometry has drifted, and the best shift gives the heading to start the registration from. The exact definitions
+ * (bins, norms, distance, guess) are in csrc/scan_context.hpp; DESIGN.md section 7b describes the search.
+ * Descriptors are built on the device at the first b200sm_search_loop_place / b200sm_get_scan_context after submaps were
+ * added, and stay there: num_rings * num_sectors * 4 + num_sectors * 8 bytes per submap.                                */
+typedef struct b200sm_scan_context_params {
+  int num_rings;        /* 1..128, default 20                                                    */
+  int num_sectors;      /* 1..720, default 60; num_rings * num_sectors <= 8192                    */
+  double max_radius;    /* finite, > 0, default 80 (metres, horizontal)                          */
+  double lidar_height;  /* finite, default 2.0: added to z (as a float) before the max           */
+} b200sm_scan_context_params;
+/* NULL: the defaults. B200REG_ERR_ARG for a value out of range (nothing changes). Every cached descriptor is dropped. */
+int b200sm_set_scan_context_params(b200sm_t s, const b200sm_scan_context_params* p);
+/* descriptor of submap `index`, num_rings * num_sectors floats, ring-major (ring i, sector j at i * num_sectors + j);
+ * capacity (floats) must hold all of it */
+int b200sm_get_scan_context(b200sm_t s, size_t index, float* out, size_t capacity);
+
+typedef struct b200sm_place_result {
+  b200sm_loop_result loop;  /* filled exactly as b200sm_search_loop_all fills a row (min_dist = position distance) */
+  double sc_distance;       /* D(newest, candidate)                                                                */
+  int shift;                /* s*: the newest sensor is turned by about 2 pi shift / num_sectors counter-clockwise
+                               relative to the candidate's                                                         */
+  int pad;
+  float guess[16];          /* the initial guess the verification aligned from, column-major                       */
+} b200sm_place_result;
+/* The newest submap against every older one with (travelled-distance gap > distance_loop_closure); there is no position
+ * gate. Those with D < sc_threshold are ranked by (D, id) and the first min(top_k, capacity) are verified exactly like a
+ * b200sm_search_loop_all row, except that align() starts from guess = P_cand * Rz(2 pi s* / num_sectors) * P_new^-1.
+ * An accepted row is the loop edge (loop.id_min, newest, loop.relative_pose) of b200sm_pose_adjust. *n_out = rows
+ * written, *n_scored (may be NULL) = eligible submaps. Fewer than two submaps: B200REG_OK with *n_out = 0.
+ * B200REG_ERR_ARG for top_k outside 1..1024, a non-finite sc_threshold, voxel_leaf_size <= 0, search_submap_num < 0 or
+ * out == NULL with capacity > 0. NDT and GICP handles alike.                                                        */
+int b200sm_search_loop_place(b200sm_t s, b200reg_t reg, float voxel_leaf_size, double threshold_loop_closure_score,
+                             double distance_loop_closure, int search_submap_num, double sc_threshold, int top_k,
+                             b200sm_place_result* out, size_t capacity, size_t* n_out, size_t* n_scored);
+/* the last place search's per-submap scores: *n = submaps at that search; min(capacity, n) rows of D (NaN for a submap
+ * that was not eligible) and s* (-1 there). Either array may be NULL.                                               */
+int b200sm_get_place_scores(b200sm_t s, size_t capacity, size_t* n, double* distances, int* shifts);
+
 /* ---- backend pose adjustment: GraphBasedSlamComponent::doPoseAdjustment (gbs.cpp:262-371) ----------------------------
  * LoopEdge of graph_based_slam_component.h: pair_id = (from, to), relative_pose = from^-1 * to (gbs.cpp:240-247).
  * A b200sm_search_loop result with accepted = 1 gives from = id_min, relative_pose = relative_pose and

@@ -463,6 +463,32 @@ class ScanMatcherSession {
     hits.resize(n);
     check(b200sm_get_global_search(s_.get(), n, &n, poses.data(), scores.data(), hits.data()));
   }
+  // ---- place recognition (b200sm_search_loop_place): a loop search by Scan Context that does not trust the drifted poses
+  void setScanContextParams(const b200sm_scan_context_params* p) { check(b200sm_set_scan_context_params(s_.get(), p)); }
+  // descriptor of submap `index`: num_rings * num_sectors floats, ring-major
+  void scanContext(size_t index, std::vector<float>& out, int num_rings = 20, int num_sectors = 60) {
+    out.resize((size_t)num_rings * num_sectors);
+    check(b200sm_get_scan_context(s_.get(), index, out.data(), out.size()));
+  }
+  // the top_k best candidates under sc_threshold, verified from the descriptors' heading; an accepted row gives the loop
+  // edge (row.loop.id_min, numSubmaps() - 1, row.loop.relative_pose). Returns the number of eligible submaps.
+  size_t searchLoopPlace(b200reg_t reg, float voxel_leaf_size, double threshold_loop_closure_score, double distance_loop_closure,
+                         int search_submap_num, double sc_threshold, int top_k, std::vector<b200sm_place_result>& rows) {
+    rows.resize(top_k > 0 ? (size_t)top_k : 1);
+    size_t n = 0, scored = 0;
+    check(b200sm_search_loop_place(s_.get(), reg, voxel_leaf_size, threshold_loop_closure_score, distance_loop_closure,
+                                   search_submap_num, sc_threshold, top_k, rows.data(), rows.size(), &n, &scored));
+    rows.resize(n);
+    return scored;
+  }
+  // the last place search's D (NaN: not eligible) and s* (-1) per submap
+  void placeScores(std::vector<double>& distances, std::vector<int>& shifts) {
+    size_t n = 0;
+    check(b200sm_get_place_scores(s_.get(), 0, &n, nullptr, nullptr));
+    distances.resize(n);
+    shifts.resize(n);
+    check(b200sm_get_place_scores(s_.get(), n, &n, distances.data(), shifts.data()));
+  }
   b200sm_localize_stats localizeStats() const {
     b200sm_localize_stats st{};
     check(b200sm_get_localize_stats(s_.get(), &st));

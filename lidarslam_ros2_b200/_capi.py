@@ -48,6 +48,7 @@ SYMBOLS = [
     "b200sm_set_prior_map_pcd", "b200sm_set_prior_map", "b200sm_set_localization_params", "b200sm_localize_cloud",
     "b200sm_localize_init", "b200sm_get_localize_stats", "b200sm_get_cut", "b200reg_ndt_score_poses",
     "b200sm_localize_global", "b200sm_get_global_search",
+    "b200sm_set_scan_context_params", "b200sm_get_scan_context", "b200sm_search_loop_place", "b200sm_get_place_scores",
     # include/b200comm.h
     "b200comm_unique_id", "b200comm_create", "b200comm_destroy", "b200comm_all_gather_rows", "b200comm_rank", "b200comm_last_error",
     "b200comm_board_create", "b200comm_board_destroy", "b200comm_board_info",
@@ -58,6 +59,15 @@ class SmLoopResult(C.Structure):
     _fields_ = [("is_candidate", C.c_int), ("id_min", C.c_int), ("accepted", C.c_int), ("pad", C.c_int),
                 ("min_dist", C.c_double), ("fitness", C.c_double), ("final_T", C.c_float * 16),
                 ("relative_pose", C.c_double * 16), ("n_source", C.c_size_t), ("n_target", C.c_size_t)]
+
+
+class SmScanContextParams(C.Structure):
+    _fields_ = [("num_rings", C.c_int), ("num_sectors", C.c_int), ("max_radius", C.c_double), ("lidar_height", C.c_double)]
+
+
+class SmPlaceResult(C.Structure):
+    _fields_ = [("loop", SmLoopResult), ("sc_distance", C.c_double), ("shift", C.c_int), ("pad", C.c_int),
+                ("guess", C.c_float * 16)]
 
 
 class SmLoopEdge(C.Structure):
@@ -225,6 +235,10 @@ def lib() -> C.CDLL:
     L.b200reg_ndt_score_poses.argtypes = [vp, i, vp, vp, vp]
     L.b200sm_localize_global.argtypes = [vp, vp, vp, sz, sz, C.c_long, C.POINTER(SmGlobalSearch), vp, vp, C.POINTER(SmGlobalResult)]
     L.b200sm_get_global_search.argtypes = [vp, sz, C.POINTER(sz), vp, vp, vp]
+    L.b200sm_set_scan_context_params.argtypes = [vp, C.POINTER(SmScanContextParams)]
+    L.b200sm_get_scan_context.argtypes = [vp, sz, vp, sz]
+    L.b200sm_search_loop_place.argtypes = [vp, vp, f, d, d, i, d, i, vp, sz, C.POINTER(sz), C.POINTER(sz)]
+    L.b200sm_get_place_scores.argtypes = [vp, sz, C.POINTER(sz), vp, vp]
     L.b200comm_unique_id.argtypes = [vp]
     L.b200comm_create.argtypes = [vp, i, i, i, C.POINTER(vp)]
     L.b200comm_destroy.argtypes = [vp]

@@ -1,0 +1,31 @@
+// Place recognition on the scan-matcher session (b200sm_search_loop_place): the Scan Context kernels of
+// place_recognition.cu. The arithmetic is csrc/scan_context.hpp's; these are the launches, enqueued on the caller's stream.
+#pragma once
+#include <cuda_runtime.h>
+
+#include <cstdint>
+
+namespace b200 {
+
+// One submap to describe: its cloud (sensor frame), its points, the first tile of the launch that serves it, and the slot
+// of the descriptor store it is written to.
+struct ScBuildEntry {
+  const float4* cloud;
+  unsigned n, first_tile, slot, pad;
+};
+constexpr int SC_BUILD_THREADS = 256, SC_BUILD_PER_THREAD = 16, SC_BUILD_TILE = SC_BUILD_THREADS * SC_BUILD_PER_THREAD;
+
+// K13a: keys[slot * R * S + bin] = max order key of the bin's points over the submaps of `table` (n_entries rows, sorted by
+// first_tile, `tiles` tiles in all). The keys of those slots must be zero beforehand. tables = R ring bounds then S sector
+// directions (scan_context.hpp's sc_tables).
+void sc_build_launch(const ScBuildEntry* table, int n_entries, unsigned tiles, uint32_t* keys, const double* tables, int num_rings,
+                     int num_sectors, float lidar_height, cudaStream_t stream);
+// The finishing pass of K13a over slots [first_slot, first_slot + n_slots): keys become the descriptor's floats in place
+// (an empty bin 0), and norms[slot * S + j] the column norms.
+void sc_finish_launch(uint32_t* keys, double* norms, size_t first_slot, size_t n_slots, int num_rings, int num_sectors,
+                      cudaStream_t stream);
+// K13b: for r < n_ids, (distance[r], shift[r]) = (D, s*) of descriptor `query_slot` against descriptor ids[r].
+void sc_search_launch(const float* desc, const double* norms, size_t query_slot, const int* ids, int n_ids, double* distance,
+                      int* shift, int num_rings, int num_sectors, cudaStream_t stream);
+
+}  // namespace b200

@@ -33,7 +33,9 @@
 #include "engine.hpp"
 #include "global_grid.hpp"
 #include "map_cut.hpp"
+#include "place_recognition.cuh"
 #include "pose_graph.hpp"
+#include "scan_context.hpp"
 #include "sensor_frame.hpp"
 
 namespace b200 {
@@ -288,6 +290,19 @@ struct b200sm_session {
   std::vector<float> global_poses;
   std::vector<double> global_scores;
   std::vector<long long> global_hits;
+  // place recognition (b200sm_search_loop_place): descriptors of submaps [0, sc_built) in slots of sc_keys (keys while being
+  // built, then the descriptor's floats) and their column norms; room for sc_cap submaps
+  ScParams sc;
+  DeviceBuffer<double> sc_tables;  // ring bounds, then sector directions
+  bool sc_tables_ready = false;
+  DeviceBuffer<uint32_t> sc_keys;
+  DeviceBuffer<double> sc_norms;
+  size_t sc_built = 0, sc_cap = 0;
+  DeviceBuffer<ScBuildEntry> sc_build_table;
+  DeviceBuffer<int> sc_ids, sc_shift;
+  DeviceBuffer<double> sc_dist;
+  std::vector<double> place_distances;  // the last place search, per submap
+  std::vector<int> place_shifts;
 };
 
 namespace {
@@ -734,11 +749,12 @@ int loop_set_source(b200sm_t s, b200reg_t reg) {
 }
 
 // one candidate: target = VoxelGrid(voxel_leaf_size) of the submaps id - search_submap_num .. id + search_submap_num
-// (:206-225), align without guess (:229), getFitnessScore (:230), loop edge when the score passes (:232-246).
+// (:206-225), align without guess (:229; the place search gives one), getFitnessScore (:230), loop edge when the score
+// passes (:232-246).
 // The reference does not test the upper index (undefined behaviour when the window runs past the newest submap);
 // here indices beyond the array are skipped like the negative ones. Nothing is uploaded: the submaps live in HBM.
 int loop_evaluate(b200sm_t s, b200reg_t reg, const LoopCandidate& cand, float voxel_leaf_size, double threshold_loop_closure_score,
-                  int search_submap_num, b200sm_loop_result* out) {
+                  int search_submap_num, b200sm_loop_result* out, const float* guess = nullptr) {
   const int n_sub = (int)s->submaps.size();
   const Submap& latest = *s->submaps[n_sub - 1];
   const int id_min = cand.id;
@@ -768,7 +784,7 @@ int loop_evaluate(b200sm_t s, b200reg_t reg, const LoopCandidate& cand, float vo
   B200_CUDA(cudaStreamSynchronize(s->stream));
   int rc = b200reg_set_input_target_device(reg, tgt, m);
   float fin[16];
-  if (rc == B200REG_OK) rc = b200reg_align(reg, nullptr, fin);  // :229, no guess
+  if (rc == B200REG_OK) rc = b200reg_align(reg, guess, fin);  // :229, no guess (a place search passes one)
   double fitness = 0;
   if (rc == B200REG_OK) rc = b200reg_get_fitness_score(reg, 1.7976931348623157e308, &fitness);  // :230
   if (rc != B200REG_OK) {
@@ -1491,6 +1507,188 @@ int b200sm_get_localize_stats(b200sm_t s, b200sm_localize_stats* out) {
 int b200sm_get_cut(b200sm_t s, float* out_xyzi, size_t capacity, size_t* n) {
   if (!s) return B200REG_ERR_ARG;
   return sm_guarded(s, [&]() { return read_back(s, s->cut.ptr, s->have_cut ? s->n_cut : 0, out_xyzi, capacity, n); });
+}
+
+}  // extern "C"
+
+// ---- place recognition (b200sm_search_loop_place): Scan Context descriptors of the submaps, built lazily on the device,
+// and a search over them that does not look at the poses (csrc/scan_context.hpp, csrc/place_recognition.cu)
+namespace {
+
+size_t sc_bins(const ScParams& p) { return (size_t)p.num_rings * p.num_sectors; }
+
+void sc_drop(b200sm_t s) {
+  s->sc_built = 0;
+  s->sc_tables_ready = false;
+}
+
+// Descriptors for every submap that has none yet, in one K13a launch and its finishing pass. Stream-ordered: the caller
+// synchronises before it reads anything back.
+int sc_ensure(b200sm_t s) {
+  const ScParams& p = s->sc;
+  const size_t n_sub = s->submaps.size(), nb = sc_bins(p);
+  if (!s->sc_tables_ready) {
+    std::vector<double> ring_b, sector_u;
+    sc_tables(p, ring_b, sector_u);
+    ring_b.insert(ring_b.end(), sector_u.begin(), sector_u.end());
+    s->sc_tables.ensure(ring_b.size());
+    B200_CUDA(cudaMemcpyAsync(s->sc_tables.ptr, ring_b.data(), ring_b.size() * sizeof(double), cudaMemcpyHostToDevice, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));  // the host vector goes out of scope
+    s->sc_tables_ready = true;
+  }
+  if (s->sc_built == n_sub) return (int)B200REG_OK;
+  if (n_sub > s->sc_cap || s->sc_keys.cap < n_sub * nb || s->sc_norms.cap < n_sub * (size_t)p.num_sectors) {
+    // grow, keeping the descriptors already built (DeviceBuffer::ensure does not preserve contents)
+    const size_t cap = std::max(n_sub + 64, s->sc_cap + s->sc_cap / 2);
+    DeviceBuffer<uint32_t> keys;
+    DeviceBuffer<double> norms;
+    keys.ensure(cap * nb);
+    norms.ensure(cap * (size_t)p.num_sectors);
+    if (s->sc_built) {
+      B200_CUDA(cudaMemcpyAsync(keys.ptr, s->sc_keys.ptr, s->sc_built * nb * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s->stream));
+      B200_CUDA(cudaMemcpyAsync(norms.ptr, s->sc_norms.ptr, s->sc_built * p.num_sectors * sizeof(double), cudaMemcpyDeviceToDevice,
+                                s->stream));
+    }
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    std::swap(keys.ptr, s->sc_keys.ptr);
+    std::swap(keys.cap, s->sc_keys.cap);
+    std::swap(norms.ptr, s->sc_norms.ptr);
+    std::swap(norms.cap, s->sc_norms.cap);
+    s->sc_cap = cap;
+  }
+  std::vector<ScBuildEntry> table;
+  unsigned long long tiles = 0;
+  for (size_t i = s->sc_built; i < n_sub; i++) {
+    const Submap& sub = *s->submaps[i];
+    if (sub.n == 0) continue;  // an empty submap owns no tile: its descriptor is all zero
+    if (sub.n > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "scan_context: a submap of 2^32 points or more");
+    table.push_back({sub.cloud, (unsigned)sub.n, (unsigned)tiles, (unsigned)i, 0u});
+    tiles += (sub.n + SC_BUILD_TILE - 1) / SC_BUILD_TILE;
+  }
+  if (tiles > 0x7fffffffull) return sm_fail(s, B200REG_ERR_ARG, "scan_context: too many points for one launch");
+  const size_t first = s->sc_built, count = n_sub - s->sc_built;
+  B200_CUDA(cudaMemsetAsync(s->sc_keys.ptr + first * nb, 0, count * nb * sizeof(uint32_t), s->stream));
+  if (!table.empty()) {
+    s->sc_build_table.ensure(table.size());
+    B200_CUDA(cudaMemcpyAsync(s->sc_build_table.ptr, table.data(), table.size() * sizeof(ScBuildEntry), cudaMemcpyHostToDevice,
+                              s->stream));
+    sc_build_launch(s->sc_build_table.ptr, (int)table.size(), (unsigned)tiles, s->sc_keys.ptr, s->sc_tables.ptr, p.num_rings,
+                    p.num_sectors, (float)p.lidar_height, s->stream);
+    s->launches += 1;
+  }
+  sc_finish_launch(s->sc_keys.ptr, s->sc_norms.ptr, first, count, p.num_rings, p.num_sectors, s->stream);
+  s->launches += 1;
+  B200_CUDA(cudaStreamSynchronize(s->stream));  // the table's host copy goes out of scope
+  s->sc_built = n_sub;
+  return (int)B200REG_OK;
+}
+
+const float* sc_desc(b200sm_t s) { return reinterpret_cast<const float*>(s->sc_keys.ptr); }
+
+}  // namespace
+
+extern "C" {
+
+int b200sm_set_scan_context_params(b200sm_t s, const b200sm_scan_context_params* p) {
+  if (!s) return B200REG_ERR_ARG;
+  ScParams q;
+  if (p) {
+    q.num_rings = p->num_rings;
+    q.num_sectors = p->num_sectors;
+    q.max_radius = p->max_radius;
+    q.lidar_height = p->lidar_height;
+  }
+  if (!sc_params_valid(q)) return sm_fail(s, B200REG_ERR_ARG, "set_scan_context_params: a parameter out of range");
+  s->sc = q;
+  sc_drop(s);
+  return B200REG_OK;
+}
+
+int b200sm_get_scan_context(b200sm_t s, size_t index, float* out, size_t capacity) {
+  if (!s || !out || index >= s->submaps.size() || capacity < sc_bins(s->sc)) return B200REG_ERR_ARG;
+  return sm_guarded(s, [&]() {
+    const int rc = sc_ensure(s);
+    if (rc != B200REG_OK) return rc;
+    const size_t nb = sc_bins(s->sc);
+    B200_CUDA(cudaMemcpyAsync(out, sc_desc(s) + index * nb, nb * sizeof(float), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_search_loop_place(b200sm_t s, b200reg_t reg, float voxel_leaf_size, double threshold_loop_closure_score,
+                             double distance_loop_closure, int search_submap_num, double sc_threshold, int top_k,
+                             b200sm_place_result* out, size_t capacity, size_t* n_out, size_t* n_scored) {
+  if (!s || !reg || !n_out || !(voxel_leaf_size > 0) || search_submap_num < 0 || top_k < 1 || top_k > SC_MAX_TOP_K ||
+      !std::isfinite(sc_threshold) || (!out && capacity))
+    return B200REG_ERR_ARG;
+  return sm_guarded(s, [&]() {
+    *n_out = 0;
+    if (n_scored) *n_scored = 0;
+    const int n_sub = (int)s->submaps.size();
+    s->place_distances.assign(n_sub, std::nan(""));
+    s->place_shifts.assign(n_sub, -1);
+    if (n_sub < 2) return (int)B200REG_OK;
+    int rc = sc_ensure(s);
+    if (rc != B200REG_OK) return rc;
+    const ScParams& p = s->sc;
+    const Submap& latest = *s->submaps[n_sub - 1];
+    std::vector<int> ids;  // the reference's first gate (gbs.cpp:193), strict; no position gate
+    for (int i = 0; i < n_sub - 1; i++)
+      if (latest.distance - s->submaps[i]->distance > distance_loop_closure) ids.push_back(i);
+    if (n_scored) *n_scored = ids.size();
+    if (ids.empty()) return (int)B200REG_OK;
+    const size_t m = ids.size();
+    s->sc_ids.ensure(m);
+    s->sc_dist.ensure(m);
+    s->sc_shift.ensure(m);
+    B200_CUDA(cudaMemcpyAsync(s->sc_ids.ptr, ids.data(), m * sizeof(int), cudaMemcpyHostToDevice, s->stream));
+    sc_search_launch(sc_desc(s), s->sc_norms.ptr, (size_t)(n_sub - 1), s->sc_ids.ptr, (int)m, s->sc_dist.ptr, s->sc_shift.ptr,
+                     p.num_rings, p.num_sectors, s->stream);
+    s->launches += 1;
+    std::vector<double> dist(m);
+    std::vector<int> shift(m);
+    B200_CUDA(cudaMemcpyAsync(dist.data(), s->sc_dist.ptr, m * sizeof(double), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaMemcpyAsync(shift.data(), s->sc_shift.ptr, m * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    for (size_t r = 0; r < m; r++) {
+      s->place_distances[ids[r]] = dist[r];
+      s->place_shifts[ids[r]] = shift[r];
+    }
+    const std::vector<int> order = sc_rank(dist.data(), ids.data(), m, sc_threshold);
+    const size_t k = std::min({order.size(), (size_t)top_k, capacity});
+    bool have_source = false;
+    for (size_t q = 0; q < k; q++) {
+      const size_t r = (size_t)order[q];
+      const int id = ids[r];
+      const Submap& cand = *s->submaps[id];
+      if (!have_source) {
+        rc = loop_set_source(s, reg);
+        if (rc != B200REG_OK) return rc;
+        have_source = true;
+      }
+      b200sm_place_result* row = out + q;
+      std::memset(row, 0, sizeof(*row));
+      row->sc_distance = dist[r];
+      row->shift = shift[r];
+      sc_guess(cand.pose, latest.pose, shift[r], p.num_sectors, row->guess);
+      const double dx = latest.pose[3] - cand.pose[3], dy = latest.pose[7] - cand.pose[7], dz = latest.pose[11] - cand.pose[11];
+      const LoopCandidate lc{id, std::sqrt(dx * dx + dy * dy + dz * dz)};  // loop_candidates' min_dist
+      rc = loop_evaluate(s, reg, lc, voxel_leaf_size, threshold_loop_closure_score, search_submap_num, &row->loop, row->guess);
+      if (rc != B200REG_OK) return rc;
+      *n_out += 1;
+    }
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_place_scores(b200sm_t s, size_t capacity, size_t* n, double* distances, int* shifts) {
+  if (!s || !n) return B200REG_ERR_ARG;
+  const size_t total = s->place_distances.size(), m = std::min(capacity, total);
+  *n = total;
+  if (distances && m) std::memcpy(distances, s->place_distances.data(), m * sizeof(double));
+  if (shifts && m) std::memcpy(shifts, s->place_shifts.data(), m * sizeof(int));
+  return B200REG_OK;
 }
 
 }  // extern "C"

@@ -251,6 +251,57 @@ class ScanMatcher:
             out.append(d)
         return out
 
+    # ---- place recognition (b200sm_search_loop_place): Scan Context descriptors, a search that ignores the drifted poses ----
+    def setScanContextParams(self, num_rings: int = 20, num_sectors: int = 60, max_radius: float = 80.0, lidar_height: float = 2.0):
+        """The descriptor's grid: num_rings x num_sectors bins out to max_radius metres; a bin holds the largest
+        z + lidar_height of its points. Drops every descriptor built so far (they are rebuilt at the next use)."""
+        p = _capi.SmScanContextParams(int(num_rings), int(num_sectors), float(max_radius), float(lidar_height))
+        self._check(self._lib.b200sm_set_scan_context_params(self._h, C.byref(p)))
+        self._scp = (int(num_rings), int(num_sectors))
+
+    def scanContext(self, index: int) -> np.ndarray:
+        """The descriptor of submap `index`, (num_rings, num_sectors) float32 (built on the device if it is not yet)."""
+        R, S = getattr(self, "_scp", (20, 60))
+        out = np.empty((R, S), dtype=np.float32)
+        self._check(self._lib.b200sm_get_scan_context(self._h, int(index), _ptr(out), out.size))
+        return out
+
+    def searchLoopPlace(self, registration, voxel_leaf_size: float = 0.2, threshold_loop_closure_score: float = 1.0,
+                        distance_loop_closure: float = 20.0, search_submap_num: int = 3, sc_threshold: float = 0.4,
+                        top_k: int = 3, capacity=None):
+        """The newest submap against every older one more than distance_loop_closure behind it along the path, by Scan
+        Context distance and whatever the poses say; the top_k best under sc_threshold are verified by the registration from
+        the heading the descriptors give (b200sm_search_loop_place). Returns (rows, n_scored): one dict per verified
+        candidate, best first, with searchLoopAll's keys plus sc_distance, shift and guess (4x4)."""
+        cap = int(top_k) if capacity is None else int(capacity)
+        arr = (_capi.SmPlaceResult * max(1, cap))()
+        n, scored = C.c_size_t(0), C.c_size_t(0)
+        self._check(self._lib.b200sm_search_loop_place(self._h, registration._h, float(voxel_leaf_size),
+                                                       float(threshold_loop_closure_score), float(distance_loop_closure),
+                                                       int(search_submap_num), float(sc_threshold), int(top_k), arr, cap,
+                                                       C.byref(n), C.byref(scored)))
+        out = []
+        for k in range(n.value):
+            p = arr[k]
+            r = p.loop
+            d = {"is_candidate": True, "id_min": int(r.id_min), "accepted": bool(r.accepted), "min_dist": float(r.min_dist),
+                 "fitness": float(r.fitness), "n_source": int(r.n_source), "n_target": int(r.n_target),
+                 "final": np.array(r.final_T, dtype=np.float32).reshape(4, 4).T.copy(), "sc_distance": float(p.sc_distance),
+                 "shift": int(p.shift), "guess": np.array(p.guess, dtype=np.float32).reshape(4, 4).T.copy()}
+            if r.accepted:
+                d["relative_pose"] = np.array(r.relative_pose, dtype=np.float64).reshape(4, 4).T.copy()
+            out.append(d)
+        return out, int(scored.value)
+
+    def placeScores(self):
+        """The last searchLoopPlace's per-submap (D float64, s* int32); D is NaN and s* -1 where a submap was not eligible."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_get_place_scores(self._h, 0, C.byref(n), None, None))
+        D = np.empty(n.value, dtype=np.float64)
+        S = np.empty(n.value, dtype=np.int32)
+        self._check(self._lib.b200sm_get_place_scores(self._h, n.value, C.byref(n), _ptr(D), _ptr(S)))
+        return D, S
+
     def poseAdjust(self, loop_edges, num_adjacent_pose_cnstraints: int = 5, max_iterations: int = 10):
         """GraphBasedSlamComponent::doPoseAdjustment's pose-graph solve (gbs.cpp:262-319) over the session's submap poses:
         loop_edges is a list of (from, to, relative_pose 4x4), e.g. (r["id_min"], numSubmaps() - 1, r["relative_pose"]) of
