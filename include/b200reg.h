@@ -484,6 +484,54 @@ int b200sm_assemble_map(b200sm_t s, const double* poses_colmajor16, float* out_x
  * No point of the map is read back. The file is written in place. n_points, n_bytes (may be NULL) = points and file size.
  * B200REG_ERR_ARG for an empty map (no file is created), B200REG_ERR_IO when the file cannot be opened or written.      */
 int b200sm_save_map_pcd_ascii(b200sm_t s, const double* poses_colmajor16, const char* path, size_t* n_points, size_t* n_bytes);
+/* ---- 2D occupancy grid of the map, for a navigation stack (nav2's map_server, AMCL) -------------------------------------
+ * No counterpart in the reference. Every submap's points are rays from its sensor origin: the endpoint is the point
+ * b200sm_assemble_map(s, poses_colmajor16, ...) returns for it, the origin the same float pose applied to (float)
+ * sensor_origin. A ray marks its endpoint's cell HIT when the endpoint lies in the height band [z_min, z_max] (map frame),
+ * and every cell its segment crosses inside the band FREE (a 4-connected Amanatides-Woo walk in 2^16-per-cell fixed
+ * point); within one submap a hit cell is not free (OctoMap's per-scan update). Each cell counts the submaps that hit it
+ * and those that freed it; its value is -1 when both are 0, else round-half-up of 100 * hits / (hits + frees). The exact
+ * definitions (skipped points, fixed point, band clip, walk and its tie rule, extent, image) are in
+ * csrc/occupancy_grid.hpp; DESIGN.md section 7b describes the build. Counts of per-submap booleans do not depend on the
+ * order of the work, so the grid is bitwise deterministic. A pose adjustment moves every submap, so each call rebuilds the
+ * grid from all submaps. NDT and GICP sessions alike; no registration handle is involved. */
+typedef struct b200sm_occupancy_params {
+  double resolution;        /* metres per cell, finite, > 0; default 0.05                                             */
+  double z_min, z_max;      /* map-frame height band, finite, z_min < z_max; defaults 0.2 and 2.0 (ground at z = 0)  */
+  double max_range;         /* finite, > 0: rays longer than this (horizontally) are skipped; default 100;
+                               max_range / resolution <= 2^14                                                         */
+  double sensor_origin[3];  /* LiDAR position in the robot frame (the translation given to b200sm_set_sensor_transform,
+                               or 0 when the clouds are in the sensor frame); default 0                               */
+  double occupied_thresh, free_thresh; /* 0 <= free_thresh < occupied_thresh <= 1; defaults 0.65, 0.25                */
+} b200sm_occupancy_params;
+typedef struct b200sm_occupancy_info {
+  unsigned width, height;            /* cells                                                                      */
+  double origin[2], resolution;      /* map-frame corner of cell (0, 0), as map_server's YAML origin               */
+  unsigned long long n_rays, n_skipped; /* points cast as rays / skipped (non-finite, or beyond max_range)          */
+  int n_batches;                     /* launches of the walks (submaps batched by a fixed 64 MiB bitmap budget)    */
+  unsigned long long n_occupied, n_free, n_unknown; /* cells the image marks 0 / 254, and cells of value -1         */
+} b200sm_occupancy_info;
+/* Build the grid from every submap at its own pose (poses_colmajor16 NULL) or at the given 16 * n_submaps doubles (the
+ * output of b200sm_pose_adjust). params NULL: the defaults. A parameter out of range, a non-finite pose entry, a sensor
+ * origin beyond 2^30 cells or farther than 2^16 cells from the band, no submaps, or a grid of more than 2^28 cells (the
+ * message gives width and height): B200REG_ERR_ARG, checked before the grid is allocated (the extent is measured on the
+ * device first, with 144 bytes per submap of tables); the previous grid stays. The
+ * session keeps the grid until the next build or destroy: 10 bytes per cell (hits and frees uint32, value, image byte;
+ * 2.7 GB at the 2^28-cell cap), plus the walks' bitmap scratch (the largest batch: at most 64 MiB, or the bitmaps of
+ * the largest submap when they are larger: 2 bits per cell of its window) and 144 bytes per submap of tables. info may
+ * be NULL. */
+int b200sm_build_occupancy_grid(b200sm_t s, const double* poses_colmajor16, const b200sm_occupancy_params* params,
+                                b200sm_occupancy_info* info);
+/* The last grid, row-major from cell (0, 0) (nav_msgs/OccupancyGrid.data): min(capacity, width * height) cells of each
+ * non-NULL array (values -1..100, hits, frees). No grid built yet: B200REG_ERR_ARG. */
+int b200sm_get_occupancy_grid(b200sm_t s, signed char* data, unsigned* hits, unsigned* frees, size_t capacity);
+/* The map_server pair of the last grid: pgm_path gets "P5", a comment line, "width height", "255", then the trinary image
+ * (0 occupied, 254 free, 205 unknown; top row first); yaml_path gets image (the PGM's basename), mode: trinary,
+ * resolution, origin: [x, y, 0], negate: 0, occupied_thresh, free_thresh (numbers that read back bitwise; the image name
+ * double-quoted, so that any file name reads back as itself). The rule is
+ * nav2's map_saver's as its documentation states it; csrc/occupancy_grid.hpp's text is the contract. No grid built yet:
+ * B200REG_ERR_ARG. A file that cannot be opened or written: B200REG_ERR_IO. */
+int b200sm_save_occupancy_map(b200sm_t s, const char* pgm_path, const char* yaml_path);
 /* The same text for a HOST PointXYZI cloud (records as in b200sm_import_submap; intensity_offset_bytes >= 0), formatted
  * on `device`. *n_bytes = size of the whole file content (header and data); min(*n_bytes, capacity) bytes are copied to
  * out, so capacity 0 is a size query. B200REG_ERR_ARG for n == 0, a negative intensity offset, or a stride or offset that

@@ -489,6 +489,27 @@ class ScanMatcherSession {
     shifts.resize(n);
     check(b200sm_get_place_scores(s_.get(), n, &n, distances.data(), shifts.data()));
   }
+  // ---- occupancy grid for a navigation stack (b200sm_build_occupancy_grid): poses empty = the submaps' own, else 16 doubles
+  // per submap, column-major (b200sm_pose_adjust's output); p nullptr = the defaults
+  b200sm_occupancy_info buildOccupancyGrid(const std::vector<double>& poses_colmajor16 = {},
+                                           const b200sm_occupancy_params* p = nullptr) {
+    b200sm_occupancy_info info{};
+    check(b200sm_build_occupancy_grid(s_.get(), poses_colmajor16.empty() ? nullptr : poses_colmajor16.data(), p, &info));
+    og_cells_ = (size_t)info.width * info.height;
+    return info;
+  }
+  // the last grid as nav_msgs/OccupancyGrid.data (row-major from cell (0, 0)); hits / frees when non-null
+  void occupancyGrid(std::vector<signed char>& data, std::vector<unsigned>* hits = nullptr, std::vector<unsigned>* frees = nullptr) {
+    data.resize(og_cells_);
+    if (hits) hits->resize(og_cells_);
+    if (frees) frees->resize(og_cells_);
+    check(b200sm_get_occupancy_grid(s_.get(), data.data(), hits ? hits->data() : nullptr, frees ? frees->data() : nullptr,
+                                    og_cells_));
+  }
+  // nav2 map_server's map.pgm + map.yaml of the last grid
+  void saveOccupancyMap(const std::string& pgm_path, const std::string& yaml_path) {
+    check(b200sm_save_occupancy_map(s_.get(), pgm_path.c_str(), yaml_path.c_str()));
+  }
   b200sm_localize_stats localizeStats() const {
     b200sm_localize_stats st{};
     check(b200sm_get_localize_stats(s_.get(), &st));
@@ -507,6 +528,7 @@ class ScanMatcherSession {
     if (rc != B200REG_OK) throw std::runtime_error(std::string("b200sm: ") + b200sm_last_error(s_.get()));
   }
   std::shared_ptr<b200sm_session> s_;
+  size_t og_cells_ = 0;  // cells of the last grid this adapter built
 };
 
 }  // namespace b200reg

@@ -49,6 +49,7 @@ SYMBOLS = [
     "b200sm_localize_init", "b200sm_get_localize_stats", "b200sm_get_cut", "b200reg_ndt_score_poses",
     "b200sm_localize_global", "b200sm_get_global_search",
     "b200sm_set_scan_context_params", "b200sm_get_scan_context", "b200sm_search_loop_place", "b200sm_get_place_scores",
+    "b200sm_build_occupancy_grid", "b200sm_get_occupancy_grid", "b200sm_save_occupancy_map",
     # include/b200comm.h
     "b200comm_unique_id", "b200comm_create", "b200comm_destroy", "b200comm_all_gather_rows", "b200comm_rank", "b200comm_last_error",
     "b200comm_board_create", "b200comm_board_destroy", "b200comm_board_info",
@@ -68,6 +69,17 @@ class SmScanContextParams(C.Structure):
 class SmPlaceResult(C.Structure):
     _fields_ = [("loop", SmLoopResult), ("sc_distance", C.c_double), ("shift", C.c_int), ("pad", C.c_int),
                 ("guess", C.c_float * 16)]
+
+
+class SmOccupancyParams(C.Structure):
+    _fields_ = [("resolution", C.c_double), ("z_min", C.c_double), ("z_max", C.c_double), ("max_range", C.c_double),
+                ("sensor_origin", C.c_double * 3), ("occupied_thresh", C.c_double), ("free_thresh", C.c_double)]
+
+
+class SmOccupancyInfo(C.Structure):
+    _fields_ = [("width", C.c_uint), ("height", C.c_uint), ("origin", C.c_double * 2), ("resolution", C.c_double),
+                ("n_rays", C.c_ulonglong), ("n_skipped", C.c_ulonglong), ("n_batches", C.c_int), ("n_occupied", C.c_ulonglong),
+                ("n_free", C.c_ulonglong), ("n_unknown", C.c_ulonglong)]
 
 
 class SmLoopEdge(C.Structure):
@@ -239,6 +251,9 @@ def lib() -> C.CDLL:
     L.b200sm_get_scan_context.argtypes = [vp, sz, vp, sz]
     L.b200sm_search_loop_place.argtypes = [vp, vp, f, d, d, i, d, i, vp, sz, C.POINTER(sz), C.POINTER(sz)]
     L.b200sm_get_place_scores.argtypes = [vp, sz, C.POINTER(sz), vp, vp]
+    L.b200sm_build_occupancy_grid.argtypes = [vp, vp, C.POINTER(SmOccupancyParams), C.POINTER(SmOccupancyInfo)]
+    L.b200sm_get_occupancy_grid.argtypes = [vp, vp, vp, vp, sz]
+    L.b200sm_save_occupancy_map.argtypes = [vp, C.c_char_p, C.c_char_p]
     L.b200comm_unique_id.argtypes = [vp]
     L.b200comm_create.argtypes = [vp, i, i, i, C.POINTER(vp)]
     L.b200comm_destroy.argtypes = [vp]

@@ -16,6 +16,8 @@
 //   doPoseAdjustment: g2o pose graph + LM (host, pose_graph.hpp)                            :262-319   -> b200sm_pose_adjust
 //   doPoseAdjustment: modified_map / modified_map_array                                     :321-368   -> b200sm_assemble_map
 //   doPoseAdjustment: savePCDFileASCII("map.pcd", modified_map)                             :369       -> b200sm_save_map_pcd_ascii
+// The 2D occupancy grid of the map for a navigation stack (b200sm_build_occupancy_grid, csrc/occupancy_grid.hpp) has no
+// counterpart in the reference: nav2's map_server pair is written next to map.pcd.
 // Localising in a saved map has no counterpart in the reference: b200sm_set_prior_map* keep the map on the device and
 // b200sm_localize_cloud registers each frame against a stable cut of it around the pose (csrc/map_cut.hpp).
 // The submaps (sensor-frame, voxel-filtered) and the targeted cloud never leave the GPU; read-back entry points exist for
@@ -33,6 +35,7 @@
 #include "engine.hpp"
 #include "global_grid.hpp"
 #include "map_cut.hpp"
+#include "occupancy.cuh"
 #include "place_recognition.cuh"
 #include "pose_graph.hpp"
 #include "scan_context.hpp"
@@ -303,6 +306,18 @@ struct b200sm_session {
   DeviceBuffer<double> sc_dist;
   std::vector<double> place_distances;  // the last place search, per submap
   std::vector<int> place_shifts;
+  // occupancy grid (b200sm_build_occupancy_grid): the per-call table, bounds and counters, the walks' bitmap scratch, and
+  // the last grid built (hits, frees, values, trinary image), kept until the next build
+  DeviceBuffer<OgEntry> og_table;
+  DeviceBuffer<int> og_bounds;
+  DeviceBuffer<unsigned long long> og_counters;
+  DeviceBuffer<uint32_t> og_scratch, og_hits, og_frees;
+  DeviceBuffer<signed char> og_values;
+  DeviceBuffer<unsigned char> og_image;
+  bool og_built = false;
+  OgParams og_params;
+  unsigned og_width = 0, og_height = 0;
+  double og_origin[2] = {0, 0};
 };
 
 namespace {
@@ -1689,6 +1704,244 @@ int b200sm_get_place_scores(b200sm_t s, size_t capacity, size_t* n, double* dist
   if (distances && m) std::memcpy(distances, s->place_distances.data(), m * sizeof(double));
   if (shifts && m) std::memcpy(shifts, s->place_shifts.data(), m * sizeof(int));
   return B200REG_OK;
+}
+
+}  // extern "C"
+
+// ---- occupancy grid: free space ray-cast from every submap's sensor origin (csrc/occupancy_grid.hpp, csrc/occupancy.cu) ----
+namespace {
+
+// K14b's scratch budget: the hit and free bitmaps of a batch of submaps (2 MB each at 0.05 m and 100 m range). A submap
+// whose bitmaps alone exceed it forms a batch of its own.
+constexpr unsigned long long OG_SCRATCH_WORDS = 16ull << 20;  // 64 MiB
+
+OgParams og_params_from(const b200sm_occupancy_params* p) {
+  OgParams q;
+  if (p) {
+    q.resolution = p->resolution;
+    q.z_min = p->z_min;
+    q.z_max = p->z_max;
+    q.max_range = p->max_range;
+    for (int k = 0; k < 3; k++) q.sensor_origin[k] = p->sensor_origin[k];
+    q.occupied_thresh = p->occupied_thresh;
+    q.free_thresh = p->free_thresh;
+  }
+  return q;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b200sm_build_occupancy_grid(b200sm_t s, const double* poses_colmajor16, const b200sm_occupancy_params* params,
+                                b200sm_occupancy_info* info) {
+  if (!s) return B200REG_ERR_ARG;
+  const OgParams p = og_params_from(params);
+  OgConst c;
+  if (const char* why = og_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_occupancy_grid: ") + why).c_str());
+  const size_t n_sub = s->submaps.size();
+  if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_occupancy_grid: the session has no submaps");
+  if (poses_colmajor16)
+    for (size_t k = 0; k < 16 * n_sub; k++)
+      if (!std::isfinite(poses_colmajor16[k])) return sm_fail(s, B200REG_ERR_ARG, "build_occupancy_grid: a non-finite pose entry");
+  // every submap's float pose and ray origin, and the entries of the submaps that have points
+  std::vector<OgEntry> all(n_sub);
+  std::vector<int> bounds(4 * n_sub);
+  for (size_t k = 0; k < n_sub; k++) {
+    const Submap& sub = *s->submaps[k];
+    if (sub.n > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_occupancy_grid: a submap of 2^32 points or more");
+    OgEntry& e = all[k];
+    std::memset(&e, 0, sizeof(e));
+    double P[16];
+    for (int r = 0; r < 4; r++)
+      for (int col = 0; col < 4; col++)
+        P[col * 4 + r] = poses_colmajor16 ? poses_colmajor16[16 * k + col * 4 + r] : sub.pose[r * 4 + col];
+    og_pose_f(P, e.T);
+    long long o[3];
+    if (!og_origin(c, p, e.T, o)) {
+      s->err = "build_occupancy_grid: the sensor origin of submap " + std::to_string(k) +
+               " lies beyond 2^30 cells, or more than 2^16 cells from the height band";
+      return (int)B200REG_ERR_ARG;
+    }
+    e.cloud = sub.cloud;
+    e.n = (unsigned)sub.n;
+    e.xo = o[0];
+    e.yo = o[1];
+    e.zo = o[2];
+    bounds[4 * k + 0] = bounds[4 * k + 2] = og_cell(o[0]);
+    bounds[4 * k + 1] = bounds[4 * k + 3] = og_cell(o[1]);
+  }
+  return sm_guarded(s, [&]() {
+    // K14a over the submaps with points: one launch, one read-back of the bounds and counts
+    std::vector<OgEntry> table;
+    std::vector<size_t> ids;
+    unsigned long long tiles = 0;
+    for (size_t k = 0; k < n_sub; k++) {
+      if (all[k].n == 0) continue;  // an empty submap owns no tile: its origin alone widens the grid
+      all[k].first_tile = (unsigned)tiles;
+      tiles += (all[k].n + OG_TILE - 1) / OG_TILE;
+      table.push_back(all[k]);
+      ids.push_back(k);
+    }
+    if (tiles > 0x7fffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_occupancy_grid: too many points for one launch");
+    std::vector<int> tb(4 * table.size());
+    for (size_t r = 0; r < ids.size(); r++) std::memcpy(&tb[4 * r], &bounds[4 * ids[r]], 4 * sizeof(int));
+    unsigned long long ctr[OG_CTR_COUNT] = {};
+    s->og_counters.ensure(OG_CTR_COUNT);
+    B200_CUDA(cudaMemsetAsync(s->og_counters.ptr, 0, OG_CTR_COUNT * sizeof(unsigned long long), s->stream));
+    if (!table.empty()) {
+      s->og_table.ensure(table.size());
+      s->og_bounds.ensure(tb.size());
+      B200_CUDA(cudaMemcpyAsync(s->og_table.ptr, table.data(), table.size() * sizeof(OgEntry), cudaMemcpyHostToDevice, s->stream));
+      B200_CUDA(cudaMemcpyAsync(s->og_bounds.ptr, tb.data(), tb.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
+      og_bounds_launch(s->og_table.ptr, (int)table.size(), (unsigned)tiles, c, s->og_bounds.ptr, s->og_counters.ptr, s->stream);
+      s->launches += 1;
+      B200_CUDA(cudaMemcpyAsync(tb.data(), s->og_bounds.ptr, tb.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+    }
+    B200_CUDA(cudaMemcpyAsync(ctr, s->og_counters.ptr, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    for (size_t r = 0; r < ids.size(); r++) std::memcpy(&bounds[4 * ids[r]], &tb[4 * r], 4 * sizeof(int));
+    int gx0 = bounds[0], gy0 = bounds[1], gx1 = bounds[2], gy1 = bounds[3];
+    for (size_t k = 1; k < n_sub; k++) {
+      gx0 = std::min(gx0, bounds[4 * k]);
+      gy0 = std::min(gy0, bounds[4 * k + 1]);
+      gx1 = std::max(gx1, bounds[4 * k + 2]);
+      gy1 = std::max(gy1, bounds[4 * k + 3]);
+    }
+    const unsigned long long W = (unsigned long long)((long long)gx1 - gx0 + 1), H = (unsigned long long)((long long)gy1 - gy0 + 1);
+    if (W * H > OG_MAX_CELLS) {
+      s->err = "build_occupancy_grid: a grid of " + std::to_string(W) + " x " + std::to_string(H) + " cells exceeds 2^28 cells";
+      return (int)B200REG_ERR_ARG;
+    }
+    // from here on the previous grid is replaced
+    s->og_built = false;
+    const size_t cells = (size_t)(W * H);
+    s->og_hits.ensure(cells);
+    s->og_frees.ensure(cells);
+    s->og_values.ensure(cells);
+    s->og_image.ensure(cells);
+    B200_CUDA(cudaMemsetAsync(s->og_hits.ptr, 0, cells * sizeof(uint32_t), s->stream));
+    B200_CUDA(cudaMemsetAsync(s->og_frees.ptr, 0, cells * sizeof(uint32_t), s->stream));
+    // windows, then batches of consecutive submaps whose bitmaps fit the scratch budget (a submap whose bitmaps alone
+    // exceed it forms a batch of its own); the scratch is sized to the largest batch so formed
+    for (size_t r = 0; r < table.size(); r++) {
+      OgEntry& e = table[r];
+      const int* b = &tb[4 * r];
+      e.x0 = b[0];
+      e.y0 = b[1];
+      e.width = (unsigned)(b[2] - b[0] + 1);
+      e.height = (unsigned)(b[3] - b[1] + 1);
+      e.stride = (e.width + 31) / 32;
+      e.rows = e.height;
+    }
+    struct Batch {
+      size_t b0, b1;
+      unsigned long long words, fold, tiles;
+    };
+    std::vector<Batch> plan;
+    unsigned long long largest = 0;
+    for (size_t b0 = 0; b0 < table.size();) {
+      Batch bt{b0, b0, 0, 0, 0};
+      while (bt.b1 < table.size()) {
+        OgEntry& e = table[bt.b1];
+        const unsigned long long w = 2ull * e.stride * e.rows;
+        if (bt.b1 > b0 && bt.words + w > OG_SCRATCH_WORDS) break;
+        e.words_at = bt.words;
+        e.fold_first = bt.fold;
+        e.first_tile = (unsigned)bt.tiles;
+        bt.words += w;
+        bt.fold += w / 2;
+        bt.tiles += (e.n + OG_TILE - 1) / OG_TILE;
+        bt.b1++;
+      }
+      largest = std::max(largest, bt.words);
+      plan.push_back(bt);
+      b0 = bt.b1;
+    }
+    s->og_scratch.ensure((size_t)largest);
+    for (const Batch& bt : plan) {
+      if (bt.words > s->og_scratch.cap || bt.b1 > s->og_table.cap)
+        return sm_fail(s, B200REG_ERR_CUDA, "build_occupancy_grid: a walk batch larger than its scratch");
+      // the previous batch's kernels read the table: this copy is stream-ordered behind them
+      B200_CUDA(cudaMemcpyAsync(s->og_table.ptr + bt.b0, table.data() + bt.b0, (bt.b1 - bt.b0) * sizeof(OgEntry),
+                                cudaMemcpyHostToDevice, s->stream));
+      B200_CUDA(cudaMemsetAsync(s->og_scratch.ptr, 0, bt.words * sizeof(uint32_t), s->stream));
+      og_walk_launch(s->og_table.ptr + bt.b0, (int)(bt.b1 - bt.b0), (unsigned)bt.tiles, c, s->og_scratch.ptr, s->og_counters.ptr,
+                     s->stream);
+      og_fold_launch(s->og_table.ptr + bt.b0, (int)(bt.b1 - bt.b0), bt.fold, s->og_scratch.ptr, gx0, gy0, (unsigned)W,
+                     s->og_hits.ptr, s->og_frees.ptr, s->stream);
+      s->launches += 2;
+    }
+    const int batches = (int)plan.size();
+    og_classify_launch(s->og_hits.ptr, s->og_frees.ptr, (unsigned)W, (unsigned)H, c.occ_value, c.free_value, s->og_values.ptr,
+                       s->og_image.ptr, s->og_counters.ptr, s->stream);
+    s->launches += 1;
+    B200_CUDA(cudaMemcpyAsync(ctr, s->og_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));  // the host table goes out of scope; the counts are read
+    if (ctr[OG_CTR_TRIPPED]) return sm_fail(s, B200REG_ERR_CUDA, "build_occupancy_grid: a walk left its submap's window");
+    s->og_built = true;
+    s->og_params = p;
+    s->og_width = (unsigned)W;
+    s->og_height = (unsigned)H;
+    s->og_origin[0] = (double)gx0 * p.resolution;
+    s->og_origin[1] = (double)gy0 * p.resolution;
+    if (info) {
+      info->width = s->og_width;
+      info->height = s->og_height;
+      info->origin[0] = s->og_origin[0];
+      info->origin[1] = s->og_origin[1];
+      info->resolution = p.resolution;
+      info->n_rays = ctr[OG_CTR_RAYS];
+      info->n_skipped = ctr[OG_CTR_SKIPPED];
+      info->n_batches = batches;
+      info->n_occupied = ctr[OG_CTR_OCCUPIED];
+      info->n_free = ctr[OG_CTR_FREE];
+      info->n_unknown = ctr[OG_CTR_UNKNOWN];
+    }
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_occupancy_grid(b200sm_t s, signed char* data, unsigned* hits, unsigned* frees, size_t capacity) {
+  if (!s) return B200REG_ERR_ARG;
+  if (!s->og_built) return sm_fail(s, B200REG_ERR_ARG, "get_occupancy_grid: no grid has been built");
+  return sm_guarded(s, [&]() {
+    const size_t m = std::min(capacity, (size_t)s->og_width * s->og_height);
+    if (m) {
+      if (data) B200_CUDA(cudaMemcpyAsync(data, s->og_values.ptr, m, cudaMemcpyDeviceToHost, s->stream));
+      if (hits) B200_CUDA(cudaMemcpyAsync(hits, s->og_hits.ptr, m * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      if (frees) B200_CUDA(cudaMemcpyAsync(frees, s->og_frees.ptr, m * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaStreamSynchronize(s->stream));
+    }
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_save_occupancy_map(b200sm_t s, const char* pgm_path, const char* yaml_path) {
+  if (!s || !pgm_path || !yaml_path) return B200REG_ERR_ARG;
+  if (!s->og_built) return sm_fail(s, B200REG_ERR_ARG, "save_occupancy_map: no grid has been built");
+  return sm_guarded(s, [&]() {
+    const size_t cells = (size_t)s->og_width * s->og_height;
+    std::vector<unsigned char> image(cells);
+    B200_CUDA(cudaMemcpyAsync(image.data(), s->og_image.ptr, cells, cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    const OgParams& p = s->og_params;
+    const std::string head = og_pgm_header(s->og_width, s->og_height, p.resolution);
+    const std::string yaml = og_yaml(pgm_path, p.resolution, s->og_origin, p.occupied_thresh, p.free_thresh);
+    auto write = [&](const char* path, const std::string& a, const unsigned char* b, size_t nb) {
+      FILE* f = std::fopen(path, "wb");
+      if (!f) {
+        s->err = std::string("save_occupancy_map: cannot open ") + path + ": " + std::strerror(errno);
+        return false;
+      }
+      bool ok = std::fwrite(a.data(), 1, a.size(), f) == a.size() && (nb == 0 || std::fwrite(b, 1, nb, f) == nb);
+      ok = (std::fclose(f) == 0) && ok;
+      if (!ok) s->err = std::string("save_occupancy_map: writing ") + path + ": " + std::strerror(errno);
+      return ok;
+    };
+    if (!write(pgm_path, head, image.data(), cells) || !write(yaml_path, yaml, nullptr, 0)) return (int)B200REG_ERR_IO;
+    return (int)B200REG_OK;
+  });
 }
 
 }  // extern "C"

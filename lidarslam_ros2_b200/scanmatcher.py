@@ -346,6 +346,41 @@ class ScanMatcher:
                                                         C.byref(n), C.byref(size)))
         return int(n.value), int(size.value)
 
+    # ---- occupancy grid for a navigation stack (b200sm_build_occupancy_grid, csrc/occupancy_grid.hpp) ----
+    def buildOccupancyGrid(self, poses=None, resolution: float = 0.05, z_min: float = 0.2, z_max: float = 2.0,
+                           max_range: float = 100.0, sensor_origin=(0.0, 0.0, 0.0), occupied_thresh: float = 0.65,
+                           free_thresh: float = 0.25) -> dict:
+        """The 2D occupancy grid of every submap at its own pose (poses None) or at `poses` (N, 4, 4), e.g. poseAdjust's:
+        free space ray-cast on the device from each submap's sensor origin (sensor_origin: the LiDAR in the robot frame),
+        hits and frees counted per submap in the map-frame height band [z_min, z_max]. Returns the build's info as a dict
+        (width, height, origin (x, y), resolution, n_rays, n_skipped, n_batches, n_occupied, n_free, n_unknown)."""
+        P = None
+        if poses is not None:
+            P = np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(self.numSubmaps(), 4, 4).transpose(0, 2, 1))
+        so = (C.c_double * 3)(*[float(v) for v in sensor_origin])
+        prm = _capi.SmOccupancyParams(float(resolution), float(z_min), float(z_max), float(max_range), so, float(occupied_thresh),
+                                      float(free_thresh))
+        info = _capi.SmOccupancyInfo()
+        self._check(self._lib.b200sm_build_occupancy_grid(self._h, _ptr(P) if P is not None else None, C.byref(prm),
+                                                          C.byref(info)))
+        self._og = info
+        return _occupancy_info(info)
+
+    def occupancyGrid(self) -> dict:
+        """The last grid: data (height, width) int8 (-1 unknown, else 0..100; row 0 is the bottom row, as
+        nav_msgs/OccupancyGrid.data), hits and frees (height, width) uint32, and the build's info."""
+        info = getattr(self, "_og", None)
+        W, H = (int(info.width), int(info.height)) if info is not None else (0, 0)
+        data = np.empty((H, W), dtype=np.int8)
+        hits = np.empty((H, W), dtype=np.uint32)
+        frees = np.empty((H, W), dtype=np.uint32)
+        self._check(self._lib.b200sm_get_occupancy_grid(self._h, _ptr(data), _ptr(hits), _ptr(frees), W * H))
+        return dict(data=data, hits=hits, frees=frees, **_occupancy_info(info))
+
+    def saveOccupancyMap(self, pgm_path, yaml_path):
+        """nav2 map_server's map.pgm + map.yaml pair of the last grid (trinary)."""
+        self._check(self._lib.b200sm_save_occupancy_map(self._h, os.fsencode(pgm_path), os.fsencode(yaml_path)))
+
     # ---- read-back ----
     def stats(self) -> dict:
         st = _capi.SmStats()
@@ -379,6 +414,10 @@ class ScanMatcher:
         out = np.empty((n.value, 4), dtype=np.float32)
         self._check(self._lib.b200sm_get_submap(self._h, index, _ptr(out), n.value, C.byref(n), _ptr(pose), C.byref(dist)))
         return out, pose.reshape(4, 4).T.copy(), float(dist.value)
+
+
+def _occupancy_info(info) -> dict:
+    return {k: (tuple(getattr(info, k)) if k == "origin" else getattr(info, k)) for k, _ in _capi.SmOccupancyInfo._fields_}
 
 
 def backend_registration(registration_method: str = "NDT", ndt_resolution: float = 5.0, ndt_num_threads: int = 0, device: int = 0):
