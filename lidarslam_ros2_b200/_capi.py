@@ -8,7 +8,7 @@ import subprocess
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 REPO_ROOT = os.path.dirname(_HERE)
-LIB_PATH = os.path.join(_HERE, "csrc", os.environ.get("B200REG_LIB_VARIANT", "libb200reg.so"))  # variant: developer A/B builds
+LIB_PATH = os.path.join(_HERE, "csrc", "libb200reg.so")
 
 OK, ERR_ARG, ERR_NO_TARGET, ERR_NO_SOURCE, ERR_CUDA, ERR_TIMEOUT, ERR_GRID, ERR_IO, ERR_FORMAT = 0, -1, -2, -3, -4, -5, -6, -7, -8
 PCD_LOAD_PIECE_BYTES = 64 << 20  # B200REG_PCD_LOAD_PIECE_BYTES

@@ -5,8 +5,6 @@
 #include <cstdlib>
 #include <cstring>
 #include <atomic>
-#include <chrono>
-#include <cstdio>
 #include <dlfcn.h>
 #include <functional>
 #include <mutex>
@@ -87,7 +85,6 @@ struct b200reg_engine {
   DeviceBuffer<unsigned> batch_ready;    // one "scan k has arrived" flag per registration of a batch
   unsigned batch_tag = 0;                // value the flags take for the current call
   b200reg_engine* siblings[3] = {nullptr, nullptr, nullptr};  // further engines of b200reg_ndt_sweep (own stream and buffers each)
-  int sweep_engines = 4;  // engines (host threads) the sweep pipelines over (developer switch: B200REG_SWEEP_ENGINES)
 
   // b200reg_ndt_score_poses
   DeviceBuffer<float> d_poses;
@@ -167,16 +164,8 @@ void ensure_nn(b200reg_t h) {
   h->nn_valid = true;
 }
 
-// developer trace (env B200REG_TRACE=1): host wall clock of the phases of one NDT align, printed to stderr
-static const bool g_trace = getenv("B200REG_TRACE") != nullptr;
-static double trace_now() {
-  return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now().time_since_epoch()).count();
-}
-static thread_local double g_trace_t[4];
-
 // ---- NDT align: enqueue / complete ------------------------------------------------------------------------
 int ndt_align_begin(b200reg_t h, const float* guess_colmajor) {
-  if (g_trace) g_trace_t[0] = trace_now();
   h->converged = 0;
   set_identity(h->final_T);
   if (!h->have_target) return fail(h, B200REG_ERR_NO_TARGET, "align: no input target");
@@ -196,7 +185,6 @@ int ndt_align_begin(b200reg_t h, const float* guess_colmajor) {
     h->align_pending = false;
     return B200REG_OK;
   }
-  if (g_trace) g_trace_t[1] = trace_now();
   h->coop_lock = std::unique_lock<std::mutex>(cooperative_launch_mutex(h->device));
   try {
     B200_CUDA(cudaEventRecord(h->ev0, h->stream));
@@ -206,7 +194,6 @@ int ndt_align_begin(b200reg_t h, const float* guess_colmajor) {
     h->coop_lock.unlock();
     throw;
   }
-  if (g_trace) g_trace_t[2] = trace_now();
   h->align_pending = true;
   return B200REG_OK;
 }
@@ -243,11 +230,6 @@ int ndt_align_end(b200reg_t h) {
       return fail(h, B200REG_ERR_TIMEOUT, "NDT solver kernel watchdog fired (grid barrier timeout)");
     }
     B200_CUDA(cudaEventElapsedTime(&h->solve_ms, h->ev0, h->ev1));
-    if (g_trace) {
-      const double t = trace_now();
-      std::fprintf(stderr, "[trace] align: prologue %.1f us, launch calls %.1f us, wait %.1f us (kernel events %.1f us)\n",
-                   g_trace_t[1] - g_trace_t[0], g_trace_t[2] - g_trace_t[1], t - g_trace_t[2], 1e3 * h->solve_ms);
-    }
     std::memcpy(h->final_T, r.final_T, sizeof(h->final_T));
     h->converged = r.converged;
     h->iterations = r.iterations;
@@ -357,11 +339,7 @@ int b200reg_create(int kind, int device, b200reg_t* out) {
     B200_CUDA(cudaEventCreate(&h->ev0));
     B200_CUDA(cudaEventCreate(&h->ev1));
     h->solver.init(device, h->stream);
-    h->solver.timing_enabled = getenv("B200REG_TIMING") != nullptr;
-    h->solver.batch_profile = getenv("B200REG_BATCH_PROFILE") != nullptr;
-    if (const char* se = getenv("B200REG_SWEEP_ENGINES")) h->sweep_engines = std::max(1, std::min(4, atoi(se)));
     h->solver.scalar_controller = getenv("B200REG_SCALAR_CTL") != nullptr;
-    h->solver.plain_launch = getenv("B200REG_PLAIN_LAUNCH") != nullptr;
     h->gicp_solver.device_bfgs = getenv("B200REG_GICP_HOST_BFGS") == nullptr;  // developer switch: host-driven BFGS
     h->gicp_solver.init(device, h->stream);
     if (kind == B200REG_GICP) {
@@ -931,23 +909,6 @@ int b200reg_debug_set_voxelgrid_dense_budget(size_t words) {
   return B200REG_OK;
 }
 
-// developer instrumentation, not part of include/b200reg.h: per-round phase stamps of the last solver launch
-int b200reg_debug_timing(b200reg_t h, unsigned long long* out48x8) {
-  if (!h || !out48x8) return B200REG_ERR_ARG;
-  return guarded(h, [&]() {
-    h->solver.read_timing(out48x8);
-    return (int)B200REG_OK;
-  });
-}
-
-int b200reg_debug_cta_eval_ns(b200reg_t h, unsigned* out, int n) {
-  if (!h || !out) return B200REG_ERR_ARG;
-  return guarded(h, [&]() {
-    h->solver.read_cta_eval_ns(out, n);
-    return (int)B200REG_OK;
-  });
-}
-
 int b200reg_gicp_get_covariances(b200reg_t h, int which, double* out9, size_t* n) {
   if (!h || h->kind != B200REG_GICP || !n) return B200REG_ERR_ARG;
   return guarded(h, [&]() {
@@ -1044,7 +1005,7 @@ bool batch_needs_sequential(b200reg_t h) {
   // One launch cannot serve: an empty map (the reference returns the guess), or a configuration whose line search runs
   // the More-Thuente inner loop (step_max <= step_min: it leaves the kernel for the f64 radius Hessian) — those take
   // the single-registration path one by one.
-  return h->map.n_voxels == 0 || !((h->ndt.step_size - h->ndt.trans_eps / 2) > 0) || h->solver.timing_enabled;
+  return h->map.n_voxels == 0 || !((h->ndt.step_size - h->ndt.trans_eps / 2) > 0);
 }
 
 // items: device-resident sources + row-major guesses, already in h->batch_items. after_launch (optional) runs on the host
@@ -1101,28 +1062,18 @@ int ndt_batch_run(b200reg_t h, int count, b200reg_batch_result* results, const s
     return fail(h, B200REG_ERR_ARG, "align_batch with a pose board attached: 1 .. min(board rows, one launch) registrations per call");
   for (int first = 0; first < count; first += per_launch) {
     const int n = std::min(per_launch, count - first);
-    const double tr0 = g_trace ? trace_now() : 0;
-    double tr1 = 0, tr2 = 0;
     {
       std::lock_guard<std::mutex> coop(cooperative_launch_mutex(h->device));
       B200_CUDA(cudaEventRecord(h->ev0, h->stream));
       if (h->board) h->board->view.tag += 1;  // every rank of the board makes the same sequence of batch calls
       h->solver.launch_batch(h->map, items.data() + first, n, h->ndt, h->batch_slots, h->board);
       B200_CUDA(cudaEventRecord(h->ev1, h->stream));
-      if (g_trace) tr1 = trace_now();
       if (after_launch) after_launch();
-      if (g_trace) tr2 = trace_now();
       // The collect kernel goes in behind ev1 (solve_ms stays the solver kernel's own time) and only AFTER the streaming
       // uploads have been issued and drained: a launch parked behind the solver could otherwise sit in front of the
       // copy stream's memory operations on a shared hardware queue while the solver still waits for exactly those.
       if (h->board) h->solver.launch_board_collect(h->board);
       B200_CUDA(cudaStreamSynchronize(h->stream));
-    }
-    if (g_trace) {
-      float kms = 0;
-      cudaEventElapsedTime(&kms, h->ev0, h->ev1);
-      std::fprintf(stderr, "[trace] batch of %d: job table + launch calls %.1f us, uploads issued %.1f us, wait %.1f us (kernel events %.1f us)\n", n,
-                   tr1 - tr0, tr2 - tr1, trace_now() - tr2, 1e3 * kms);
     }
     float ms = 0;
     B200_CUDA(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
@@ -1335,7 +1286,7 @@ extern "C" int b200reg_ndt_sweep(b200reg_t h, int count, const float* const* sou
     return B200REG_ERR_ARG;
   if (stride_bytes < 12 || (stride_bytes % 4) != 0) return B200REG_ERR_ARG;
   if (count == 0) return B200REG_OK;
-  const int n_eng = std::max(1, std::min(std::min(h->sweep_engines, 4), count));
+  const int n_eng = std::min(4, count);  // engines (host threads) the sweep pipelines over
   b200reg_t eng[4] = {h, nullptr, nullptr, nullptr};
   for (int e = 1; e < n_eng; e++) {
     if (!h->siblings[e - 1]) {

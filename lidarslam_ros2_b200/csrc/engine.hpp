@@ -287,11 +287,6 @@ class NdtSolver {
   int index_in_smem() const { return index_in_smem_; }
   int launches = 0;
   bool scalar_controller = false;  // developer switch (env B200REG_SCALAR_CTL=1)
-  bool plain_launch = false;       // developer switch (env B200REG_PLAIN_LAUNCH=1): non-cooperative launch
-  bool timing_enabled = false;  // developer instrumentation (env B200REG_TIMING=1)
-  bool batch_profile = false;   // developer instrumentation (env B200REG_BATCH_PROFILE=1): per-CTA wait / evaluate / reduce cycles
-  void read_timing(unsigned long long* out48x8) const;
-  void read_cta_eval_ns(unsigned* out, int n) const;
   // per-round trace of align-mode single launches (b200reg_ndt_set_trace / b200reg_ndt_get_trace)
   void set_trace(int capacity);
   int read_trace(b200reg_ndt_trace_record* out, int cap);  // copies up to cap records, returns the rounds counted

@@ -14,10 +14,6 @@
 #include <vector>
 
 #include "bfgs6.hpp"
-#include <chrono>
-#include <cstdio>
-#include <cstdlib>
-
 #include "gicp.hpp"
 #include "nn_search.cuh"
 
@@ -999,17 +995,6 @@ b200reg_gicp_trace_record* GicpSolver::trace_slot(int type) {
 
 GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, size_t n_target, const float4* source,
                               size_t n_source, const GicpConfig& cfg, const float* guess16, cudaStream_t s, bool traced) {
-  // developer trace (env B200REG_GICP_TRACE=1): host wall clock per phase of one align, printed to stderr
-  static const bool trace = getenv("B200REG_GICP_TRACE") != nullptr;
-  auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-  double t_prev = trace ? now() : 0, t_cov = 0, t_nn = 0, t_inner = 0;
-  auto lap = [&](double& acc) {
-    if (!trace) return;
-    B200_CUDA(cudaStreamSynchronize(s));
-    const double t = now();
-    acc += t - t_prev;
-    t_prev = t;
-  };
   evaluations_ = 0;
   inner_ms = 0;
   inner_launches = 0;
@@ -1026,7 +1011,6 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
   out.evaluations = 0;
   prepare(target_grid, target, n_target, source, n_source, cfg, guess16, s);
 
-  lap(t_cov);
   float transformation[16], previous[16];
   set_identity16(transformation);
   set_identity16(previous);
@@ -1034,7 +1018,6 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
   int nr_iterations = 0;
   while (!converged) {
     const int m = correspondences(target_grid, cfg, guess16, transformation, s);
-    lap(t_nn);
     std::memcpy(previous, transformation, sizeof(previous));
     if (m < 4) {  // NotEnoughPointsException → caught → break (:187-192, :494-498)
       if (tracing_ && (outer_rec = trace_slot(2))) {
@@ -1119,7 +1102,6 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
         result = bfgs.testGradient(cfg.gradient_tol);
       } while (result == BFGS_Running && inner < cfg.max_inner_iterations);
     }
-    lap(t_inner);
     if (tracing_ && (outer_rec = trace_slot(2))) {
       outer_rec->inner = inner;
       outer_rec->evaluation = evaluations_ - evaluations_before;
@@ -1170,10 +1152,6 @@ GicpOutcome GicpSolver::align(const NnGrid& target_grid, const float4* target, s
     std::memcpy(r->final_T, out.final_T, sizeof(r->final_T));
   }
   tracing_ = false;
-  if (trace)
-    std::fprintf(stderr, "[gicp trace] source grid + covariances + transform %.3f ms, correspondences (NN + Mahalanobis) %.3f ms, "
-                         "inner BFGS launches %.3f ms (kernel events %.3f ms), %d outer iterations, %d evaluations\n",
-                 t_cov, t_nn, t_inner, inner_ms, nr_iterations, evaluations_);
   return out;
 }
 

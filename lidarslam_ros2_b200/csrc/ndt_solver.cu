@@ -65,10 +65,6 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-#define B200_STAMP(cond, round, slot)                                                                  \
-  do {                                                                                                 \
-    if (L.timing && !L.jobs && (cond) && (round) < NDT_TIMING_ROUNDS) W->timing[round][slot] = globaltimer_ns(); \
-  } while (0)
 
 // ---- TMA bulk copy helpers (cp.async.bulk → UBLKCP) -----------------------------------------------------
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -336,7 +332,6 @@ struct CtlShared {
   float facf[8];      // f32 sin/cos of the same angles (for the transform)
   unsigned code[72];  // shared-memory copy of kAngleTableCode
   int ready;          // per-round: bit w set once reducing warp w has summed all its partial rows
-  unsigned long long t_warp[32];  // timing mode: when each reducing warp finished
   // the registration this controller is working on (batch launches take new ones from NdtSolverWork::next_job)
   int cur_job;     // index into NdtLaunch::jobs (0 for a single launch)
   int cur_n_src;   // its source size (trans_probability = score / n_src)
@@ -927,8 +922,6 @@ __device__ __noinline__ void controller_cta(const NdtLaunch& L, CtlShared& cs, d
   }
 
   const int all_ready = (1 << SOLVER_WARPS) - 2;
-  const bool prof = batch && L.timing && tid == 0;  // developer instrumentation: cycles waiting for rows / in the controller step
-  long long c_rows = 0, c_step = 0;
   for (int round = 0;; round++) {
     if (warp != 0) {
       // ---- warps 1..23: fixed-order reduction of the evaluators' partial rows --------------------------------------
@@ -986,7 +979,6 @@ __device__ __noinline__ void controller_cta(const NdtLaunch& L, CtlShared& cs, d
         W->result.error = 1;
         cs.done = 3;
       }
-      if (L.timing && lane == 0) cs.t_warp[warp] = globaltimer_ns();
       __threadfence_block();
       __syncwarp();
       if (lane == 0) atomicOr(&cs.ready, 1 << warp);
@@ -1009,18 +1001,6 @@ __device__ __noinline__ void controller_cta(const NdtLaunch& L, CtlShared& cs, d
         }
       }
       __threadfence_block();
-      const long long t_rows = prof ? clock64() : 0;
-      if (prof) c_rows += t_rows - t0;
-      B200_STAMP(lane == 0, round, 4);
-      if (L.timing && lane == 0 && round < NDT_TIMING_ROUNDS) {
-        unsigned long long tmax = 0, tmin = ~0ull;
-        for (int w = 1; w < SOLVER_WARPS; w++) {
-          tmax = max(tmax, cs.t_warp[w]);
-          tmin = min(tmin, cs.t_warp[w]);
-        }
-        W->timing[round][10] = tmin;
-        W->timing[round][11] = tmax;
-      }
       {
         double t = 0;
 #pragma unroll
@@ -1028,7 +1008,6 @@ __device__ __noinline__ void controller_cta(const NdtLaunch& L, CtlShared& cs, d
         cs.tot[lane] = t;
       }
       __syncwarp();
-      B200_STAMP(lane == 0, round, 5);
       if (lane == 0) cs.build = 0;
       __syncwarp();
       if (cs.done == 3 || round >= NDT_MAX_ROUNDS) {  // watchdog: tell the evaluators to leave
@@ -1043,9 +1022,7 @@ __device__ __noinline__ void controller_cta(const NdtLaunch& L, CtlShared& cs, d
         if (L.trace && lane == 0) cs.trace_fast = handled ? 1 : 0;
         if (!handled && lane == 0) controller(L, cs, W);
         __syncwarp();
-        B200_STAMP(lane == 0, round, 8);
         if (cs.build) build_control(cs, lane);
-        B200_STAMP(lane == 0, round, 9);
         __syncwarp();
         if (L.trace) {
           trace_round(L, cs, lane, round);
@@ -1075,18 +1052,12 @@ __device__ __noinline__ void controller_cta(const NdtLaunch& L, CtlShared& cs, d
       }
       __syncwarp();
       publish(round + pub_shift);
-      if (prof) c_step += clock64() - t_rows;
-      B200_STAMP(lane == 0, round, 6);
       if (lane == 0) cs.ready = 0;
     }
     __syncthreads();
     if (cs.done) break;
   }
   if (batch) {
-    if (prof) {
-      W->cta_eval_ns[n_eval_i + slot][0] = (unsigned)(c_rows >> 10);
-      W->cta_eval_ns[n_eval_i + slot][1] = (unsigned)(c_step >> 10);
-    }
     __threadfence_system();
     return;
   }
@@ -1132,7 +1103,6 @@ __global__ void __launch_bounds__(SOLVER_THREADS, SOLVER_MIN_CTAS) ndt_solver_ke
     return;
   }
   const int my_rank = (int)blockIdx.x;
-  if (L.timing && my_rank == 0 && tid == 0) W->timing[NDT_TIMING_ROUNDS - 1][0] = globaltimer_ns();  // kernel entry
 
   // ---- evaluator CTAs --------------------------------------------------------------------------------------
   // Every evaluator serves all slots in turn: while the controller of one registration reduces, solves and publishes,
@@ -1204,9 +1174,7 @@ __global__ void __launch_bounds__(SOLVER_THREADS, SOLVER_MIN_CTAS) ndt_solver_ke
       }
     }
   }
-  if (L.timing && my_rank == 0 && tid == 0) W->timing[NDT_TIMING_ROUNDS - 1][1] = globaltimer_ns();  // prologue done
   bool skip_eval = L.resume != 0;
-  const bool stamp0 = (my_rank == 0 && tid == 0);
   const float gd2 = (float)L.d2;
   const int pub_shift = batch ? 1 : 0;  // see controller_cta
 
@@ -1218,10 +1186,6 @@ __global__ void __launch_bounds__(SOLVER_THREADS, SOLVER_MIN_CTAS) ndt_solver_ke
     alive[k] = k < n_slots;
   }
   int n_alive = n_slots;
-  // developer instrumentation (L.timing in a batch launch): SM cycles this CTA spent waiting for control blocks,
-  // evaluating, and reducing — read back with b200reg_debug_cta_eval_ns (three counters per CTA, in kilocycles)
-  const bool prof = batch && L.timing && tid == 0;
-  long long c_wait = 0, c_eval = 0, c_red = 0, c_mark = prof ? clock64() : 0;
   for (int s = 0; n_alive > 0; s = (s + 1 >= n_slots) ? 0 : s + 1) {
     int round = 0;
     bool live = false;
@@ -1258,7 +1222,6 @@ __global__ void __launch_bounds__(SOLVER_THREADS, SOLVER_MIN_CTAS) ndt_solver_ke
         payload = (unsigned)v;
       }
       reinterpret_cast<unsigned*>(&ctl_s[s])[tid] = payload;
-      if (!batch && round > 0) B200_STAMP(stamp0, round - 1, 7);
     }
     __syncthreads();
     const NdtControl& ctl = ctl_s[s];
@@ -1269,13 +1232,6 @@ __global__ void __launch_bounds__(SOLVER_THREADS, SOLVER_MIN_CTAS) ndt_solver_ke
       n_alive--;
       continue;
     }
-    if (prof) {
-      const long long t = clock64();
-      c_wait += t - c_mark;
-      c_mark = t;
-    }
-    if (!batch) B200_STAMP(stamp0, round, 0);
-    const unsigned long long t_round = (!batch && L.timing && tid == 0) ? globaltimer_ns() : 0ull;
 
     // ---- (0b) batch: a new registration on this slot — restage its points ----------------------------------------
     if (batch && ctl.job != slot_job[s]) {
@@ -1329,16 +1285,6 @@ __global__ void __launch_bounds__(SOLVER_THREADS, SOLVER_MIN_CTAS) ndt_solver_ke
           }
         }
       }
-      if (prof) {
-        const long long t = clock64();
-        c_eval += t - c_mark;
-        c_mark = t;
-      }
-      if (!batch) B200_STAMP(stamp0, round, 1);
-      if (!batch && L.timing && tid == 0 && round == 2) {
-        W->cta_eval_ns[my_rank][0] = (unsigned)t_round;
-        W->cta_eval_ns[my_rank][1] = (unsigned)globaltimer_ns();
-      }
 
       // ---- (2) per-warp reduction: lane L sums slot L over the warp's 32 columns in fixed order (f64), CTA partial --
       if (acc.first) {
@@ -1385,28 +1331,12 @@ __global__ void __launch_bounds__(SOLVER_THREADS, SOLVER_MIN_CTAS) ndt_solver_ke
         const double sum = (sa + sb) + (sc2 + sd);
         st_relaxed_gpu_u64(reinterpret_cast<unsigned long long*>(&W->partials[s][round & 1][my_rank][tid]),
                            (unsigned long long)__double_as_longlong(sum));
-        if (!batch && L.timing && round == 2 && tid == 0) W->cta_eval_ns[my_rank][2] = (unsigned)globaltimer_ns();
-      }
-      if (prof) {
-        const long long t = clock64();
-        c_red += t - c_mark;
-        c_mark = t;
-      }
-      if (!batch) {
-        B200_STAMP(stamp0, round, 2);
-        B200_STAMP(stamp0, round, 3);
       }
     }
     skip_eval = false;
 #pragma unroll
     for (int k = 0; k < NDT_MAX_SLOTS; k++)
       if (k == s) rounds[k] = round + 1;
-  }
-  if (prof) {
-    W->cta_eval_ns[my_rank][0] = (unsigned)(c_wait >> 10);
-    W->cta_eval_ns[my_rank][1] = (unsigned)(c_eval >> 10);
-    W->cta_eval_ns[my_rank][2] = (unsigned)(c_red >> 10);
-    W->cta_eval_ns[my_rank][3] = (unsigned)((clock64() - c_mark) >> 10);
   }
 }
 
@@ -1457,13 +1387,6 @@ void NdtSolver::init(int device, cudaStream_t s) {
     B200_CUDA(cudaFuncSetAttribute(kernel_for(m), cudaFuncAttributeMaxDynamicSharedMemorySize, SOLVER_MAX_DYN_SMEM));
 }
 
-void NdtSolver::read_cta_eval_ns(unsigned* out, int n) const {
-  B200_CUDA(cudaMemcpy(out, d_work_->cta_eval_ns, sizeof(unsigned) * 4 * n, cudaMemcpyDeviceToHost));
-}
-void NdtSolver::read_timing(unsigned long long* out) const {
-  B200_CUDA(cudaMemcpy(out, d_work_->timing, sizeof(unsigned long long) * NDT_TIMING_ROUNDS * NDT_TIMING_SLOTS,
-                       cudaMemcpyDeviceToHost));
-}
 void NdtSolver::set_trace(int capacity) {
   if (d_trace_) cudaFree(d_trace_);
   d_trace_ = nullptr;
@@ -1541,7 +1464,6 @@ void NdtSolver::fill_common(NdtLaunch& L, const VoxelMap& map, const NdtConfig& 
   L.n_voxels = (int)map.n_voxels;
   L.search_method = cfg.search_method;
   L.mode = mode;
-  L.timing = timing_enabled ? 1 : 0;
   L.scalar_controller = scalar_controller ? 1 : 0;
   L.epoch = epoch_++;
   L.max_iterations = cfg.max_iterations;
@@ -1609,11 +1531,7 @@ void NdtSolver::launch(const VoxelMap& map, const float4* src, size_t n_src, con
   block_ = SOLVER_THREADS;
   KernelFn fn = kernel_for(cfg.search_method);
   void* args[] = {&L};
-  if (plain_launch) {  // developer switch: measure what the cooperative launch costs
-    B200_CUDA(cudaLaunchKernel((const void*)fn, dim3(grid_), dim3(SOLVER_THREADS), args, dyn_smem, stream_));
-  } else {
-    B200_CUDA(cudaLaunchCooperativeKernel((const void*)fn, dim3(grid_), dim3(SOLVER_THREADS), args, dyn_smem, stream_));
-  }
+  B200_CUDA(cudaLaunchCooperativeKernel((const void*)fn, dim3(grid_), dim3(SOLVER_THREADS), args, dyn_smem, stream_));
   launches += 1;
 }
 
@@ -1693,7 +1611,6 @@ void NdtSolver::launch_batch(const VoxelMap& map, const BatchItem* items, int n,
   size_t dyn_smem = 0;
   const int n_slots = std::max(1, std::min(std::min(slots, NDT_MAX_SLOTS), n));
   fill_common(L, map, cfg, NDT_MODE_ALIGN, n_slots, dyn_smem);
-  L.timing = batch_profile ? 1 : 0;
   L.result_host = h_batch_results_;
   L.jobs = d_jobs_;
   L.n_jobs = n;

@@ -49,10 +49,6 @@ struct NdtState {
   int phase, nr_iterations, evaluations, converged;
 };
 
-constexpr int NDT_TIMING_ROUNDS = 48;
-constexpr int NDT_TIMING_SLOTS = 12;
-// slots (globaltimer ns): 0 CTA0 round start, 1 CTA0 after evaluate, 2/3 CTA0 partial row stored,
-//                         4 last CTA detected, 5 partials reduced, 6 controller done, 7 CTA0 released
 // Signalling between the evaluator CTAs and the controller CTA carries its own validity ("flag in data", as in NCCL's
 // LL protocol), so neither direction needs a counter, a fence or a second dependent round trip:
 //  * control block, controller -> evaluators: every 32-bit word travels as one 64-bit store {payload, sequence}; an
@@ -95,8 +91,6 @@ struct NdtSolverWork {
   NdtResult result;
   alignas(128) unsigned long long ctl_ll[NDT_MAX_SLOTS][NDT_CTL_COPIES][NDT_CTL_LL_WORDS];
   alignas(128) double partials[NDT_MAX_SLOTS][2][NDT_MAX_CTAS][SLOT_COUNT];
-  unsigned long long timing[NDT_TIMING_ROUNDS][NDT_TIMING_SLOTS];
-  unsigned cta_eval_ns[NDT_MAX_CTAS][4];  // timing mode, round 2, low 32 bits of globaltimer: start, evaluate end, published
 };
 
 struct NdtLaunch {
@@ -122,7 +116,6 @@ struct NdtLaunch {
   int acc_offset;         // byte offset of the per-thread accumulators in dynamic shared memory (after the rank index)
   int pts_offset;         // byte offset of the staged source points (n_slots x SMEM_POINTS float4) after the accumulators
   int scalar_controller;  // 1: disable the warp-parallel controller fast path (developer switch)
-  int timing;  // 1: record per-phase globaltimer stamps into work->timing (developer instrumentation)
   int resume;  // 1: state/control already in work (after a K2 pass); first round skips the evaluation
   int index_in_smem;
   int max_iterations;

@@ -8,7 +8,7 @@ from lidarslam_ros2_b200 import synth
 cfg, res = sys.argv[1], float(sys.argv[2])
 src, tgt, _ = synth.registration_pair(cfg, res)
 o = oracle.NDT(resolution=res, transformation_epsilon=0.01); o.set_target(tgt); o.set_source(src); To = o.align()
-print("timing env:", os.environ.get("B200REG_TIMING"), "oracle iters", o.iterations)
+print("oracle iters", o.iterations)
 g = m.NormalDistributionsTransform(); g.setResolution(res); g.setTransformationEpsilon(0.01)
 g.setInputTarget(tgt); g.setInputSource(src)
 for k in range(4):
