@@ -532,6 +532,62 @@ int b200sm_get_occupancy_grid(b200sm_t s, signed char* data, unsigned* hits, uns
  * nav2's map_saver's as its documentation states it; csrc/occupancy_grid.hpp's text is the contract. No grid built yet:
  * B200REG_ERR_ARG. A file that cannot be opened or written: B200REG_ERR_IO. */
 int b200sm_save_occupancy_map(b200sm_t s, const char* pgm_path, const char* yaml_path);
+/* ---- static map: the map without what moved while it was recorded ---------------------------------------------------
+ * No counterpart in the reference. Every submap's points are rays from its sensor origin through a 3D voxel grid: the
+ * endpoint is the point b200sm_assemble_map(s, poses_colmajor16, ...) returns for it, the origin the same float pose
+ * applied to (float) sensor_origin. A ray HITS its endpoint's voxel and FREES the voxels of the first ray_fraction of its
+ * length (a 6-connected Amanatides-Woo walk in 2^16-per-voxel fixed point; the rest of the ray is not freed, because rays
+ * that graze a surface cross its voxels just before their ends). Only voxels some endpoint lies in are counted; within one
+ * submap a hit voxel is not free (OctoMap's per-scan update). Each voxel counts the submaps that hit it and those that
+ * freed it; it is DYNAMIC when frees >= min_frees and round-half-up of 100 * hits / (hits + frees) <= rint(100 *
+ * dynamic_thresh). The static map is the assembled map, in its order, without the points whose voxel is dynamic; points
+ * that are not rays (non-finite, or beyond max_range) are kept. The exact definitions are in csrc/static_map.hpp;
+ * DESIGN.md section 7b describes the build. Counts of per-submap booleans do not depend on the order of the work, so the
+ * result is bitwise deterministic. Each call rebuilds from all submaps; the session's submaps are not changed. NDT and GICP
+ * sessions alike; no registration handle is involved. */
+typedef struct b200sm_static_map_params {
+  double resolution;        /* metres per voxel, finite, > 0; default 0.2                                             */
+  double max_range;         /* finite, > 0: rays longer than this are not cast (their points are kept); default 100;
+                               max_range / resolution <= 2^14                                                         */
+  double sensor_origin[3];  /* LiDAR position in the robot frame (as for b200sm_build_occupancy_grid); default 0       */
+  double ray_fraction;      /* the part of each ray that frees voxels, (0, 1] (rint(ray_fraction * 2^16) >= 1);
+                               default 0.85                                                                           */
+  unsigned min_frees;       /* >= 1; default 2                                                                        */
+  double dynamic_thresh;    /* [0, 1]; default 0.4                                                                    */
+} b200sm_static_map_params;
+typedef struct b200sm_static_map_info {
+  int box_origin[3];                 /* voxel (i, j, k) of the box's lower corner: map x in [i, i + 1) * resolution */
+  unsigned box_dims[3];              /* voxels; the box bounds every ray's endpoint voxel (0 when there is no ray)   */
+  unsigned long long n_rays, n_skipped; /* points cast as rays / not cast (non-finite, or beyond max_range)          */
+  unsigned long long n_voxels, n_dynamic_voxels; /* voxels some endpoint lies in; of those, the dynamic ones         */
+  unsigned long long n_points, n_static_points;  /* the assembled map; the static map                               */
+  int n_batches;                     /* launches of the walks (submaps batched by a fixed 64 MiB bitmap budget)      */
+} b200sm_static_map_info;
+/* Build the static map from every submap at its own pose (poses_colmajor16 NULL) or at the given 16 * n_submaps doubles
+ * (the output of b200sm_pose_adjust). params NULL: the defaults. A parameter out of range, a non-finite pose entry, a
+ * sensor origin beyond 2^30 voxels, no submaps, a map of 2^32 points or more, or a box of more than 2^31 - 1 voxels:
+ * B200REG_ERR_ARG, checked before anything is sized from the box (the box is measured on the device first, with 120
+ * bytes per submap of tables); the previous build stays. The session keeps the build until the next one or destroy:
+ * the rank index (8 bytes per 32 box voxels), 9 bytes per occupied voxel (hits, frees, flag), the static map (16 bytes per
+ * point), the walks' bitmap scratch (the largest batch: at most 64 MiB, or two bits per occupied voxel when that is
+ * more) and 4 bytes per 1024 points of tile counts. info may be NULL. */
+int b200sm_build_static_map(b200sm_t s, const double* poses_colmajor16, const b200sm_static_map_params* params,
+                            b200sm_static_map_info* info);
+/* The last static map: x, y, z, intensity floats. *n = its points; min(*n, capacity) points are copied, so capacity 0 is
+ * a size query. offsets (may be NULL) = n_submaps at the build + 1 prefix sums: submap i's kept points are
+ * out[offsets[i] .. offsets[i+1]) (modified_map_array's i-th SubMap without its dynamic points). No build yet:
+ * B200REG_ERR_ARG. */
+int b200sm_get_static_map(b200sm_t s, float* out_xyzi, size_t capacity, size_t* n, size_t* offsets);
+/* The occupied voxels of the last build in rank order (ascending (k, j, i) within the box): *n = their number;
+ * min(*n, capacity) rows of each non-NULL array: ijk3 (3 ints, the voxel), hits, frees, dynamic (0 / 1). For tuning the
+ * parameters. No build yet: B200REG_ERR_ARG. */
+int b200sm_get_map_voxels(b200sm_t s, int* ijk3, unsigned* hits, unsigned* frees, unsigned char* dynamic, size_t capacity,
+                          size_t* n);
+/* pcl::io::savePCDFileASCII(path, static map): the text of b200sm_save_map_pcd_ascii for the last static map, formatted
+ * on the device and written by the same double-buffered chunks. n_points, n_bytes (may be NULL) = points and file size.
+ * No build yet, or a static map without points (no file is created): B200REG_ERR_ARG. A file that cannot be opened or
+ * written: B200REG_ERR_IO. */
+int b200sm_save_static_map_pcd_ascii(b200sm_t s, const char* path, size_t* n_points, size_t* n_bytes);
 /* The same text for a HOST PointXYZI cloud (records as in b200sm_import_submap; intensity_offset_bytes >= 0), formatted
  * on `device`. *n_bytes = size of the whole file content (header and data); min(*n_bytes, capacity) bytes are copied to
  * out, so capacity 0 is a size query. B200REG_ERR_ARG for n == 0, a negative intensity offset, or a stride or offset that

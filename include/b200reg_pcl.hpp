@@ -510,6 +510,34 @@ class ScanMatcherSession {
   void saveOccupancyMap(const std::string& pgm_path, const std::string& yaml_path) {
     check(b200sm_save_occupancy_map(s_.get(), pgm_path.c_str(), yaml_path.c_str()));
   }
+  // ---- static map (b200sm_build_static_map): the map without what moved while it was recorded; poses empty = the
+  // submaps' own, else 16 doubles per submap, column-major (b200sm_pose_adjust's output); p nullptr = the defaults
+  b200sm_static_map_info buildStaticMap(const std::vector<double>& poses_colmajor16 = {}, const b200sm_static_map_params* p = nullptr) {
+    b200sm_static_map_info info{};
+    check(b200sm_build_static_map(s_.get(), poses_colmajor16.empty() ? nullptr : poses_colmajor16.data(), p, &info));
+    sm_sub_ = numSubmaps();
+    return info;
+  }
+  // the last static map, x y z intensity per point; offsets (when non-null) = per-submap prefix sums (submaps at the build + 1)
+  void staticMap(std::vector<float>& xyzi, std::vector<size_t>* offsets = nullptr) {
+    size_t n = 0;
+    check(b200sm_get_static_map(s_.get(), nullptr, 0, &n, nullptr));
+    xyzi.resize(4 * n);
+    if (offsets) offsets->resize(sm_sub_ + 1);
+    check(b200sm_get_static_map(s_.get(), xyzi.data(), n, &n, offsets ? offsets->data() : nullptr));
+  }
+  // the occupied voxels of the last build in rank order: 3 ints each, hits, frees, dynamic flags
+  void mapVoxels(std::vector<int>& ijk3, std::vector<unsigned>& hits, std::vector<unsigned>& frees, std::vector<unsigned char>& dynamic) {
+    size_t n = 0;
+    check(b200sm_get_map_voxels(s_.get(), nullptr, nullptr, nullptr, nullptr, 0, &n));
+    ijk3.resize(3 * n);
+    hits.resize(n);
+    frees.resize(n);
+    dynamic.resize(n);
+    check(b200sm_get_map_voxels(s_.get(), ijk3.data(), hits.data(), frees.data(), dynamic.data(), n, &n));
+  }
+  // PCL's ASCII PCD of the last static map (as saveMapPCDASCII writes the map)
+  void saveStaticMapPcd(const std::string& path) { check(b200sm_save_static_map_pcd_ascii(s_.get(), path.c_str(), nullptr, nullptr)); }
   b200sm_localize_stats localizeStats() const {
     b200sm_localize_stats st{};
     check(b200sm_get_localize_stats(s_.get(), &st));
@@ -529,6 +557,7 @@ class ScanMatcherSession {
   }
   std::shared_ptr<b200sm_session> s_;
   size_t og_cells_ = 0;  // cells of the last grid this adapter built
+  size_t sm_sub_ = 0;    // submaps at the last static-map build of this adapter
 };
 
 }  // namespace b200reg

@@ -50,6 +50,7 @@ SYMBOLS = [
     "b200sm_localize_global", "b200sm_get_global_search",
     "b200sm_set_scan_context_params", "b200sm_get_scan_context", "b200sm_search_loop_place", "b200sm_get_place_scores",
     "b200sm_build_occupancy_grid", "b200sm_get_occupancy_grid", "b200sm_save_occupancy_map",
+    "b200sm_build_static_map", "b200sm_get_static_map", "b200sm_get_map_voxels", "b200sm_save_static_map_pcd_ascii",
     # include/b200comm.h
     "b200comm_unique_id", "b200comm_create", "b200comm_destroy", "b200comm_all_gather_rows", "b200comm_rank", "b200comm_last_error",
     "b200comm_board_create", "b200comm_board_destroy", "b200comm_board_info",
@@ -80,6 +81,17 @@ class SmOccupancyInfo(C.Structure):
     _fields_ = [("width", C.c_uint), ("height", C.c_uint), ("origin", C.c_double * 2), ("resolution", C.c_double),
                 ("n_rays", C.c_ulonglong), ("n_skipped", C.c_ulonglong), ("n_batches", C.c_int), ("n_occupied", C.c_ulonglong),
                 ("n_free", C.c_ulonglong), ("n_unknown", C.c_ulonglong)]
+
+
+class SmStaticMapParams(C.Structure):
+    _fields_ = [("resolution", C.c_double), ("max_range", C.c_double), ("sensor_origin", C.c_double * 3),
+                ("ray_fraction", C.c_double), ("min_frees", C.c_uint), ("dynamic_thresh", C.c_double)]
+
+
+class SmStaticMapInfo(C.Structure):
+    _fields_ = [("box_origin", C.c_int * 3), ("box_dims", C.c_uint * 3), ("n_rays", C.c_ulonglong), ("n_skipped", C.c_ulonglong),
+                ("n_voxels", C.c_ulonglong), ("n_dynamic_voxels", C.c_ulonglong), ("n_points", C.c_ulonglong),
+                ("n_static_points", C.c_ulonglong), ("n_batches", C.c_int)]
 
 
 class SmLoopEdge(C.Structure):
@@ -254,6 +266,10 @@ def lib() -> C.CDLL:
     L.b200sm_build_occupancy_grid.argtypes = [vp, vp, C.POINTER(SmOccupancyParams), C.POINTER(SmOccupancyInfo)]
     L.b200sm_get_occupancy_grid.argtypes = [vp, vp, vp, vp, sz]
     L.b200sm_save_occupancy_map.argtypes = [vp, C.c_char_p, C.c_char_p]
+    L.b200sm_build_static_map.argtypes = [vp, vp, C.POINTER(SmStaticMapParams), C.POINTER(SmStaticMapInfo)]
+    L.b200sm_get_static_map.argtypes = [vp, vp, sz, C.POINTER(sz), vp]
+    L.b200sm_get_map_voxels.argtypes = [vp, vp, vp, vp, vp, sz, C.POINTER(sz)]
+    L.b200sm_save_static_map_pcd_ascii.argtypes = [vp, C.c_char_p, C.POINTER(sz), C.POINTER(sz)]
     L.b200comm_unique_id.argtypes = [vp]
     L.b200comm_create.argtypes = [vp, i, i, i, C.POINTER(vp)]
     L.b200comm_destroy.argtypes = [vp]

@@ -381,6 +381,55 @@ class ScanMatcher:
         """nav2 map_server's map.pgm + map.yaml pair of the last grid (trinary)."""
         self._check(self._lib.b200sm_save_occupancy_map(self._h, os.fsencode(pgm_path), os.fsencode(yaml_path)))
 
+    # ---- static map: what moved while the map was recorded removed (b200sm_build_static_map, csrc/static_map.hpp) ----
+    def buildStaticMap(self, poses=None, resolution: float = 0.2, max_range: float = 100.0, sensor_origin=(0.0, 0.0, 0.0),
+                       ray_fraction: float = 0.85, min_frees: int = 2, dynamic_thresh: float = 0.4) -> dict:
+        """The map without its dynamic points, every submap at its own pose (poses None) or at `poses` (N, 4, 4), e.g.
+        poseAdjust's: each point is a ray from its submap's sensor origin (sensor_origin: the LiDAR in the robot frame) through
+        a 3D voxel grid; the first ray_fraction of each ray frees the voxels it crosses, and a voxel freed by at least
+        min_frees submaps and hit by at most dynamic_thresh of those that saw it is dynamic. Returns the build's info as a
+        dict (box_origin, box_dims, n_rays, n_skipped, n_voxels, n_dynamic_voxels, n_points, n_static_points, n_batches)."""
+        P = None
+        if poses is not None:
+            P = np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(self.numSubmaps(), 4, 4).transpose(0, 2, 1))
+        so = (C.c_double * 3)(*[float(v) for v in sensor_origin])
+        prm = _capi.SmStaticMapParams(float(resolution), float(max_range), so, float(ray_fraction), int(min_frees),
+                                      float(dynamic_thresh))
+        info = _capi.SmStaticMapInfo()
+        self._check(self._lib.b200sm_build_static_map(self._h, _ptr(P) if P is not None else None, C.byref(prm), C.byref(info)))
+        self._sm_sub = self.numSubmaps()
+        return _struct_dict(info)
+
+    def staticMap(self, capacity=None):
+        """The last static map: (cloud (M, 4) float32 in the assembled map's order, offsets (N + 1,) int64 per submap, N the
+        submaps at the build). capacity: copy at most that many points."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_get_static_map(self._h, None, 0, C.byref(n), None))
+        m = n.value if capacity is None else min(int(capacity), n.value)
+        offsets = np.zeros(getattr(self, "_sm_sub", 0) + 1, dtype=np.uint64)
+        out = np.empty((max(m, 1), 4), dtype=np.float32)
+        self._check(self._lib.b200sm_get_static_map(self._h, _ptr(out), m, C.byref(n), _ptr(offsets)))
+        return out[:m], offsets.astype(np.int64)
+
+    def mapVoxels(self) -> dict:
+        """The occupied voxels of the last build in rank order: ijk (V, 3) int32, hits, frees (V,) uint32, dynamic (V,) bool."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_get_map_voxels(self._h, None, None, None, None, 0, C.byref(n)))
+        V = n.value
+        ijk = np.empty((max(V, 1), 3), dtype=np.int32)
+        hits = np.empty(max(V, 1), dtype=np.uint32)
+        frees = np.empty(max(V, 1), dtype=np.uint32)
+        dyn = np.empty(max(V, 1), dtype=np.uint8)
+        self._check(self._lib.b200sm_get_map_voxels(self._h, _ptr(ijk), _ptr(hits), _ptr(frees), _ptr(dyn), V, C.byref(n)))
+        return dict(ijk=ijk[:V], hits=hits[:V], frees=frees[:V], dynamic=dyn[:V].astype(bool))
+
+    def saveStaticMapPcd(self, path):
+        """pcl::io::savePCDFileASCII(path, static map) of the last build, as saveMapPCDASCII writes a map. Returns (points,
+        file bytes)."""
+        n, size = C.c_size_t(0), C.c_size_t(0)
+        self._check(self._lib.b200sm_save_static_map_pcd_ascii(self._h, os.fsencode(path), C.byref(n), C.byref(size)))
+        return int(n.value), int(size.value)
+
     # ---- read-back ----
     def stats(self) -> dict:
         st = _capi.SmStats()
@@ -418,6 +467,10 @@ class ScanMatcher:
 
 def _occupancy_info(info) -> dict:
     return {k: (tuple(getattr(info, k)) if k == "origin" else getattr(info, k)) for k, _ in _capi.SmOccupancyInfo._fields_}
+
+
+def _struct_dict(st) -> dict:
+    return {k: (tuple(getattr(st, k)) if hasattr(getattr(st, k), "_length_") else getattr(st, k)) for k, _ in st._fields_}
 
 
 def backend_registration(registration_method: str = "NDT", ndt_resolution: float = 5.0, ndt_num_threads: int = 0, device: int = 0):
