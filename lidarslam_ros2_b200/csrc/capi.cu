@@ -83,7 +83,6 @@ struct b200reg_engine {
   int sibling_launches_seen[3] = {0, 0, 0};
   cudaStream_t copy_stream = nullptr;    // streaming uploads of b200reg_ndt_align_batch
   DeviceBuffer<unsigned> batch_ready;    // one "scan k has arrived" flag per registration of a batch
-  unsigned batch_tag = 0;                // value the flags take for the current call
   b200reg_engine* siblings[3] = {nullptr, nullptr, nullptr};  // further engines of b200reg_ndt_sweep (own stream and buffers each)
 
   // b200reg_ndt_score_poses
@@ -1030,12 +1029,24 @@ int ndt_batch_run(b200reg_t h, int count, b200reg_batch_result* results, const s
   if (sequential && h->board)
     return fail(h, B200REG_ERR_ARG, "align_batch with a pose board attached needs the one-launch path (non-empty map, step_size > transformation_epsilon / 2)");
   if (sequential) {
+    // Each registration reads its float4 scan in place; the handle's own source is put back afterwards (also when a
+    // call throws), so that the calls after the batch (align, derivatives, getAligned, ...) see the source the caller
+    // set, as they do after a one-launch batch.
+    struct KeepSource {
+      b200reg_t h;
+      const float4* view;
+      size_t n;
+      bool have;
+      ~KeepSource() {
+        h->src_view = view;
+        h->n_source = n;
+        h->have_source = have;
+      }
+    } keep{h, h->src_view, h->n_source, h->have_source};
     int worst = B200REG_OK;
     float ms = 0;
     for (int k = 0; k < count; k++) {
-      h->d_source.ensure(items[k].n_src);
-      B200_CUDA(cudaMemcpyAsync(h->d_source.ptr, items[k].src, items[k].n_src * sizeof(float4), cudaMemcpyDeviceToDevice, h->stream));
-      h->src_view = h->d_source.ptr;
+      h->src_view = static_cast<const float4*>(items[k].src);
       h->n_source = items[k].n_src;
       h->have_source = true;
       float Tc[16];
@@ -1179,8 +1190,18 @@ int b200reg_ndt_align_batch(b200reg_t h, int count, const float* const* sources,
       // flag. Registration k starts as soon as scan k is there, so the upload of the later scans (and, for pageable
       // memory, the CPU staging copy) is hidden behind the registration of the earlier ones.
       if (!h->copy_stream) B200_CUDA(cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
-      h->batch_ready.ensure((size_t)count);
-      const unsigned tag = ++h->batch_tag;
+      // The flags are not cleared before every launch. A newly allocated buffer is zeroed once, so it holds flags and
+      // nothing else, and the value a call waits for is new to the whole process: a leftover value equal to it would
+      // let the solver read a scan before its copy has arrived.
+      if ((size_t)count > h->batch_ready.cap) {
+        h->batch_ready.ensure((size_t)count);
+        B200_CUDA(cudaMemsetAsync(h->batch_ready.ptr, 0, h->batch_ready.cap * sizeof(unsigned), h->stream));
+        B200_CUDA(cudaStreamSynchronize(h->stream));  // done before the copy stream raises any flag
+      }
+      static std::atomic<unsigned> last_tag{0};
+      unsigned tag;
+      do tag = last_tag.fetch_add(1u) + 1u;
+      while (tag == 0u);
       for (int k = 0; k < count; k++) {
         NdtSolver::BatchItem& it = h->batch_items[k];
         it.src = h->batch_uploader.raw.ptr + raw_off[k];

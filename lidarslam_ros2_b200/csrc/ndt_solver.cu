@@ -1110,6 +1110,7 @@ __global__ void __launch_bounds__(SOLVER_THREADS, SOLVER_MIN_CTAS) ndt_solver_ke
   // the sequential part of a Newton round.
   __shared__ __align__(16) NdtControl ctl_s[NDT_MAX_SLOTS];
   __shared__ int abort_flag;
+  __shared__ unsigned lapped_to;  // batch: the latest control-block sequence a lapped CTA found (0: none)
   __shared__ __align__(8) unsigned long long tma_bar;
   __shared__ const unsigned char* slot_src[NDT_MAX_SLOTS];
   __shared__ int slot_nsrc[NDT_MAX_SLOTS], slot_job[NDT_MAX_SLOTS], slot_stride[NDT_MAX_SLOTS];
@@ -1161,7 +1162,11 @@ __global__ void __launch_bounds__(SOLVER_THREADS, SOLVER_MIN_CTAS) ndt_solver_ke
     }
   };
   if (tid < NDT_MAX_SLOTS) slot_job[tid] = -1;
-  if (tid == 0) abort_flag = 0;
+  if (tid == 0) {
+    abort_flag = 0;
+    lapped_to = 0u;
+  }
+  __syncthreads();
   if (!batch) stage_points(0, reinterpret_cast<const unsigned char*>(L.src), 16, L.n_src);
 
   if (L.index_in_smem) {
@@ -1200,30 +1205,50 @@ __global__ void __launch_bounds__(SOLVER_THREADS, SOLVER_MIN_CTAS) ndt_solver_ke
     // ---- (0) the control block of (slot s, round): from the launch parameters (single launch, round 0) or from the
     // slot's controller CTA — thread k polls word k until it carries the expected sequence number (one 64-bit load
     // brings payload and validity together) -----------------------------------------------------------------------
-    if (tid < NDT_CONTROL_WORDS) {
-      unsigned payload;
-      if (!batch && round == 0) {
-        const int* src = L.resume ? reinterpret_cast<const int*>(&W->control) : reinterpret_cast<const int*>(&L.init);
-        payload = (unsigned)(L.resume ? __ldcg(src + tid) : src[tid]);
-      } else {
-        const unsigned long long* wsrc = &W->ctl_ll[s][my_rank % NDT_CTL_COPIES][tid];
-        const unsigned want = ctl_sequence(L.epoch, round - 1 + pub_shift);
-        const long long t0 = clock64();
-        unsigned long long v;
-        for (;;) {
-          v = ld_relaxed_gpu_u64(wsrc);
-          if ((unsigned)(v >> 32) == want) break;
-          if (clock64() - t0 > SPIN_TIMEOUT_CYCLES) {
-            W->result.error = 1;
-            abort_flag = 1;
-            break;
+    // A batch slot's controller waits only for the evaluators that own points of its current registration. The others
+    // still step through its rounds, and one busy with a long evaluation for another slot can be lapped: the block it
+    // waits for has already been replaced by a later one. Such a CTA owns no points of the rounds it missed, so it takes
+    // the latest block instead (lapped_to: the sequence every word of it must carry). A CTA that owns points of a round
+    // cannot be lapped there, since the controller waits for its row.
+    unsigned want = ctl_sequence(L.epoch, round - 1 + pub_shift);
+    for (;;) {
+      if (tid < NDT_CONTROL_WORDS) {
+        unsigned payload;
+        if (!batch && round == 0) {
+          const int* src = L.resume ? reinterpret_cast<const int*>(&W->control) : reinterpret_cast<const int*>(&L.init);
+          payload = (unsigned)(L.resume ? __ldcg(src + tid) : src[tid]);
+        } else {
+          const unsigned long long* wsrc = &W->ctl_ll[s][my_rank % NDT_CTL_COPIES][tid];
+          const long long t0 = clock64();
+          unsigned long long v;
+          for (;;) {
+            v = ld_relaxed_gpu_u64(wsrc);
+            const int ahead = (int)((unsigned)(v >> 32) - want);  // < 0: an older block (this launch's or an earlier one's)
+            if (ahead == 0) break;
+            if (ahead > 0 && ahead < 65536) {
+              atomicMax(&lapped_to, (unsigned)(v >> 32));
+              break;
+            }
+            if (clock64() - t0 > SPIN_TIMEOUT_CYCLES) {
+              W->result.error = 1;
+              abort_flag = 1;
+              break;
+            }
           }
+          payload = (unsigned)v;
         }
-        payload = (unsigned)v;
+        reinterpret_cast<unsigned*>(&ctl_s[s])[tid] = payload;
       }
-      reinterpret_cast<unsigned*>(&ctl_s[s])[tid] = payload;
+      __syncthreads();
+      const unsigned to = lapped_to;
+      if (to == 0u || abort_flag) break;
+      __syncthreads();  // every thread has read lapped_to
+      if (tid == 0) lapped_to = 0u;
+      __syncthreads();
+      round += (int)(to - want);
+      want = to;
+      // (the words are read again for exactly `to`, or for a later block if the controller moved on once more)
     }
-    __syncthreads();
     const NdtControl& ctl = ctl_s[s];
     if (ctl.mode != EVAL_DERIV || abort_flag) {  // this slot is finished (or the watchdog fired)
 #pragma unroll
