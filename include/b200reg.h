@@ -469,6 +469,73 @@ typedef struct b200sm_pose_adjust_result {
  * num_adjacent_pose_cnstraints < 1 or max_iterations < 0. optimizer.save("pose_graph.g2o") (:319) is not reproduced. */
 int b200sm_pose_adjust(b200sm_t s, int num_adjacent_pose_cnstraints, const b200sm_loop_edge* loop_edges, int n_loop_edges,
                        int max_iterations, double* poses_out, b200sm_pose_adjust_result* result);
+
+/* ---- merging a second mapping session into the session's map ---------------------------------------------------------
+ * A session's submaps form segments: one recording's contiguous run each. A session starts with one; every successful
+ * b200sm_merge_session appends the other session's submaps as a new one. On a session of more than one segment
+ * b200sm_set_scan, b200sm_receive_cloud and b200sm_update_map return B200REG_ERR_ARG and change nothing (it is a backend's
+ * map); b200sm_import_submap appends to the last segment; b200sm_pose_adjust puts its odometry edges inside each segment
+ * (with one segment: exactly the edges above); the loop searches, the map assembly, PCD saving, the occupancy grid and the
+ * static map work on all the submaps. Definitions: csrc/session_merge.hpp; DESIGN.md section 7b.                       */
+typedef struct b200sm_merge_params {
+  double sc_threshold;                  /* candidates need D < sc_threshold; finite, default 0.4                   */
+  int top_k;                            /* candidates kept per src submap, 1..32, default 3                          */
+  int max_verifications;                /* candidates verified, best (D, b, a) first, 1..1024, default 64            */
+  float voxel_leaf_size;                /* VoxelGrid of the verification's target window, > 0, default 0.3           */
+  double threshold_loop_closure_score;  /* a verified pair is accepted iff fitness < this; not NaN, default 1.0       */
+  int search_submap_num;                /* target window a +- search_submap_num (inside a's segment), >= 0, default 1 */
+  double consistency_translation;       /* cycle-error tolerance |t(E)| <= t + drift_t * L, metres, default 1.5      */
+  double consistency_rotation;          /* acos((tr R(E) - 1) / 2) <= r + drift_r * L, radians, default 0.1           */
+  double consistency_drift_translation; /* per metre travelled around the cycle, default 0.02                         */
+  double consistency_drift_rotation;    /* radians per metre, default 0.003; the four: finite, >= 0                   */
+  int min_inliers;                      /* the merge succeeds iff the consistent set has this many rows, >= 1, def. 2 */
+  int num_adjacent_pose_cnstraints;     /* odometry edges of the joint adjustment, >= 1, default 5                    */
+  int max_iterations;                   /* LM iterations of the joint adjustment, >= 0, default 10                    */
+} b200sm_merge_params;
+typedef struct b200sm_merge_row {
+  b200sm_place_result place;  /* loop.id_min = a (dst), loop.relative_pose = Z = P_a^-1 (F P_b) when accepted,
+                                 loop.min_dist = |t(P_a) - t(F P_b)|; guess = P_a Rz(2 pi s* / S) P_b^-1; sc_distance, shift */
+  int src_id;                 /* b (src)                                                                                  */
+  int inlier;                 /* rank in the consistent set (the order of the inter-session edges), -1 when not in it    */
+} b200sm_merge_row;
+typedef struct b200sm_merge_result {
+  int merged;                       /* 1: src was appended to dst as a new segment                                        */
+  int query_tile;                   /* src descriptors per block of the score launch                                     */
+  unsigned long long pairs_scored;  /* n_A * n_B                                                                          */
+  int candidates, verified, accepted, inliers;
+  int first_submap;                 /* the new segment's first submap (n_A), -1 when not merged                          */
+  double T[16];                     /* T*, the first inlier's F (column-major): the rigid placement X_b = T* P_b        */
+  b200sm_pose_adjust_result adjust; /* the joint adjustment (zero when not merged)                                        */
+} b200sm_merge_result;
+/* Merge session src (B, any frame) into dst (A): (1) D(b, a) and s* of every src submap b against every dst submap a, on
+ * the device in one launch (Scan Context, bitwise b200sm_search_loop_place's for the same pair); (2) per b the first
+ * top_k a with D < sc_threshold in (D, a) order, selected on the device; all of them ordered by (D, b, a), the first
+ * max_verifications verified; (3) a verification is b200sm_search_loop_place's with source = src submap b moved by its
+ * pose, target = VoxelGrid(voxel_leaf_size) of dst submaps a +- search_submap_num inside a's segment and guess
+ * sc_guess(P_a, P_b, s*); (4) the accepted rows in (fitness, row) order each join the consistent set iff their cycle error
+ * with every row already in it is within tolerance; (5) with at least min_inliers rows: X_b = T* P_b, the joint pose
+ * adjustment over dst's submaps then src's at X_b (numbered n_A + b), odometry edges per segment, then loop_edges (merged
+ * numbering), then (a, n_A + b, Z) per inlier in rank order; vertex 0 fixed; poses_out (may be NULL) = (n_A + n_B) * 16
+ * doubles column-major; (6) src's submaps (clouds device to device, intensity included) are appended to dst at X_b with
+ * distance d_{A,last} + d_b, as a new segment (as several when src is itself a merged map: its segments are kept). The
+ * odometry rule leaves the first submap of every segment without an odometry edge, as the reference leaves vertex 0: an
+ * appended segment's first submap moves in the adjustment only through a loop edge of its own (an inlier with b = 0, or a
+ * caller's edge), and otherwise stays at X_b. A candidate with an empty src submap or an empty target window is reported
+ * as a row that is not accepted (fitness = HUGE_VAL) and registers nothing. b200sm_pose_adjust(dst) with loop_edges followed by the inter-session edges
+ * gives poses_out bit for bit. src is only read. Otherwise (no candidate, or fewer inliers) B200REG_OK with merged = 0:
+ * the rows are reported, poses_out is untouched and dst's submaps, poses, segments and descriptors are as they were.
+ * rows[0 .. *n_rows) = min(verified, capacity) rows in verification order. params NULL: the defaults. B200REG_ERR_ARG,
+ * with nothing changed, for a NULL handle, dst == src, sessions on different devices or with different Scan Context
+ * parameters, an empty session, n_A * n_B > 2^28, a parameter out of range, a loop edge id outside [0, n_A + n_B) or with
+ * from == to (or a non-finite relative_pose), or rows == NULL with capacity > 0. NDT and GICP handles alike.         */
+int b200sm_merge_session(b200sm_t dst, b200sm_t src, b200reg_t reg, const b200sm_merge_params* params,
+                         const b200sm_loop_edge* loop_edges, int n_loop_edges, b200sm_merge_row* rows, size_t capacity,
+                         size_t* n_rows, double* poses_out, b200sm_merge_result* result);
+/* the last merge's score matrix: *n_query = n_B, *n_cand = n_A; min(capacity, n_B * n_A) entries of D and s*, row-major
+ * by src submap (entry b * n_A + a). Either array may be NULL. */
+int b200sm_get_merge_scores(b200sm_t dst, size_t capacity, size_t* n_query, size_t* n_cand, double* distances, int* shifts);
+/* the first submap of every segment: *n = segments (0 for a session without submaps), min(capacity, n) copied */
+int b200sm_get_segments(b200sm_t s, size_t* first, size_t capacity, size_t* n);
 /* The map of every submap moved by a pose cast to float (modified map gbs.cpp:321-368; publishMap sm.cpp:529-552 when
  * poses == NULL, i.e. the submaps' own poses), assembled on the device in one launch. Output is x, y, z, intensity
  * floats in submap order. *n = total points; min(*n, capacity) points are copied, so capacity 0 is a size query (it

@@ -489,6 +489,25 @@ class ScanMatcherSession {
     shifts.resize(n);
     check(b200sm_get_place_scores(s_.get(), n, &n, distances.data(), shifts.data()));
   }
+  // ---- merging a second recording (b200sm_merge_session): `other`'s submaps are appended as a new segment when at least
+  // min_inliers consistent matches are found. p nullptr = the defaults; loop_edges in merged numbering (other's submap b is
+  // numSubmaps() + b). rows = the verified pairs; poses_out = the joint adjustment's (n_A + n_B) x 16 column-major doubles
+  // when merged. Returns the result (result.merged says whether this session changed).
+  b200sm_merge_result mergeSession(const ScanMatcherSession& other, b200reg_t reg, std::vector<b200sm_merge_row>& rows,
+                                   std::vector<double>& poses_out, const b200sm_merge_params* p = nullptr,
+                                   const std::vector<b200sm_loop_edge>& loop_edges = {}) {
+    size_t na = 0, nb = 0, n = 0;
+    check(b200sm_num_submaps(s_.get(), &na));
+    check(b200sm_num_submaps(other.handle(), &nb));
+    rows.resize(p ? (size_t)std::max(p->max_verifications, 1) : 64);
+    std::vector<double> poses(16 * (na + nb));
+    b200sm_merge_result r{};
+    check(b200sm_merge_session(s_.get(), other.handle(), reg, p, loop_edges.empty() ? nullptr : loop_edges.data(),
+                               (int)loop_edges.size(), rows.data(), rows.size(), &n, poses.data(), &r));
+    rows.resize(n);
+    if (r.merged) poses_out.swap(poses);
+    return r;
+  }
   // ---- occupancy grid for a navigation stack (b200sm_build_occupancy_grid): poses empty = the submaps' own, else 16 doubles
   // per submap, column-major (b200sm_pose_adjust's output); p nullptr = the defaults
   b200sm_occupancy_info buildOccupancyGrid(const std::vector<double>& poses_colmajor16 = {},

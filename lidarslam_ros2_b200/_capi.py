@@ -51,6 +51,7 @@ SYMBOLS = [
     "b200sm_set_scan_context_params", "b200sm_get_scan_context", "b200sm_search_loop_place", "b200sm_get_place_scores",
     "b200sm_build_occupancy_grid", "b200sm_get_occupancy_grid", "b200sm_save_occupancy_map",
     "b200sm_build_static_map", "b200sm_get_static_map", "b200sm_get_map_voxels", "b200sm_save_static_map_pcd_ascii",
+    "b200sm_merge_session", "b200sm_get_merge_scores", "b200sm_get_segments",
     # include/b200comm.h
     "b200comm_unique_id", "b200comm_create", "b200comm_destroy", "b200comm_all_gather_rows", "b200comm_rank", "b200comm_last_error",
     "b200comm_board_create", "b200comm_board_destroy", "b200comm_board_info",
@@ -101,6 +102,30 @@ class SmLoopEdge(C.Structure):
 class SmPoseAdjustResult(C.Structure):
     _fields_ = [("chi2_initial", C.c_double), ("chi2_final", C.c_double), ("iterations", C.c_int), ("trials", C.c_int),
                 ("n_vertices", C.c_int), ("n_edges", C.c_int)]
+
+
+class SmMergeParams(C.Structure):
+    _fields_ = [("sc_threshold", C.c_double), ("top_k", C.c_int), ("max_verifications", C.c_int), ("voxel_leaf_size", C.c_float),
+                ("threshold_loop_closure_score", C.c_double), ("search_submap_num", C.c_int),
+                ("consistency_translation", C.c_double), ("consistency_rotation", C.c_double),
+                ("consistency_drift_translation", C.c_double), ("consistency_drift_rotation", C.c_double),
+                ("min_inliers", C.c_int), ("num_adjacent_pose_cnstraints", C.c_int), ("max_iterations", C.c_int)]
+
+
+MERGE_DEFAULTS = dict(sc_threshold=0.4, top_k=3, max_verifications=64, voxel_leaf_size=0.3, threshold_loop_closure_score=1.0,
+                      search_submap_num=1, consistency_translation=1.5, consistency_rotation=0.1,
+                      consistency_drift_translation=0.02, consistency_drift_rotation=0.003, min_inliers=2,
+                      num_adjacent_pose_cnstraints=5, max_iterations=10)
+
+
+class SmMergeRow(C.Structure):
+    _fields_ = [("place", SmPlaceResult), ("src_id", C.c_int), ("inlier", C.c_int)]
+
+
+class SmMergeResult(C.Structure):
+    _fields_ = [("merged", C.c_int), ("query_tile", C.c_int), ("pairs_scored", C.c_ulonglong), ("candidates", C.c_int),
+                ("verified", C.c_int), ("accepted", C.c_int), ("inliers", C.c_int), ("first_submap", C.c_int),
+                ("T", C.c_double * 16), ("adjust", SmPoseAdjustResult)]
 
 
 class SmStats(C.Structure):
@@ -270,6 +295,10 @@ def lib() -> C.CDLL:
     L.b200sm_get_static_map.argtypes = [vp, vp, sz, C.POINTER(sz), vp]
     L.b200sm_get_map_voxels.argtypes = [vp, vp, vp, vp, vp, sz, C.POINTER(sz)]
     L.b200sm_save_static_map_pcd_ascii.argtypes = [vp, C.c_char_p, C.POINTER(sz), C.POINTER(sz)]
+    L.b200sm_merge_session.argtypes = [vp, vp, vp, C.POINTER(SmMergeParams), vp, i, vp, sz, C.POINTER(sz), vp,
+                                        C.POINTER(SmMergeResult)]
+    L.b200sm_get_merge_scores.argtypes = [vp, sz, C.POINTER(sz), C.POINTER(sz), vp, vp]
+    L.b200sm_get_segments.argtypes = [vp, vp, sz, C.POINTER(sz)]
     L.b200comm_unique_id.argtypes = [vp]
     L.b200comm_create.argtypes = [vp, i, i, i, C.POINTER(vp)]
     L.b200comm_destroy.argtypes = [vp]

@@ -28,4 +28,17 @@ void sc_finish_launch(uint32_t* keys, double* norms, size_t first_slot, size_t n
 void sc_search_launch(const float* desc, const double* norms, size_t query_slot, const int* ids, int n_ids, double* distance,
                       int* shift, int num_rings, int num_sectors, cudaStream_t stream);
 
+// K16 (b200sm_merge_session): queries per block of the score launch, from the descriptor's size and the device's opt-in
+// shared memory shared by MERGE_BLOCKS_PER_SM blocks, 1..MERGE_QUERY_TILE_MAX.
+constexpr int MERGE_QUERY_TILE_MAX = 32, MERGE_BLOCKS_PER_SM = 5;
+int merge_query_tile(int num_rings, int num_sectors);
+// distance[b * n_cand + a], shift[b * n_cand + a] = (D, s*) of query descriptor b (q_desc) against candidate a (c_desc),
+// bitwise K13b's for the same pair; one launch.
+void merge_scores_launch(const float* q_desc, const double* q_norms, int n_query, const float* c_desc, const double* c_norms,
+                         int n_cand, double* distance, int* shift, int num_rings, int num_sectors, cudaStream_t stream);
+// per query row b: the first top_k candidates with D < threshold in (D, a) order, at sel_*[b * top_k + r]; sel_a = -1
+// past the row's last candidate.
+void merge_select_launch(const double* distance, const int* shift, int n_query, int n_cand, double threshold, int top_k, int* sel_a,
+                         double* sel_d, int* sel_s, cudaStream_t stream);
+
 }  // namespace b200

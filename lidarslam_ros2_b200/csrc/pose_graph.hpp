@@ -201,16 +201,27 @@ inline void edge_jacobians(const Iso& E, const Iso& zinv, double* Jf, double* Jt
 // doPoseAdjustment's graph (gbs.cpp:276-315): for i > k, edges (i-k+j, i), j = 0..k-1, measurement pose_from^-1 * pose_i;
 // then the loop edges in the caller's order. Vertex 0 is never the end of an odometry edge (i - k + j >= 1): it is
 // reached through loop edges only, exactly as in the reference.
-inline std::vector<Edge> build_edges(const std::vector<Iso>& X, int k, const int* loop_from_to, const Iso* loop_rel, int n_loops) {
+//
+// A map merged from several recordings (b200sm_merge_session) applies the rule per segment: seg_first[s] is the first vertex
+// of segment s (ascending, seg_first[0] = 0), and local index i of a segment starting at f0 gives the edges
+// (f0 + i-k+j, f0 + i). No odometry edge crosses a segment boundary; with one segment the edges are the ones above.
+inline std::vector<Edge> build_edges(const std::vector<Iso>& X, int k, const std::vector<int>& seg_first, const int* loop_from_to,
+                                     const Iso* loop_rel, int n_loops) {
   std::vector<Edge> E;
   const int n = (int)X.size();
-  for (int i = k + 1; i < n; i++)
-    for (int j = 0; j < k; j++) {
-      const int f = i - k + j;
-      E.push_back({f, i, inverse(compose(inverse(X[f]), X[i]))});
-    }
+  for (size_t s = 0; s < seg_first.size(); s++) {
+    const int f0 = seg_first[s], f1 = s + 1 < seg_first.size() ? seg_first[s + 1] : n;
+    for (int i = k + 1; i < f1 - f0; i++)
+      for (int j = 0; j < k; j++) {
+        const int f = f0 + i - k + j, t = f0 + i;
+        E.push_back({f, t, inverse(compose(inverse(X[f]), X[t]))});
+      }
+  }
   for (int l = 0; l < n_loops; l++) E.push_back({loop_from_to[2 * l], loop_from_to[2 * l + 1], inverse(loop_rel[l])});
   return E;
+}
+inline std::vector<Edge> build_edges(const std::vector<Iso>& X, int k, const int* loop_from_to, const Iso* loop_rel, int n_loops) {
+  return build_edges(X, k, std::vector<int>{0}, loop_from_to, loop_rel, n_loops);
 }
 
 // Block (6x6) envelope (profile) Cholesky of a symmetric positive definite matrix. Row r stores its blocks from first[r]

@@ -318,6 +318,71 @@ class ScanMatcher:
         return (poses[:n].reshape(n, 4, 4).transpose(0, 2, 1).copy(),
                 {k: getattr(r, k) for k, _ in _capi.SmPoseAdjustResult._fields_})
 
+    # ---- merging a second session (b200sm_merge_session) ----
+    def mergeSession(self, other, registration, loop_edges=(), capacity=None, **params):
+        """Merge session `other` (another recording, in a frame of its own) into this one: Scan Context scores of every
+        pair on the device, the best candidates verified by `registration`, a consistent set of them kept, the joint pose
+        adjustment, and on success `other`'s submaps appended as a new segment at their rigid placement. params: the fields
+        of b200sm_merge_params (defaults in _capi.MERGE_DEFAULTS). loop_edges: (from, to, relative_pose 4x4) in merged
+        numbering (this session's submaps, then other's at numSubmaps() + b). Returns (rows, poses, result): one dict per
+        verified pair in verification order (searchLoopPlace's keys plus src_id, inlier, inlier_rank), the adjusted poses
+        (n_A + n_B, 4, 4) or None when the merge did not succeed, and the result dict (T as a 4x4, edges: the inter-session
+        loop edges in rank order, ready for poseAdjust)."""
+        unknown = set(params) - set(_capi.MERGE_DEFAULTS)
+        if unknown:
+            raise TypeError(f"mergeSession: unknown parameters {sorted(unknown)}")
+        p = _capi.SmMergeParams(**{**_capi.MERGE_DEFAULTS, **params})
+        edges = (_capi.SmLoopEdge * max(1, len(loop_edges)))()
+        for k, (f, t, Z) in enumerate(loop_edges):
+            edges[k].from_, edges[k].to = int(f), int(t)
+            edges[k].relative_pose[:] = np.asarray(Z, dtype=np.float64).T.reshape(16).tolist()
+        nA, nB = self.numSubmaps(), other.numSubmaps()
+        cap = int(p.max_verifications) if capacity is None else int(capacity)
+        arr = (_capi.SmMergeRow * max(1, cap))()
+        poses = np.zeros((max(1, nA + nB), 16), dtype=np.float64)
+        n = C.c_size_t(0)
+        r = _capi.SmMergeResult()
+        self._check(self._lib.b200sm_merge_session(self._h, other._h, registration._h, C.byref(p), edges, len(loop_edges), arr, cap,
+                                                   C.byref(n), _ptr(poses), C.byref(r)))
+        rows = []
+        for k in range(n.value):
+            m = arr[k]
+            q, lp = m.place, m.place.loop
+            d = {"id_min": int(lp.id_min), "src_id": int(m.src_id), "accepted": bool(lp.accepted), "min_dist": float(lp.min_dist),
+                 "fitness": float(lp.fitness), "n_source": int(lp.n_source), "n_target": int(lp.n_target),
+                 "final": np.array(lp.final_T, dtype=np.float32).reshape(4, 4).T.copy(), "sc_distance": float(q.sc_distance),
+                 "shift": int(q.shift), "guess": np.array(q.guess, dtype=np.float32).reshape(4, 4).T.copy(),
+                 "inlier": m.inlier >= 0, "inlier_rank": int(m.inlier)}
+            if lp.accepted:
+                d["relative_pose"] = np.array(lp.relative_pose, dtype=np.float64).reshape(4, 4).T.copy()
+            rows.append(d)
+        res = {k: getattr(r, k) for k, _ in _capi.SmMergeResult._fields_ if k not in ("T", "adjust")}
+        res["merged"] = bool(r.merged)
+        res["T"] = np.array(r.T, dtype=np.float64).reshape(4, 4).T.copy()
+        res["adjust"] = {k: getattr(r.adjust, k) for k, _ in _capi.SmPoseAdjustResult._fields_}
+        res["edges"] = [(d["id_min"], nA + d["src_id"], d["relative_pose"]) for d in sorted(
+            (d for d in rows if d["inlier"]), key=lambda d: d["inlier_rank"])]
+        out = poses[:nA + nB].reshape(nA + nB, 4, 4).transpose(0, 2, 1).copy() if r.merged else None
+        return rows, out, res
+
+    def mergeScores(self):
+        """The last mergeSession's score matrix: (D (n_B, n_A) float64, s* (n_B, n_A) int32), row b = the other session's
+        submap b."""
+        nq, nc = C.c_size_t(0), C.c_size_t(0)
+        self._check(self._lib.b200sm_get_merge_scores(self._h, 0, C.byref(nq), C.byref(nc), None, None))
+        D = np.empty((nq.value, nc.value), dtype=np.float64)
+        S = np.empty((nq.value, nc.value), dtype=np.int32)
+        self._check(self._lib.b200sm_get_merge_scores(self._h, D.size, C.byref(nq), C.byref(nc), _ptr(D), _ptr(S)))
+        return D, S
+
+    def segments(self) -> list:
+        """The first submap of every segment (one per recording merged into this session)."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_get_segments(self._h, None, 0, C.byref(n)))
+        out = np.zeros(max(1, n.value), dtype=np.uint64)
+        self._check(self._lib.b200sm_get_segments(self._h, _ptr(out), n.value, C.byref(n)))
+        return [int(v) for v in out[:n.value]]
+
     def assembleMap(self, poses=None, capacity=None):
         """The map of every submap moved by its pose cast to float (publishMap sm.cpp:529-552 when poses is None, else the
         modified map of gbs.cpp:321-368), assembled on the device in one launch. Returns (cloud (M, 4) float32, offsets
