@@ -222,8 +222,8 @@ int b200reg_gicp_num_correspondences(b200reg_t h, int* out);
 int b200reg_gicp_correspondences(b200reg_t h, const float* guess, const float* T, int* corr, float* maha9, int* m);
 /* one evaluation of the fixed-correspondence objective (operator() when want_grad == 0, else fdf;
  * gicp_omp_impl.hpp:244-366) at state x6 on the correspondences of the last align() / b200reg_gicp_correspondences, by
- * the path align() uses (the persistent kernel, or with B200REG_GICP_HOST_BFGS set at creation one reduction launch).
- * g6 is written when want_grad; T12 (may be NULL) = the f32 row-major 3x4 transform that path built from x6.
+ * the persistent inner-loop kernel align() uses, run for this one call.
+ * g6 is written when want_grad; T12 (may be NULL) = the f32 row-major 3x4 transform the kernel built from x6.
  * B200REG_ERR_ARG when there are fewer than 4 correspondences or the clouds changed since they were found. */
 int b200reg_gicp_objective(b200reg_t h, const double* x6, int want_grad, double* f, double* g6, float* T12);
 /* NDT read-back for the controller tests: an opt-in per-round trace of b200reg_align (batch calls are never traced).
@@ -264,8 +264,8 @@ int b200reg_ndt_get_trace(b200reg_t h, b200reg_ndt_trace_record* out, int capaci
 /* GICP read-back for the optimiser tests: an opt-in trace of b200reg_align (batch calls are never traced), one stream of
  * records in the order they happen. estimateRigidTransformationBFGS (gicp_omp_impl.hpp:180-241) appends a type 0 record
  * per functor call and a type 1 record per minimizeOneStep; each outer iteration of computeTransformation (:369-515)
- * ends with a type 2 record. Both BFGS paths trace: the device controller (each of the twelve T words is written by the
- * controller thread that published it) and the host BFGS of a handle created with B200REG_GICP_HOST_BFGS.
+ * ends with a type 2 record. The type 0 and 1 records come from the persistent inner-loop kernel's controller: each of
+ * the twelve T words is written by the controller thread that published it.
  * b200reg_gicp_set_trace(h, capacity) keeps room for `capacity` records (0 turns tracing off); b200reg_gicp_get_trace
  * copies min(*n, capacity, cap) records of the last align() and sets *n to the number of records it produced, which
  * exceeds the capacity when the trace overflowed. Fields a record type does not use are 0. */

@@ -2,14 +2,12 @@
 // Implements the minimiser the reference calls at gicp_omp_impl.hpp:209-230 — PCL 1.12 `BFGS<Functor>`
 // (pcl/registration/bfgs.h, external), a port of GSL's vector_bfgs2 + Fletcher bracketing/sectioning line search
 // (multimin/linear_minimize.c) — with sigma=0.01, rho=0.01, tau1=9, tau2=0.05, tau3=0.5, order=3.
-// The 6-vector state machine is __host__ __device__ and templated on the functor: the host instantiation drives one K7
-// reduction kernel per functor evaluation; the device instantiation runs inside the persistent inner-loop kernel
-// (gicp.cu: every thread of the controller CTA executes it redundantly and identically, so that the whole CTA takes part
-// in each functor evaluation).
+// The 6-vector state machine is __host__ __device__ and templated on the functor. The engine instantiates it inside the
+// persistent inner-loop kernel (gicp.cu: every thread of the controller CTA executes it redundantly and identically, so
+// that the whole CTA takes part in each functor evaluation); tests/hostmath compiles it with g++ to compare it with the
+// oracle's BFGS.
 #pragma once
 #include <math.h>
-
-#include <functional>
 
 #if defined(__CUDACC__)
 #define B200_BFGS_HD __host__ __device__
@@ -22,12 +20,6 @@ namespace b200 {
 constexpr double BFGS_DBL_EPSILON = 2.220446049250313e-16;
 
 enum BfgsStatus { BFGS_NegativeGradientEpsilon = -3, BFGS_NotStarted = -2, BFGS_Running = -1, BFGS_Success = 0, BFGS_NoProgress = 1 };
-
-struct BfgsFunctor6 {
-  std::function<double(const double*)> f;
-  std::function<void(const double*, double*)> df;
-  std::function<void(const double*, double&, double*)> fdf;
-};
 
 template <class Functor>
 class Bfgs6T {
@@ -335,7 +327,5 @@ class Bfgs6T {
     return BFGS_Success;
   }
 };
-
-using Bfgs6 = Bfgs6T<BfgsFunctor6>;  // host instantiation: std::function callbacks that launch K7
 
 }  // namespace b200

@@ -339,7 +339,6 @@ int b200reg_create(int kind, int device, b200reg_t* out) {
     B200_CUDA(cudaEventCreate(&h->ev1));
     h->solver.init(device, h->stream);
     h->solver.scalar_controller = getenv("B200REG_SCALAR_CTL") != nullptr;
-    h->gicp_solver.device_bfgs = getenv("B200REG_GICP_HOST_BFGS") == nullptr;  // developer switch: host-driven BFGS
     h->gicp_solver.init(device, h->stream);
     if (kind == B200REG_GICP) {
       h->corr_dist = 5.0;  // gicp_omp.h:119

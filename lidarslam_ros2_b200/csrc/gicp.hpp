@@ -1,5 +1,6 @@
-// GICP engine behind the C-ABI: K5 kNN covariances, K6 correspondences + Mahalanobis matrices, K7 cost / gradient
-// reductions, and the host-side BFGS driver (pclomp::GeneralizedIterativeClosestPoint, gicp_omp_impl.hpp).
+// GICP engine behind the C-ABI: K5 kNN covariances, K6 correspondences + Mahalanobis matrices, K7 the persistent
+// inner-loop kernel (BFGS and cost / gradient reductions), and the host-side outer loop
+// (pclomp::GeneralizedIterativeClosestPoint, gicp_omp_impl.hpp).
 #pragma once
 #include "engine.hpp"
 
@@ -62,9 +63,9 @@ class GicpSolver {
   // matrices; returns (and keeps) the correspondence count m
   int correspondences(const NnGrid& target_grid, const GicpConfig& cfg, const float* guess_rowmajor16,
                       const float* transformation_rowmajor16, cudaStream_t s);
-  // one functor evaluation at state x on the current correspondences, by the path align() uses: the persistent kernel in
-  // evaluate-once mode (device_bfgs) or one gicp_cost_kernel launch. g6 is written when want_grad; T12 (row-major 3x4) is
-  // the f32 transform that path built from x. Requires m >= 4 (align() never evaluates with fewer).
+  // one functor evaluation at state x on the current correspondences, by the persistent kernel align() uses, in
+  // evaluate-once mode. g6 is written when want_grad; T12 (row-major 3x4) is the f32 transform the kernel built from x.
+  // Requires m >= 4 (align() never evaluates with fewer).
   void evaluate(const double* x, bool want_grad, double* f, double* g6, float* T12);
   // read-back of the last K6 pass: corr n_source ints (-1 = none), maha n_source x 9 floats (meaningful where corr >= 0)
   void read_correspondences(int* corr, float* maha9, cudaStream_t s);
@@ -73,9 +74,6 @@ class GicpSolver {
   int last_correspondences() const { return last_m_; }
   size_t n_source() const { return n_source_; }
   int launches = 0;
-  // true: estimateRigidTransformationBFGS runs as ONE persistent cooperative kernel per outer iteration (BFGS on the
-  // device); false: host-side BFGS, one K7 launch + synchronisation per functor evaluation
-  bool device_bfgs = true;
   // accounting of the last align(): device time of the persistent inner kernel(s), their launches, and the
   // (correspondence, evaluation) products they processed (algorithmic bytes = that times 72, DESIGN.md section 4)
   float inner_ms = 0;
@@ -86,7 +84,6 @@ class GicpSolver {
   int read_trace(b200reg_gicp_trace_record* out, int cap) const;  // copies up to cap records, returns the records counted
 
  private:
-  void fdf(const float* T_rowmajor16, bool want_grad, double* f, double* g_t3, double* R9);
   // returns the BFGS status; x is updated in place. eval_once: 0 runs the BFGS; 1 (f only) or 2 (f and g) makes exactly
   // one functor call at x instead, its result left in *h_inner_result_
   int inner_loop_device(double* x, const GicpConfig& cfg, int* inner_iterations, int eval_once = 0);
@@ -107,10 +104,7 @@ class GicpSolver {
   DeviceBuffer<int> nn_idx_;
   DeviceBuffer<float> nn_d2_;
   DeviceBuffer<float4> moved_;                    // source transformed by the guess ("output" cloud)
-  DeviceBuffer<double> partials_;                 // per-CTA partial sums (16 doubles each)
-  DeviceBuffer<double> result_;                   // 16 doubles
-  DeviceBuffer<unsigned> counter_;
-  double* h_result_ = nullptr;                    // pinned
+  DeviceBuffer<unsigned> counter_;                // K6's correspondence count
   size_t n_source_ = 0, n_target_ = 0;
   const float4* target_ = nullptr;
   int last_m_ = 0;

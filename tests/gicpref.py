@@ -30,10 +30,8 @@ What is computed
 The bound
   A recursive f64 sum whose deepest chain of additions has D steps is within D u sum|term| of the exact sum (u = 2^-53,
   first order). The kernel's chains:
-    device path (gicp_inner_kernel): the points a thread takes in its evaluator chunk (ceil(chunk / 256)), the 5-level
-      shuffle tree, 8 warps, the 10 rows a controller thread sums, the 16 interleaved chains;
-    host path (gicp_cost_kernel): the points a thread takes in the grid-stride loop (ceil(n / (blocks 256))), 5, 8, the
-      ceil(blocks / 16) partials of a chain, 16.
+    gicp_inner_kernel: the points a thread takes in its evaluator chunk (ceil(chunk / 256)), the 5-level shuffle tree,
+      8 warps, the 10 rows a controller thread sums, the 16 interleaved chains.
   The oracle sums serially: D = m. Each entry's bound is (D + c) u sum|term| scaled like the entry (1 / m or 2 / m), c = 4
   for the final division and multiplication. g[3..5] add sum_ij |m1|(j, i) bound(R(i, j)) and the double sin / cos of
   the device (<= 2 ulp) and host (<= 1 ulp) libraries: each m1 entry is a sum of products of up to three of them, so it
@@ -233,12 +231,6 @@ def depth_device(n, sm_count):
     return -(-chunk // GI_THREADS) + 5 + 8 + GI_MAX_CTAS // 16 + 16
 
 
-def depth_host(n, sm_count):
-    """Deepest f64 summation chain of gicp_cost_kernel for n source points on sm_count SMs."""
-    blocks = max(1, min(-(-n // 256), sm_count * 2))
-    return -(-n // (blocks * 256)) + 5 + 8 + -(-blocks // 16) + 16
-
-
 def evaluator_partition(n, sm_count):
     """(n_eval, chunk) of the persistent kernel: the evaluator CTA k takes points [k chunk, min(n, (k + 1) chunk))."""
     n_eval = max(1, min(-(-n // GI_THREADS), min(sm_count, GI_MAX_CTAS) - 1))
@@ -247,7 +239,7 @@ def evaluator_partition(n, sm_count):
 
 def objective(T, x, moved, target, corr, maha, depth, R_swap=False):
     """Exact sums of the functor at transform T (12 or 16 f32, row-major) and state x: dict(f32path, f, g (6,), R (3,3),
-    bounds b_f32path, b_f, b_g (6,), and the terms). depth: the D of the path compared with (depth_device / depth_host /
+    bounds b_f32path, b_f, b_g (6,), and the terms). depth: the D of the summation compared with (depth_device, or
     m for the oracle). R_swap exchanges R[0,1] and R[1,0] (a power check)."""
     tm = terms(T, moved, target, corr, maha)
     m = len(tm["fdf"])
@@ -370,14 +362,10 @@ def cloud_of_size(target, n, seed=0, T=None):
     return p.astype(F32)
 
 
-def ladder(sm_count, host=False):
-    """Source sizes at the evaluator partition's edges (device), plus the host reduction's (host=True)."""
-    S = sm_count
-    e = min(S, GI_MAX_CTAS) - 1
-    sizes = [4, 5, 255, 256, 257, 256 * e - 1, 256 * e, 256 * e + 1]
-    if host:
-        sizes += [256 * 1, 256 * 15, 256 * 16, 256 * 17, 512 * S - 1, 512 * S, 512 * S + 1]
-    return sorted(set(sizes))
+def ladder(sm_count):
+    """Source sizes at the evaluator partition's edges."""
+    e = min(sm_count, GI_MAX_CTAS) - 1
+    return sorted({4, 5, 255, 256, 257, 256 * e - 1, 256 * e, 256 * e + 1})
 
 
 def surface_pair(seed=17):

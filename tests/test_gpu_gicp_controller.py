@@ -1,11 +1,9 @@
-"""GICP's optimiser (the device controller of gicp_inner_kernel running Bfgs6T, and the host Bfgs6 of a handle created
-with B200REG_GICP_HOST_BFGS) call by call, through the opt-in trace of align(): every functor call, BFGS step and outer
-iteration is replayed bit for bit by the float64 restatement of tests/gicpctl_ref.py from the recorded (f, g); the
-bookkeeping must follow from the records exactly; every in-BFGS evaluation must be a real evaluation, bitwise equal to
-b200reg_gicp_objective at the recorded x on the correspondences of its outer iteration, and on the small scenes within
-the bound of the float64 reference gicpref.objective. Run on an H100 with -m gpu; each test prints its largest ratio to
-its bound and the branch counts."""
-import os
+"""GICP's optimiser (the device controller of gicp_inner_kernel running Bfgs6T) call by call, through the opt-in trace
+of align(): every functor call, BFGS step and outer iteration is replayed bit for bit by the float64 restatement of
+tests/gicpctl_ref.py from the recorded (f, g); the bookkeeping must follow from the records exactly; every in-BFGS
+evaluation must be a real evaluation, bitwise equal to b200reg_gicp_objective at the recorded x on the correspondences
+of its outer iteration, and on the small scenes within the bound of the float64 reference gicpref.objective. Run on an
+H100 with -m gpu; each test prints its largest ratio to its bound and the branch counts."""
 from collections import Counter
 
 import numpy as np
@@ -16,10 +14,7 @@ import gicpref as G
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
-HOST_ENV = "B200REG_GICP_HOST_BFGS"
 CAP = 1 << 15
-PATHS = [False, True]
-PATH_IDS = ["device", "host"]
 _scenes = {}
 
 
@@ -53,14 +48,9 @@ def _cfg(name):
     return dict(trans_eps=1e-8, max_iterations=6) if name == "headline" else {}
 
 
-def _handle(b200, src, tgt, host=False, cfg=None, cap=CAP):
+def _handle(b200, src, tgt, cfg=None, cap=CAP):
     cfg = cfg or {}
-    if host:
-        os.environ[HOST_ENV] = "1"
-    try:
-        g = b200.GeneralizedIterativeClosestPoint()
-    finally:
-        os.environ.pop(HOST_ENV, None)
+    g = b200.GeneralizedIterativeClosestPoint()
     g.setMaxCorrespondenceDistance(5.0)
     if "trans_eps" in cfg:
         g.setTransformationEpsilon(cfg["trans_eps"])
@@ -132,28 +122,26 @@ def _check_evaluations(g, src, tgt, recs, guess, depth=None, stride=1):
     return worst
 
 
-@pytest.mark.parametrize("host", PATHS, ids=PATH_IDS)
 @pytest.mark.parametrize("name", ["pair", "tiny", "small", "c1", "headline"])
-def test_trace_replays_and_evaluations_are_real(b200, sms, name, host):
+def test_trace_replays_and_evaluations_are_real(b200, sms, name):
     src, tgt = _scene(name)
     cfg = _cfg(name)
     depth = None
     if name in ("pair", "tiny", "small"):
-        depth = (G.depth_host if host else G.depth_device)(len(src), sms)
+        depth = G.depth_device(len(src), sms)
     total, worst_eval, worst_T = Counter(), 0.0, 0.0
     for guess in (None, G.GUESS):
-        g = _handle(b200, src, tgt, host, cfg)
+        g = _handle(b200, src, tgt, cfg)
         T, recs = _traced(g, guess)
         r = _replay(g, T, recs, guess, cfg)
         total.update(r["counts"])
         worst_T = max(worst_T, r["worst_T"])
         worst_eval = max(worst_eval, _check_evaluations(g, src, tgt, recs, guess, depth, stride=1 if name != "small" else 3))
-    print(f"\n{name} {'host' if host else 'device'}: every record bitwise, largest T / bound {worst_T:.3g}, largest "
+    print(f"\n{name}: every record bitwise, largest T / bound {worst_T:.3g}, largest "
           f"evaluation / bound {worst_eval:.3g}; branches {dict(sorted(total.items()))}")
 
 
-@pytest.mark.parametrize("host", PATHS, ids=PATH_IDS)
-def test_generators(b200, host):
+def test_generators(b200):
     """Entry NoProgress with its NaN direction, m = 4, m < 4, the inner cap and a far start, replayed and evaluated."""
     s, t = _scene("small")
     total = Counter()
@@ -161,7 +149,7 @@ def test_generators(b200, host):
                 "offset_near": X.offset_pair(s, t, (0.3, 0.1, 0.0), (0.0, 0.0, 0.02)),
                 "offset_far": X.offset_pair(s, t, (3.0, -2.0, 0.5), (0.0, 0.0, 0.2))}
     for name, (src, tgt) in fixtures.items():
-        g = _handle(b200, src, tgt, host)
+        g = _handle(b200, src, tgt)
         T, recs = _traced(g, None)
         r = _replay(g, T, recs, None, {})
         total.update(r["counts"])
@@ -177,7 +165,7 @@ def test_generators(b200, host):
             assert r["counts"]["inner_cap"] > 0
         if name != "m3":
             _check_evaluations(g, src, tgt, recs, None)
-    print(f"\ngenerators {'host' if host else 'device'}: branches {dict(sorted(total.items()))}")
+    print(f"\ngenerators: branches {dict(sorted(total.items()))}")
 
 
 def test_evaluator_ladder(b200, sms):
@@ -192,24 +180,22 @@ def test_evaluator_ladder(b200, sms):
         print(f"\nladder n = {n}: evaluators {G.evaluator_partition(n, sms)[0]}, {len(recs)} records bitwise")
 
 
-@pytest.mark.parametrize("host", PATHS, ids=PATH_IDS)
-def test_stale_state(b200, host):
+def test_stale_state(b200):
     """Three different aligns on one handle, each bitwise (trace and result) a fresh handle's."""
     s, t = _scene("small")
     s2, _ = _scene("tiny")
-    A = _handle(b200, s, t, host)
+    A = _handle(b200, s, t)
     for src, guess in ((s, G.GUESS), (s, None), (s2, G.GUESS)):
         A.setInputSource(src)
         Ta, ra = _traced(A, guess)
-        F = _handle(b200, src, t, host)
+        F = _handle(b200, src, t)
         Tf, rf = _traced(F, guess)
         assert _bits(Ta) == _bits(Tf) and _bits(ra) == _bits(rf)
 
 
-@pytest.mark.parametrize("host", PATHS, ids=PATH_IDS)
-def test_trace_neutral_and_overflow(b200, host):
+def test_trace_neutral_and_overflow(b200):
     s, t = _scene("small")
-    on, off = _handle(b200, s, t, host), _handle(b200, s, t, host, cap=0)
+    on, off = _handle(b200, s, t), _handle(b200, s, t, cap=0)
     Ton, recs = _traced(on, G.GUESS)
     Toff = off.align(G.GUESS)
     assert _bits(Ton) == _bits(Toff)
@@ -217,7 +203,7 @@ def test_trace_neutral_and_overflow(b200, host):
     for k in ("iterations", "evaluations"):
         assert a[k] == b[k], k
     assert on.hasConverged() == off.hasConverged()
-    small = _handle(b200, s, t, host, cap=5)
+    small = _handle(b200, s, t, cap=5)
     assert _bits(small.align(G.GUESS)) == _bits(Ton)
     part, n = small.trace()
     assert n == len(recs) and len(part) == 5 and _bits(part) == _bits(recs[:5])

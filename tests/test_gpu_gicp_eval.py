@@ -1,9 +1,7 @@
-"""GICP's correspondence pass (K6) and objective evaluation (K7, both the persistent device-BFGS kernel and the host-driven
-gicp_cost_kernel) against the float64 reference of tests/gicpref.py, entry by entry: correspondences exactly, Mahalanobis
-matrices bit for bit, f / f32path / g within the bound the reference derives for the path's summation order. Each test
-prints its largest |kernel - reference| / bound."""
-import os
-
+"""GICP's correspondence pass (K6) and objective evaluation (K7, the persistent inner-loop kernel) against the float64
+reference of tests/gicpref.py, entry by entry: correspondences exactly, Mahalanobis matrices bit for bit, f / f32path / g
+within the bound the reference derives for the kernel's summation order. Each test prints its largest
+|kernel - reference| / bound."""
 import numpy as np
 import pytest
 
@@ -12,7 +10,6 @@ import gridref as GR
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
-HOST_ENV = "B200REG_GICP_HOST_BFGS"
 
 
 @pytest.fixture(scope="module")
@@ -48,14 +45,8 @@ def _scene(name):
     return _scenes[name]
 
 
-def _handle(b200, src, tgt, host=False, corr_dist=5.0):
-    """A GICP handle; host=True creates it with the host-driven BFGS switch set."""
-    if host:
-        os.environ[HOST_ENV] = "1"
-    try:
-        g = b200.GeneralizedIterativeClosestPoint()
-    finally:
-        os.environ.pop(HOST_ENV, None)
+def _handle(b200, src, tgt, corr_dist=5.0):
+    g = b200.GeneralizedIterativeClosestPoint()
     g.setMaxCorrespondenceDistance(corr_dist)
     g.setInputTarget(tgt)
     g.setInputSource(src)
@@ -83,7 +74,7 @@ def _k6(g, src, tgt, corr_dist=5.0, guess=None, T=None):
 
 
 def _k7(g, ref, tgt, x, depth):
-    """One fdf and one f-only evaluation against the reference at the transform the path returned; largest ratio."""
+    """One fdf and one f-only evaluation against the reference at the transform the kernel returned; largest ratio."""
     f, grad, T = g.objective(x, True)
     f32, _, T2 = g.objective(x, False)
     assert np.array_equal(T.view(np.int32), T2.view(np.int32))
@@ -141,84 +132,60 @@ def test_k6_far_pass_km_shift_large_rotation(b200):
 
 
 # ---- K7 ---------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("host", [False, True], ids=["device", "host"])
-def test_k7_matches_reference(b200, sms, host):
+def test_k7_matches_reference(b200, sms):
     worst = 0.0
     for name in ("pair", "small"):
         src, tgt = _scene(name)
-        g = _handle(b200, src, tgt, host=host)
+        g = _handle(b200, src, tgt)
         ref = _k6(g, src, tgt, guess=G.GUESS, T=G.T_OFF)
-        depth = (G.depth_host if host else G.depth_device)(len(src), sms)
+        depth = G.depth_device(len(src), sms)
         for x in G.STATES.values():
             r, _ = _k7(g, ref, tgt, x, depth)
             worst = max(worst, r)
-    print(f"K7 {'host' if host else 'device'}: largest ratio {worst:.3g}")
+    print(f"K7: largest ratio {worst:.3g}")
 
 
-def test_k7_paths_agree(b200, sms):
-    src, tgt = _scene("small")
-    gd, gh = _handle(b200, src, tgt), _handle(b200, src, tgt, host=True)
-    rd, rh = _k6(gd, src, tgt, guess=G.GUESS), _k6(gh, src, tgt, guess=G.GUESS)
-    worst, same_T = 0.0, 0
-    for x in G.STATES.values():
-        _, a = _k7(gd, rd, tgt, x, G.depth_device(len(src), sms))
-        _, b = _k7(gh, rh, tgt, x, G.depth_host(len(src), sms))
-        if not np.array_equal(a["T"].view(np.int32), b["T"].view(np.int32)):
-            continue  # cosf / sinf of the device and the host may differ in the last bit; each matched the reference
-        same_T += 1
-        tf = a["bound"]["b_f"] + b["bound"]["b_f"]
-        tg = a["bound"]["b_g"] + b["bound"]["b_g"]
-        assert abs(a["f"] - b["f"]) <= tf and np.all(np.abs(a["g"] - b["g"]) <= tg)
-        worst = max(worst, abs(a["f"] - b["f"]) / tf, float((np.abs(a["g"] - b["g"]) / tg).max()))
-    assert same_T >= 1  # x = 0 builds the identity on both
-    print(f"K7 device vs host: largest ratio {worst:.3g} over {same_T} states with equal T")
-
-
-def _ladder_case(b200, src, tgt, host, sms, x=G.STATES["moderate"]):
-    g = _handle(b200, src, tgt, host=host)
+def _ladder_case(b200, src, tgt, sms, x=G.STATES["moderate"]):
+    g = _handle(b200, src, tgt)
     ref = _k6(g, src, tgt)
     if ref["m"] < 4:
         return 0.0
-    depth = (G.depth_host if host else G.depth_device)(len(src), sms)
-    return _k7(g, ref, tgt, x, depth)[0]
+    return _k7(g, ref, tgt, x, G.depth_device(len(src), sms))[0]
 
 
-@pytest.mark.parametrize("host", [False, True], ids=["device", "host"])
-def test_partition_ladder(b200, sms, host):
+def test_partition_ladder(b200, sms):
     _, tgt = _scene("small")
     worst = {}
-    for n in G.ladder(sms, host=host):
+    for n in G.ladder(sms):
         src = G.cloud_of_size(tgt, n, seed=n)
-        worst[n] = _ladder_case(b200, src, tgt, host, sms)
+        worst[n] = _ladder_case(b200, src, tgt, sms)
     # correspondences confined to one evaluator chunk: the other evaluators contribute exactly +0.0
     n = 256 * (min(sms, G.GI_MAX_CTAS) - 1) + 1
     n_eval, chunk = G.evaluator_partition(n, sms)
     base = G.cloud_of_size(tgt, n, seed=7)
     for which in (0, n_eval // 2, n_eval - 1):
         src, _ = G.confine_to_chunk(base, n_eval, chunk, which)
-        worst[f"chunk{which}"] = _ladder_case(b200, src, tgt, host, sms)
-    print(f"ladder {'host' if host else 'device'}: largest ratio {max(worst.values()):.3g}", worst)
+        worst[f"chunk{which}"] = _ladder_case(b200, src, tgt, sms)
+    print(f"ladder: largest ratio {max(worst.values()):.3g}", worst)
 
 
-@pytest.mark.parametrize("host", [False, True], ids=["device", "host"])
-def test_large_scans(b200, sms, host):
+def test_large_scans(b200, sms):
     src, tgt = _scene("headline")
-    worst = [_ladder_case(b200, src, tgt, host, sms)]
+    worst = [_ladder_case(b200, src, tgt, sms)]
     big = G.cloud_of_size(tgt, 250_000, seed=11)
-    worst.append(_ladder_case(b200, big, tgt, host, sms))
-    print(f"headline and 250k ({'host' if host else 'device'}): ratios {worst}")
+    worst.append(_ladder_case(b200, big, tgt, sms))
+    print(f"headline and 250k: ratios {worst}")
 
 
 # ---- m at 3 and 4, stale state, end to end ---------------------------------------------------------------------------
-@pytest.mark.parametrize("host", [False, True], ids=["device", "host"])
-def test_three_and_four_correspondences(b200, oracle_mod, sms, host):
+def test_three_and_four_correspondences(b200, oracle_mod, sms):
     from lidarslam_ros2_b200 import synth
     from lidarslam_ros2_b200.registration import B200RegError
 
     _, tgt = _scene("tiny")
     for m in (3, 4):
         src = G.exact_m_scan(tgt, m)
-        g = _handle(b200, src, tgt, host=host)
+        g = _handle(b200, src, tgt)
         ref = _k6(g, src, tgt)
         assert ref["m"] == m
         if m == 3:
@@ -232,8 +199,8 @@ def test_three_and_four_correspondences(b200, oracle_mod, sms, host):
             assert dt < 1e-6 and dr < 1e-6
             assert not g.hasConverged() and not o.converged
         else:
-            r, _ = _k7(g, ref, tgt, G.STATES["moderate"], (G.depth_host if host else G.depth_device)(len(src), sms))
-            print(f"m = 4 ({'host' if host else 'device'}): ratio {r:.3g}")
+            r, _ = _k7(g, ref, tgt, G.STATES["moderate"], G.depth_device(len(src), sms))
+            print(f"m = 4: ratio {r:.3g}")
 
 
 def _bits(a):
@@ -267,19 +234,19 @@ def test_stale_state(b200):
 
 
 @pytest.mark.parametrize("name", ["pair", "small"])
-def test_host_path_align_end_to_end(b200, oracle_mod, name):
+def test_align_end_to_end(b200, oracle_mod, name):
     from lidarslam_ros2_b200 import synth
 
     src, tgt = _scene(name)
-    gh, gd = _handle(b200, src, tgt, host=True), _handle(b200, src, tgt)
+    g = _handle(b200, src, tgt)
     o = oracle_mod.GICP(max_correspondence_distance=5.0)
     o.set_target(tgt)
     o.set_source(src)
     To = o.align()
-    Th, Td = gh.align(), gd.align()
-    dt, dr = synth.pose_error(Th, To)
+    T = g.align()
+    dt, dr = synth.pose_error(T, To)
     assert dt < 1e-3 and dr < 1e-3, (dt, dr)
-    assert gh.hasConverged() == o.converged
-    sh, sd = gh.stats(), gd.stats()
-    print(f"{name}: host path {sh['iterations']} iterations / {sh['evaluations']} evaluations, device path "
-          f"{sd['iterations']} / {sd['evaluations']}, oracle {o.iterations} iterations; host vs oracle {dt:.2e} m {dr:.2e} rad")
+    assert g.hasConverged() == o.converged
+    st = g.stats()
+    print(f"{name}: {st['iterations']} iterations / {st['evaluations']} evaluations, oracle {o.iterations} iterations; "
+          f"vs oracle {dt:.2e} m {dr:.2e} rad")
