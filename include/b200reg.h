@@ -466,7 +466,8 @@ typedef struct b200sm_pose_adjust_result {
  * (the adjusted Isometry3d of every vertex; vertex 0 is fixed). The session's own submap poses are NOT changed:
  * searchLoop, updateMap and the targeted cloud keep using the frontend's poses, as in the reference.
  * B200REG_ERR_ARG for a loop edge id outside [0, n_submaps) or from == to, a non-finite relative_pose,
- * num_adjacent_pose_cnstraints < 1 or max_iterations < 0. optimizer.save("pose_graph.g2o") (:319) is not reproduced. */
+ * num_adjacent_pose_cnstraints < 1 or max_iterations < 0. optimizer.save("pose_graph.g2o") (:319) is written by
+ * b200sm_save_session, with the session's submaps, from the same graph. */
 int b200sm_pose_adjust(b200sm_t s, int num_adjacent_pose_cnstraints, const b200sm_loop_edge* loop_edges, int n_loop_edges,
                        int max_iterations, double* poses_out, b200sm_pose_adjust_result* result);
 
@@ -536,6 +537,44 @@ int b200sm_merge_session(b200sm_t dst, b200sm_t src, b200reg_t reg, const b200sm
 int b200sm_get_merge_scores(b200sm_t dst, size_t capacity, size_t* n_query, size_t* n_cand, double* distances, int* shifts);
 /* the first submap of every segment: *n = segments (0 for a session without submaps), min(capacity, n) copied */
 int b200sm_get_segments(b200sm_t s, size_t* first, size_t capacity, size_t* n);
+
+/* ---- saving a mapping session to disk and loading it back ------------------------------------------------------------
+ * A directory: session.txt (the manifest: Scan Context parameters, segments, every submap's point count, distance and
+ * pose, and the caller's graph: num_adjacent_pose_cnstraints, loop edges, adjusted poses or none; every double printed
+ * with %.17g, so it reads back bitwise), pose_graph.g2o (the graph as the reference's optimizer.save writes it,
+ * gbs.cpp:319; an export, never read back) and submaps/%06zu.pcd (one binary PCD per submap as pcl::io::savePCDFileBinary
+ * writes a dense PointXYZI cloud: the sensor-frame rows, intensity included; an empty submap is a header with POINTS 0).
+ * Definitions: csrc/session_io.hpp; DESIGN.md section 7b. */
+typedef struct b200sm_session_io_info {
+  size_t n_submaps, n_segments, n_points;
+  int n_loop_edges, num_adjacent_pose_cnstraints, adjusted;
+  unsigned long long n_bytes; /* bytes written / read, all files */
+} b200sm_session_io_info;
+/* Save the session into dir (created when missing, as is dir/submaps; files of an earlier save that this one does not name
+ * are left alone). loop_edges / num_adjacent_pose_cnstraints are b200sm_pose_adjust's; adjusted_poses_colmajor16 (may be
+ * NULL) = 16 * n_submaps doubles, e.g. its output. The submap bodies come to the host through two pinned buffers, the
+ * next copy overlapping the current write. An existing session.txt is removed before the first submap file is opened;
+ * the new one is written to session.txt.tmp and renamed into place only after every other file closed without error, so
+ * a failed save never leaves a manifest that names a partial file. B200REG_ERR_ARG before any file is touched for an
+ * empty session, num_adjacent_pose_cnstraints < 1, a loop edge id outside [0, n_submaps) or with from == to, or a
+ * non-finite relative or adjusted pose; B200REG_ERR_IO for a file or directory that cannot be created or written. */
+int b200sm_save_session(b200sm_t s, const char* dir, int num_adjacent_pose_cnstraints, const b200sm_loop_edge* loop_edges,
+                        int n_loop_edges, const double* adjusted_poses_colmajor16, b200sm_session_io_info* info);
+/* Load dir into an empty session (no submaps, frames or imports; otherwise B200REG_ERR_ARG). The manifest is parsed whole
+ * first; every submap file is read by b200reg_load_pcd's reader (a binary body unpacked on the device) and its POINTS must
+ * be the manifest's count. The result is the session b200sm_import_submap of every saved submap in order gives, with the
+ * saved segments and Scan Context parameters (descriptors are rebuilt lazily, bitwise). A loaded session is a backend's
+ * map: b200sm_set_scan, b200sm_receive_cloud and b200sm_update_map return B200REG_ERR_ARG on it; b200sm_import_submap
+ * appends to its last segment. B200REG_ERR_IO: a file cannot be opened or read. B200REG_ERR_FORMAT: the manifest
+ * deviates from its format (b200sm_last_error names the line) or a submap file is not what it says. After either, and
+ * after B200REG_ERR_ARG, the session is as it was: empty, with its Scan Context parameters, holding no submap memory.
+ * After B200REG_ERR_CUDA it holds no submaps. */
+int b200sm_load_session(b200sm_t s, const char* dir, b200sm_session_io_info* info);
+/* The graph the loaded session was saved with: *n_loop_edges = L, min(capacity, L) loop edges copied;
+ * adjusted_poses_colmajor16 (may be NULL) receives 16 * n doubles (n: submaps at the save) when it was saved with adjusted
+ * poses; *num_adjacent_pose_cnstraints (may be NULL). A session that was not loaded: B200REG_ERR_ARG. */
+int b200sm_get_session_graph(b200sm_t s, b200sm_loop_edge* loop_edges, size_t capacity, size_t* n_loop_edges,
+                             double* adjusted_poses_colmajor16, int* num_adjacent_pose_cnstraints);
 /* The map of every submap moved by a pose cast to float (modified map gbs.cpp:321-368; publishMap sm.cpp:529-552 when
  * poses == NULL, i.e. the submaps' own poses), assembled on the device in one launch. Output is x, y, z, intensity
  * floats in submap order. *n = total points; min(*n, capacity) points are copied, so capacity 0 is a size query (it

@@ -508,6 +508,29 @@ class ScanMatcherSession {
     if (r.merged) poses_out.swap(poses);
     return r;
   }
+  // ---- the session on disk (b200sm_save_session / b200sm_load_session): dir/session.txt, dir/pose_graph.g2o and one binary
+  // PCD per submap under dir/submaps. adjusted_poses: empty, or 16 * numSubmaps() doubles column-major (poseAdjust's output)
+  b200sm_session_io_info saveSession(const std::string& dir, const std::vector<b200sm_loop_edge>& loop_edges = {},
+                                     int num_adjacent_pose_cnstraints = 5, const std::vector<double>& adjusted_poses = {}) {
+    b200sm_session_io_info info{};
+    if (!adjusted_poses.empty() && adjusted_poses.size() != 16 * numSubmaps())
+      throw std::runtime_error("saveSession: adjusted_poses must hold 16 doubles per submap");
+    check(b200sm_save_session(s_.get(), dir.c_str(), num_adjacent_pose_cnstraints, loop_edges.empty() ? nullptr : loop_edges.data(),
+                              (int)loop_edges.size(), adjusted_poses.empty() ? nullptr : adjusted_poses.data(), &info));
+    return info;
+  }
+  // into this (empty) session; loop_edges, adjusted_poses (empty when saved without) and k: the graph it was saved with
+  b200sm_session_io_info loadSession(const std::string& dir, std::vector<b200sm_loop_edge>& loop_edges, std::vector<double>& adjusted_poses,
+                                     int& num_adjacent_pose_cnstraints) {
+    b200sm_session_io_info info{};
+    check(b200sm_load_session(s_.get(), dir.c_str(), &info));
+    size_t n = 0;
+    loop_edges.resize(info.n_loop_edges);
+    adjusted_poses.assign(info.adjusted ? 16 * info.n_submaps : 0, 0.0);
+    check(b200sm_get_session_graph(s_.get(), loop_edges.empty() ? nullptr : loop_edges.data(), loop_edges.size(), &n,
+                                   adjusted_poses.empty() ? nullptr : adjusted_poses.data(), &num_adjacent_pose_cnstraints));
+    return info;
+  }
   // ---- occupancy grid for a navigation stack (b200sm_build_occupancy_grid): poses empty = the submaps' own, else 16 doubles
   // per submap, column-major (b200sm_pose_adjust's output); p nullptr = the defaults
   b200sm_occupancy_info buildOccupancyGrid(const std::vector<double>& poses_colmajor16 = {},

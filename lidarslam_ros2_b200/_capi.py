@@ -52,6 +52,7 @@ SYMBOLS = [
     "b200sm_build_occupancy_grid", "b200sm_get_occupancy_grid", "b200sm_save_occupancy_map",
     "b200sm_build_static_map", "b200sm_get_static_map", "b200sm_get_map_voxels", "b200sm_save_static_map_pcd_ascii",
     "b200sm_merge_session", "b200sm_get_merge_scores", "b200sm_get_segments",
+    "b200sm_save_session", "b200sm_load_session", "b200sm_get_session_graph",
     # include/b200comm.h
     "b200comm_unique_id", "b200comm_create", "b200comm_destroy", "b200comm_all_gather_rows", "b200comm_rank", "b200comm_last_error",
     "b200comm_board_create", "b200comm_board_destroy", "b200comm_board_info",
@@ -126,6 +127,11 @@ class SmMergeResult(C.Structure):
     _fields_ = [("merged", C.c_int), ("query_tile", C.c_int), ("pairs_scored", C.c_ulonglong), ("candidates", C.c_int),
                 ("verified", C.c_int), ("accepted", C.c_int), ("inliers", C.c_int), ("first_submap", C.c_int),
                 ("T", C.c_double * 16), ("adjust", SmPoseAdjustResult)]
+
+
+class SmSessionIoInfo(C.Structure):
+    _fields_ = [("n_submaps", C.c_size_t), ("n_segments", C.c_size_t), ("n_points", C.c_size_t), ("n_loop_edges", C.c_int),
+                ("num_adjacent_pose_cnstraints", C.c_int), ("adjusted", C.c_int), ("n_bytes", C.c_ulonglong)]
 
 
 class SmStats(C.Structure):
@@ -299,6 +305,9 @@ def lib() -> C.CDLL:
                                         C.POINTER(SmMergeResult)]
     L.b200sm_get_merge_scores.argtypes = [vp, sz, C.POINTER(sz), C.POINTER(sz), vp, vp]
     L.b200sm_get_segments.argtypes = [vp, vp, sz, C.POINTER(sz)]
+    L.b200sm_save_session.argtypes = [vp, C.c_char_p, i, vp, i, vp, C.POINTER(SmSessionIoInfo)]
+    L.b200sm_load_session.argtypes = [vp, C.c_char_p, C.POINTER(SmSessionIoInfo)]
+    L.b200sm_get_session_graph.argtypes = [vp, vp, sz, C.POINTER(sz), vp, C.POINTER(i)]
     L.b200comm_unique_id.argtypes = [vp]
     L.b200comm_create.argtypes = [vp, i, i, i, C.POINTER(vp)]
     L.b200comm_destroy.argtypes = [vp]

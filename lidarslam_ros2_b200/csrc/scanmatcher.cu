@@ -33,6 +33,8 @@
 #include <string>
 #include <vector>
 
+#include <sys/stat.h>
+
 #include "../../include/b200reg.h"
 #include "deskew.hpp"
 #include "engine.hpp"
@@ -43,6 +45,7 @@
 #include "pose_graph.hpp"
 #include "scan_context.hpp"
 #include "sensor_frame.hpp"
+#include "session_io.hpp"
 #include "session_merge.hpp"
 #include "static_map.cuh"
 
@@ -261,6 +264,12 @@ struct b200sm_session {
   // first submap of every segment (one recording's contiguous run of submaps); b200sm_merge_session appends one per merge.
   // A session of more than one segment is a backend's map: the frontend's calls are refused on it.
   std::vector<int> seg_first{0};
+  // b200sm_load_session: the session is a saved map (a backend's map: the frontend's calls are refused on it), and the graph
+  // it was saved with (loop edges, num_adjacent_pose_cnstraints, the adjusted poses or none)
+  bool loaded = false;
+  std::vector<sio::LoopEdge> graph_loops;
+  int graph_k = 0;
+  std::vector<double> graph_poses;
   DeviceBuffer<float4> targeted;
   size_t n_targeted = 0;
   DeviceBuffer<float4> loop_src, loop_tgt;  // search_loop scratch
@@ -645,6 +654,7 @@ int b200sm_set_scan(b200sm_t s, b200reg_t reg, const float* points, size_t n, si
       (intensity_offset_bytes >= 0 && (intensity_offset_bytes % 4) != 0))
     return B200REG_ERR_ARG;
   if (s->seg_first.size() > 1) return sm_fail(s, B200REG_ERR_ARG, "set_scan: the session holds a merged map of several recordings");
+  if (s->loaded) return sm_fail(s, B200REG_ERR_ARG, "set_scan: the session holds a map loaded by b200sm_load_session");
   return sm_guarded(s, [&]() {
     upload_frame(s, points, n, stride_bytes, intensity_offset_bytes);
     const int rc = set_source_from_scan(s, reg);
@@ -657,6 +667,7 @@ int b200sm_update_map(b200sm_t s, b200reg_t reg, const float* final_T_colmajor16
                       int adopt_now) {
   if (!s || !final_T_colmajor16 || !position3 || !quat_xyzw) return B200REG_ERR_ARG;
   if (s->seg_first.size() > 1) return sm_fail(s, B200REG_ERR_ARG, "update_map: the session holds a merged map of several recordings");
+  if (s->loaded) return sm_fail(s, B200REG_ERR_ARG, "update_map: the session holds a map loaded by b200sm_load_session");
   return sm_guarded(s, [&]() {
     float T[16];
     for (int r = 0; r < 4; r++)
@@ -682,6 +693,7 @@ int b200sm_receive_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t 
                          double* pose7_out, float* final_T_colmajor16_out, int* map_updated) {
   if (!valid_frame_args(s, reg, points, n, stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
   if (s->seg_first.size() > 1) return sm_fail(s, B200REG_ERR_ARG, "receive_cloud: the session holds a merged map of several recordings");
+  if (s->loaded) return sm_fail(s, B200REG_ERR_ARG, "receive_cloud: the session holds a map loaded by b200sm_load_session");
   return sm_guarded(s, [&]() {
     if (map_updated) *map_updated = 0;
     const bool use_odom = s->odom_armed;  // armed for this frame only, like the de-skew
@@ -2020,6 +2032,281 @@ int b200sm_get_segments(b200sm_t s, size_t* first, size_t capacity, size_t* n) {
   const size_t total = s->submaps.empty() ? 0 : s->seg_first.size();
   *n = total;
   for (size_t k = 0; k < std::min(capacity, total); k++) first[k] = (size_t)s->seg_first[k];
+  return B200REG_OK;
+}
+
+}  // extern "C"
+
+// ---- saving and loading a session (csrc/session_io.hpp) ----
+namespace {
+
+constexpr size_t SIO_PIECE_BYTES = (size_t)16 << 20;  // largest device-to-host copy of a submap body: 1 Mi points
+
+int sio_io_fail(b200sm_t s, const std::string& why) {
+  s->err = why;
+  return (int)B200REG_ERR_IO;
+}
+
+bool sio_make_dir(const std::string& d) {
+  struct stat st;
+  if (mkdir(d.c_str(), 0777) == 0) return true;
+  return errno == EEXIST && stat(d.c_str(), &st) == 0 && S_ISDIR(st.st_mode);
+}
+
+bool sio_write_text(const std::string& path, const std::string& text) {
+  FILE* fp = std::fopen(path.c_str(), "wb");
+  if (!fp) return false;
+  const bool ok = std::fwrite(text.data(), 1, text.size(), fp) == text.size();
+  return (std::fclose(fp) == 0) && ok;
+}
+
+// Every submap file: the binary PCD header, then the submap's float4 rows as they are on the device. The rows come to the
+// host in pieces of at most SIO_PIECE_BYTES through the two pinned staging buffers in turn, and piece p + 1 is copied
+// while this thread writes piece p (write_pcd_ascii's scheme); a buffer is refilled only after its previous piece has
+// been written. An empty submap is a header alone.
+int sio_write_submaps(b200sm_t s, const std::string& sub_dir, unsigned long long* bytes) {
+  struct Piece {
+    size_t sub, first, count;  // points
+  };
+  const size_t per_piece = SIO_PIECE_BYTES / sizeof(float4);
+  std::vector<Piece> pieces;
+  size_t most = 1;
+  for (size_t i = 0; i < s->submaps.size(); i++) {
+    const size_t n = s->submaps[i]->n;
+    size_t first = 0;
+    do {
+      const size_t c = std::min(per_piece, n - first);
+      pieces.push_back({i, first, c});
+      most = std::max(most, c * sizeof(float4));
+      first += c;
+    } while (first < n);
+  }
+  for (auto& st : s->pcd_staging) st.ensure(most);
+  cudaEvent_t copied[2] = {nullptr, nullptr};
+  FILE* fp = nullptr;
+  struct Cleanup {  // on every return: no copy into the staging buffers left in flight, no file left open
+    cudaEvent_t* ev;
+    FILE** fp;
+    cudaStream_t st;
+    ~Cleanup() {
+      cudaStreamSynchronize(st);
+      for (int b = 0; b < 2; b++)
+        if (ev[b]) cudaEventDestroy(ev[b]);
+      if (*fp) std::fclose(*fp);
+    }
+  } cleanup{copied, &fp, s->stream};
+  for (cudaEvent_t& e : copied) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  auto enqueue = [&](size_t p) {
+    const Piece& q = pieces[p];
+    if (q.count)
+      B200_CUDA(cudaMemcpyAsync(s->pcd_staging[p & 1].ptr, s->submaps[q.sub]->cloud + q.first, q.count * sizeof(float4),
+                                cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaEventRecord(copied[p & 1], s->stream));
+  };
+  enqueue(0);
+  std::string path;
+  for (size_t p = 0; p < pieces.size(); p++) {
+    if (p + 1 < pieces.size()) enqueue(p + 1);  // its buffer held piece p - 1, already written
+    const Piece& q = pieces[p];
+    const size_t n = s->submaps[q.sub]->n;
+    if (q.first == 0) {
+      path = sub_dir + "/" + sio::submap_name(q.sub);
+      fp = std::fopen(path.c_str(), "wb");
+      if (!fp) return sio_io_fail(s, "save_session: cannot create " + path + ": " + std::strerror(errno));
+      const std::string header = sio::pcd_binary_header(n);
+      if (std::fwrite(header.data(), 1, header.size(), fp) != header.size())
+        return sio_io_fail(s, "save_session: writing " + path + ": " + std::strerror(errno));
+      *bytes += header.size();
+    }
+    B200_CUDA(cudaEventSynchronize(copied[p & 1]));
+    const size_t b = q.count * sizeof(float4);
+    if (b && std::fwrite(s->pcd_staging[p & 1].ptr, 1, b, fp) != b)
+      return sio_io_fail(s, "save_session: writing " + path + ": " + std::strerror(errno));
+    *bytes += b;
+    if (q.first + q.count == n) {
+      const int rc = std::fclose(fp);
+      fp = nullptr;
+      if (rc != 0) return sio_io_fail(s, "save_session: writing " + path + ": " + std::strerror(errno));
+    }
+  }
+  return (int)B200REG_OK;
+}
+
+bool sio_session_empty(b200sm_t s) { return s->submaps.empty() && !s->d_scan && !s->initial_cloud_received && !s->loaded; }
+
+}  // namespace
+
+extern "C" {
+
+int b200sm_save_session(b200sm_t s, const char* dir, int num_adjacent_pose_cnstraints, const b200sm_loop_edge* loop_edges,
+                        int n_loop_edges, const double* adjusted_poses_colmajor16, b200sm_session_io_info* info) {
+  if (!s || !dir || !*dir || num_adjacent_pose_cnstraints < 1 || n_loop_edges < 0 || (n_loop_edges && !loop_edges))
+    return s ? sm_fail(s, B200REG_ERR_ARG, "save_session: a NULL or empty argument, num_adjacent_pose_cnstraints < 1 or n_loop_edges < 0")
+             : B200REG_ERR_ARG;
+  const size_t n = s->submaps.size();
+  if (n == 0) return sm_fail(s, B200REG_ERR_ARG, "save_session: the session has no submaps");
+  for (int l = 0; l < n_loop_edges; l++) {
+    const b200sm_loop_edge& e = loop_edges[l];
+    if (e.from < 0 || e.from >= (int)n || e.to < 0 || e.to >= (int)n || e.from == e.to)
+      return sm_fail(s, B200REG_ERR_ARG, "save_session: loop edge with a submap id out of range or from == to");
+    for (int k = 0; k < 16; k++)
+      if (!std::isfinite(e.relative_pose[k])) return sm_fail(s, B200REG_ERR_ARG, "save_session: non-finite relative_pose");
+  }
+  if (adjusted_poses_colmajor16)
+    for (size_t k = 0; k < 16 * n; k++)
+      if (!std::isfinite(adjusted_poses_colmajor16[k])) return sm_fail(s, B200REG_ERR_ARG, "save_session: non-finite adjusted pose");
+  return sm_guarded(s, [&]() {
+    sio::Manifest m;
+    m.sc = s->sc;
+    m.seg_first = s->seg_first;
+    m.points.resize(n);
+    m.distance.resize(n);
+    m.pose.resize(16 * n);
+    for (size_t i = 0; i < n; i++) {
+      const Submap& sub = *s->submaps[i];
+      m.points[i] = sub.n;
+      m.distance[i] = sub.distance;
+      for (int r = 0; r < 4; r++)
+        for (int c = 0; c < 4; c++) m.pose[16 * i + c * 4 + r] = sub.pose[r * 4 + c];
+    }
+    m.k = num_adjacent_pose_cnstraints;
+    m.loops.resize(n_loop_edges);
+    for (int l = 0; l < n_loop_edges; l++) {
+      m.loops[l].from = loop_edges[l].from;
+      m.loops[l].to = loop_edges[l].to;
+      std::memcpy(m.loops[l].rel, loop_edges[l].relative_pose, sizeof(m.loops[l].rel));
+    }
+    m.adjusted = adjusted_poses_colmajor16 != nullptr;
+    if (m.adjusted) m.adjusted_pose.assign(adjusted_poses_colmajor16, adjusted_poses_colmajor16 + 16 * n);
+    const std::string d = dir, sub_dir = d + "/submaps", manifest = d + "/session.txt", tmp = manifest + ".tmp";
+    if (!sio_make_dir(d) || !sio_make_dir(sub_dir))
+      return sio_io_fail(s, "save_session: cannot create " + sub_dir + ": " + std::strerror(errno));
+    // no manifest may name a submap file while it is being rewritten
+    if (std::remove(manifest.c_str()) != 0 && errno != ENOENT)
+      return sio_io_fail(s, "save_session: cannot remove " + manifest + ": " + std::strerror(errno));
+    unsigned long long bytes = 0;
+    int rc = sio_write_submaps(s, sub_dir, &bytes);
+    if (rc != B200REG_OK) return rc;
+    const std::string g2o = sio::write_g2o(m), text = sio::write_manifest(m);
+    if (!sio_write_text(d + "/pose_graph.g2o", g2o))
+      return sio_io_fail(s, "save_session: writing " + d + "/pose_graph.g2o: " + std::strerror(errno));
+    if (!sio_write_text(tmp, text)) {
+      const int e = errno;
+      std::remove(tmp.c_str());
+      return sio_io_fail(s, "save_session: writing " + tmp + ": " + std::strerror(e));
+    }
+    if (std::rename(tmp.c_str(), manifest.c_str()) != 0)
+      return sio_io_fail(s, "save_session: renaming " + tmp + ": " + std::strerror(errno));
+    bytes += g2o.size() + text.size();
+    if (info) {
+      std::size_t pts = 0;
+      for (unsigned long long p : m.points) pts += (size_t)p;
+      info->n_submaps = n;
+      info->n_segments = m.seg_first.size();
+      info->n_points = pts;
+      info->n_loop_edges = n_loop_edges;
+      info->num_adjacent_pose_cnstraints = m.k;
+      info->adjusted = m.adjusted ? 1 : 0;
+      info->n_bytes = bytes;
+    }
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_load_session(b200sm_t s, const char* dir, b200sm_session_io_info* info) {
+  if (!s || !dir || !*dir) return s ? sm_fail(s, B200REG_ERR_ARG, "load_session: a NULL or empty directory") : B200REG_ERR_ARG;
+  if (!sio_session_empty(s))
+    return sm_fail(s, B200REG_ERR_ARG, "load_session: the session is not empty (it holds submaps or has received frames)");
+  return sm_guarded(s, [&]() {
+    const std::string d = dir, path = d + "/session.txt";
+    // (1) the whole manifest, parsed before anything is allocated
+    std::string text;
+    {
+      FILE* fp = std::fopen(path.c_str(), "rb");
+      if (!fp) return sio_io_fail(s, "load_session: cannot open " + path + ": " + std::strerror(errno));
+      char buf[1 << 16];
+      size_t got;
+      while ((got = std::fread(buf, 1, sizeof buf, fp)) > 0) text.append(buf, got);
+      const bool bad = std::ferror(fp) != 0;
+      std::fclose(fp);
+      if (bad) return sio_io_fail(s, "load_session: reading " + path);
+    }
+    sio::Manifest m;
+    std::string why;
+    if (!sio::parse_manifest(text, m, why)) return sm_fail(s, B200REG_ERR_FORMAT, ("load_session: " + path + " " + why).c_str());
+    // (2) every submap file through the PCD reader (a binary body is unpacked on the device by the upload kernel), its
+    // rows copied device to device into an arena of the load's own; the session takes it over only when all are in
+    const size_t n = m.n();
+    SubmapArena arena;
+    std::vector<std::unique_ptr<Submap>> subs;
+    DeviceBuffer<float4> rows;
+    unsigned long long bytes = text.size(), pts = 0;
+    for (size_t i = 0; i < n; i++) {
+      const std::string file = d + "/submaps/" + sio::submap_name(i);
+      size_t got = 0;
+      const int before = s->pcd_loader.launches;
+      const int rc = s->pcd_loader.load(file.c_str(), rows, &got, why, s->stream);
+      s->launches += s->pcd_loader.launches - before;
+      if (rc != B200REG_OK) {
+        s->err = "load_session: " + file + ": " + why;
+        return rc;
+      }
+      if (got != m.points[i])
+        return sm_fail(s, B200REG_ERR_FORMAT, ("load_session: " + file + ": POINTS " + std::to_string(got) + ", the manifest says " +
+                                               std::to_string(m.points[i])).c_str());
+      struct stat st;
+      if (stat(file.c_str(), &st) == 0) bytes += (unsigned long long)st.st_size;
+      std::unique_ptr<Submap> sub(new Submap());
+      sub->cloud = arena.alloc(std::max<size_t>(got, 1));
+      sub->n = got;
+      // stream-ordered before the next file's upload into `rows`
+      if (got) B200_CUDA(cudaMemcpyAsync(sub->cloud, rows.ptr, got * sizeof(float4), cudaMemcpyDeviceToDevice, s->stream));
+      for (int r = 0; r < 4; r++)
+        for (int c = 0; c < 4; c++) sub->pose[r * 4 + c] = m.pose[16 * i + c * 4 + r];
+      sub->distance = m.distance[i];
+      pts += got;
+      subs.push_back(std::move(sub));
+    }
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    // (3) what b200sm_import_submap of every submap in order gives, then the segments and the Scan Context parameters
+    std::swap(s->arena.chunks, arena.chunks);
+    s->arena.used = arena.used;
+    s->arena.cap = arena.cap;
+    s->submaps = std::move(subs);
+    s->seg_first = m.seg_first;
+    s->latest_distance = s->submaps.back()->distance;
+    s->sc = m.sc;
+    sc_drop(s);
+    s->loaded = true;
+    s->graph_loops = m.loops;
+    s->graph_k = m.k;
+    s->graph_poses = m.adjusted_pose;
+    if (info) {
+      info->n_submaps = n;
+      info->n_segments = m.seg_first.size();
+      info->n_points = (size_t)pts;
+      info->n_loop_edges = (int)m.loops.size();
+      info->num_adjacent_pose_cnstraints = m.k;
+      info->adjusted = m.adjusted ? 1 : 0;
+      info->n_bytes = bytes;
+    }
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_session_graph(b200sm_t s, b200sm_loop_edge* loop_edges, size_t capacity, size_t* n_loop_edges,
+                             double* adjusted_poses_colmajor16, int* num_adjacent_pose_cnstraints) {
+  if (!s || !n_loop_edges || (!loop_edges && capacity)) return s ? sm_fail(s, B200REG_ERR_ARG, "get_session_graph: a NULL argument") : B200REG_ERR_ARG;
+  if (!s->loaded) return sm_fail(s, B200REG_ERR_ARG, "get_session_graph: the session was not loaded by b200sm_load_session");
+  *n_loop_edges = s->graph_loops.size();
+  for (size_t l = 0; l < std::min(capacity, s->graph_loops.size()); l++) {
+    loop_edges[l].from = s->graph_loops[l].from;
+    loop_edges[l].to = s->graph_loops[l].to;
+    std::memcpy(loop_edges[l].relative_pose, s->graph_loops[l].rel, sizeof(loop_edges[l].relative_pose));
+  }
+  if (adjusted_poses_colmajor16 && !s->graph_poses.empty())
+    std::memcpy(adjusted_poses_colmajor16, s->graph_poses.data(), s->graph_poses.size() * sizeof(double));
+  if (num_adjacent_pose_cnstraints) *num_adjacent_pose_cnstraints = s->graph_k;
   return B200REG_OK;
 }
 

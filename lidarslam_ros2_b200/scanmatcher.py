@@ -14,6 +14,15 @@ from . import _capi
 from .registration import B200RegError, GeneralizedIterativeClosestPoint, NormalDistributionsTransform, _as_cloud, _ptr
 
 
+def _loop_edges(loop_edges):
+    """(from, to, relative_pose 4x4) tuples as a b200sm_loop_edge array (at least one element)."""
+    edges = (_capi.SmLoopEdge * max(1, len(loop_edges)))()
+    for k, (f, t, Z) in enumerate(loop_edges):
+        edges[k].from_, edges[k].to = int(f), int(t)
+        edges[k].relative_pose[:] = np.asarray(Z, dtype=np.float64).T.reshape(16).tolist()
+    return edges
+
+
 class ScanMatcher:
     """Parameters carry the reference's names and defaults (scanmatcher_component.cpp:26-50)."""
 
@@ -382,6 +391,42 @@ class ScanMatcher:
         out = np.zeros(max(1, n.value), dtype=np.uint64)
         self._check(self._lib.b200sm_get_segments(self._h, _ptr(out), n.value, C.byref(n)))
         return [int(v) for v in out[:n.value]]
+
+    # ---- saving and loading a session (b200sm_save_session / b200sm_load_session) ----
+    def saveSession(self, dir, loop_edges=(), num_adjacent_pose_cnstraints: int = 5, poses=None) -> dict:
+        """Save the session into directory `dir`: session.txt (the manifest), pose_graph.g2o (the reference's
+        optimizer.save output) and submaps/%06zu.pcd (binary PCD, sensor frame). loop_edges: (from, to, relative_pose 4x4)
+        as poseAdjust takes them; poses: the adjusted poses (N, 4, 4) or None. Returns the info dict (n_bytes: all files)."""
+        edges = _loop_edges(loop_edges)
+        n = self.numSubmaps()
+        P = None
+        if poses is not None:
+            P = np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(-1, 4, 4).transpose(0, 2, 1)).reshape(-1)
+            if P.size != 16 * n:
+                raise ValueError(f"saveSession: {P.size // 16} poses for {n} submaps")
+        info = _capi.SmSessionIoInfo()
+        self._check(self._lib.b200sm_save_session(self._h, os.fsencode(dir), int(num_adjacent_pose_cnstraints), edges,
+                                                  len(loop_edges), _ptr(P) if P is not None else None, C.byref(info)))
+        return {k: getattr(info, k) for k, _ in _capi.SmSessionIoInfo._fields_}
+
+    def loadSession(self, dir):
+        """Load a directory saveSession wrote into this (empty) session. Returns (loop_edges, poses, k, info): the graph it
+        was saved with (edges as (from, to, relative_pose 4x4), the adjusted poses (N, 4, 4) or None,
+        num_adjacent_pose_cnstraints) and the info dict."""
+        info = _capi.SmSessionIoInfo()
+        self._check(self._lib.b200sm_load_session(self._h, os.fsencode(dir), C.byref(info)))
+        with open(os.path.join(dir, "session.txt"), "rb") as f:  # the restored descriptor grid: line 2 of the manifest
+            f.readline()
+            tok = f.readline().split()
+        self._scp = (int(tok[1]), int(tok[2]))
+        L, n = int(info.n_loop_edges), int(info.n_submaps)
+        edges = (_capi.SmLoopEdge * max(1, L))()
+        got, k = C.c_size_t(0), C.c_int(0)
+        P = np.zeros((max(1, n), 16), dtype=np.float64)
+        self._check(self._lib.b200sm_get_session_graph(self._h, edges, L, C.byref(got), _ptr(P), C.byref(k)))
+        out = [(int(e.from_), int(e.to), np.array(e.relative_pose, dtype=np.float64).reshape(4, 4).T.copy()) for e in edges[:L]]
+        poses = P[:n].reshape(n, 4, 4).transpose(0, 2, 1).copy() if info.adjusted else None
+        return out, poses, int(k.value), {k_: getattr(info, k_) for k_, _ in _capi.SmSessionIoInfo._fields_}
 
     def assembleMap(self, poses=None, capacity=None):
         """The map of every submap moved by its pose cast to float (publishMap sm.cpp:529-552 when poses is None, else the
