@@ -97,14 +97,6 @@ namespace {
 void set_identity(float* T) {
   for (int k = 0; k < 16; k++) T[k] = (k % 5 == 0) ? 1.0f : 0.0f;
 }
-void col_to_row(const float* c, float* r) {
-  for (int i = 0; i < 4; i++)
-    for (int j = 0; j < 4; j++) r[i * 4 + j] = c[j * 4 + i];
-}
-void row_to_col(const float* r, float* c) {
-  for (int i = 0; i < 4; i++)
-    for (int j = 0; j < 4; j++) c[j * 4 + i] = r[i * 4 + j];
-}
 
 template <typename F>
 int guarded(b200reg_t h, F&& f) {

@@ -75,6 +75,18 @@ struct Mat34f {
   float m[12];
 };
 
+// 4x4 column-major <-> row-major, each entry static_cast to the destination's element type
+template <typename S, typename D>
+inline void col_to_row(const S* c, D* r) {
+  for (int i = 0; i < 4; i++)
+    for (int j = 0; j < 4; j++) r[i * 4 + j] = static_cast<D>(c[j * 4 + i]);
+}
+template <typename S, typename D>
+inline void row_to_col(const S* r, D* c) {
+  for (int i = 0; i < 4; i++)
+    for (int j = 0; j < 4; j++) c[j * 4 + i] = static_cast<D>(r[i * 4 + j]);
+}
+
 // ---- small PTX helpers ------------------------------------------------------------------------------
 #ifdef __CUDACC__
 __device__ __forceinline__ unsigned ld_relaxed_gpu(const unsigned* p) {
@@ -91,6 +103,19 @@ __device__ __forceinline__ unsigned atom_add_acq_rel_gpu(unsigned* p, unsigned v
   return old;
 }
 __device__ __forceinline__ void fence_acq_rel_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
+
+// The entry of a launch's table that serves `v` (a tile, a word): the last of the n entries whose `key` is <= v (the
+// table is sorted by `key`, its first entry's key is 0; an entry that owns nothing shares its key with the next one).
+template <typename E, typename K, typename V>
+__device__ __forceinline__ int entry_of(const E* __restrict__ table, int n, V v, K E::*key) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (table[mid].*key <= v) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
 
 // order-preserving float <-> uint mapping for atomicMin/atomicMax on floats
 __device__ __forceinline__ unsigned float_to_ordered(float f) {

@@ -7,17 +7,6 @@
 namespace b200 {
 namespace {
 
-// the entry of tile `tile`: the last one with first_tile <= tile (empty submaps own no tile)
-__device__ __forceinline__ int og_entry_of(const OgEntry* __restrict__ table, int n_entries, unsigned tile) {
-  int lo = 0, hi = n_entries - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (table[mid].first_tile <= tile) lo = mid;
-    else hi = mid - 1;
-  }
-  return lo;
-}
-
 __device__ __forceinline__ OgConst og_const(double S, long long R, long long zlo, long long zhi) {
   OgConst c;
   c.S = S;
@@ -33,7 +22,7 @@ __device__ __forceinline__ OgConst og_const(double S, long long R, long long zlo
 __global__ void __launch_bounds__(OG_THREADS) og_bounds_kernel(const OgEntry* __restrict__ table, int n_entries, double S, long long R,
                                                                long long zlo, long long zhi, int* __restrict__ bounds,
                                                                unsigned long long* __restrict__ counters) {
-  const int k = og_entry_of(table, n_entries, blockIdx.x);
+  const int k = entry_of(table, n_entries, blockIdx.x, &OgEntry::first_tile);
   const OgEntry& e = table[k];
   const OgConst c = og_const(S, R, zlo, zhi);
   const unsigned base = (blockIdx.x - e.first_tile) * (unsigned)OG_TILE + threadIdx.x;
@@ -94,7 +83,7 @@ __device__ __forceinline__ void og_mark(uint32_t* words, unsigned stride, int x0
 __global__ void __launch_bounds__(OG_THREADS) og_walk_kernel(const OgEntry* __restrict__ table, int n_entries, double S, long long R,
                                                              long long zlo, long long zhi, uint32_t* __restrict__ scratch,
                                                              unsigned long long* __restrict__ counters) {
-  const int k = og_entry_of(table, n_entries, blockIdx.x);
+  const int k = entry_of(table, n_entries, blockIdx.x, &OgEntry::first_tile);
   const OgEntry& e = table[k];
   const OgConst c = og_const(S, R, zlo, zhi);
   const int x0 = e.x0, y0 = e.y0;
@@ -126,13 +115,7 @@ __global__ void __launch_bounds__(OG_THREADS) og_fold_kernel(const OgEntry* __re
                                                              uint32_t* __restrict__ hits, uint32_t* __restrict__ frees) {
   const unsigned long long g = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
   if (g >= fold_words) return;
-  int lo = 0, hi = n_entries - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (table[mid].fold_first <= g) lo = mid;
-    else hi = mid - 1;
-  }
-  const OgEntry& e = table[lo];
+  const OgEntry& e = table[entry_of(table, n_entries, g, &OgEntry::fold_first)];
   const unsigned long long w = g - e.fold_first;
   const uint32_t h = scratch[e.words_at + w];
   const uint32_t f = scratch[e.words_at + (unsigned long long)e.stride * e.rows + w] & ~h;

@@ -28,13 +28,7 @@ __global__ void __launch_bounds__(SC_BUILD_THREADS) scan_context_kernel(const Sc
   for (int k = threadIdx.x; k < num_rings + 2 * num_sectors; k += blockDim.x) sc_smem[k] = tables[k];
   for (int k = threadIdx.x; k < nb; k += blockDim.x) bins[k] = 0u;
   const unsigned tile = blockIdx.x;
-  int lo = 0, hi = n_entries - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (table[mid].first_tile <= tile) lo = mid;
-    else hi = mid - 1;
-  }
-  const ScBuildEntry e = table[lo];
+  const ScBuildEntry e = table[entry_of(table, n_entries, tile, &ScBuildEntry::first_tile)];
   __syncthreads();
   const unsigned base = (tile - e.first_tile) * (unsigned)SC_BUILD_TILE + threadIdx.x;
   for (int j = 0; j < SC_BUILD_PER_THREAD; j++) {

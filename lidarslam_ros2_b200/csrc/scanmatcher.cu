@@ -184,6 +184,19 @@ struct Submap {
   double distance = 0;
 };
 
+// A submap of n rows in `arena` with its row-major pose and travelled distance. The rows are copied device to device from
+// `rows` on `stream`; with rows == nullptr the caller fills them.
+std::unique_ptr<Submap> new_submap(SubmapArena& arena, const float4* rows, size_t n, const double* pose_rowmajor16, double distance,
+                                   cudaStream_t stream) {
+  std::unique_ptr<Submap> sub(new Submap());
+  sub->cloud = arena.alloc(std::max<size_t>(n, 1));
+  sub->n = n;
+  if (rows && n) B200_CUDA(cudaMemcpyAsync(sub->cloud, rows, n * sizeof(float4), cudaMemcpyDeviceToDevice, stream));
+  std::memcpy(sub->pose, pose_rowmajor16, sizeof(sub->pose));
+  sub->distance = distance;
+  return sub;
+}
+
 // Map assembly (publishMap sm.cpp:529-552, modified_map gbs.cpp:321-368): one table entry per submap, uploaded per call.
 struct AssembleEntry {
   const float4* cloud;
@@ -200,13 +213,7 @@ constexpr int ASSEMBLE_THREADS = 256, ASSEMBLE_PER_THREAD = 4, ASSEMBLE_TILE = A
 __global__ void __launch_bounds__(ASSEMBLE_THREADS) assemble_map_kernel(const AssembleEntry* __restrict__ table, int n_sub,
                                                                         float4* __restrict__ out) {
   const unsigned tile = blockIdx.x;
-  int lo = 0, hi = n_sub - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (table[mid].first_tile <= tile) lo = mid;
-    else hi = mid - 1;
-  }
-  const AssembleEntry& e = table[lo];
+  const AssembleEntry& e = table[entry_of(table, n_sub, tile, &AssembleEntry::first_tile)];
   float T[12];
 #pragma unroll
   for (int k = 0; k < 12; k++) T[k] = e.T.m[k];
@@ -387,6 +394,50 @@ int sm_fail(b200sm_t s, int code, const char* msg) {
   return code;
 }
 
+// the record layout the uploader reads: x, y, z first, 4-byte fields; no intensity when the offset is negative
+bool valid_layout(size_t stride_bytes, long intensity_offset_bytes) {
+  return stride_bytes >= 12 && (stride_bytes % 4) == 0 && (intensity_offset_bytes < 0 || (intensity_offset_bytes % 4) == 0);
+}
+
+// A session of several segments or loaded from disk is a backend's map: the frontend's calls are refused on it. `what`
+// prefixes the message.
+int refuse_backend_map(b200sm_t s, const char* what) {
+  if (s->seg_first.size() > 1)
+    return sm_fail(s, B200REG_ERR_ARG, (std::string(what) + ": the session holds a merged map of several recordings").c_str());
+  if (s->loaded) return sm_fail(s, B200REG_ERR_ARG, (std::string(what) + ": the session holds a map loaded by b200sm_load_session").c_str());
+  return B200REG_OK;
+}
+
+// the caller's loop edges over submaps [0, n): ids in range, from != to, a finite relative pose. `what` prefixes the
+// messages.
+int check_loop_edges(b200sm_t s, const b200sm_loop_edge* loop_edges, int n_loop_edges, int n, const char* what) {
+  for (int l = 0; l < n_loop_edges; l++) {
+    const b200sm_loop_edge& e = loop_edges[l];
+    if (e.from < 0 || e.from >= n || e.to < 0 || e.to >= n || e.from == e.to)
+      return sm_fail(s, B200REG_ERR_ARG, (std::string(what) + ": loop edge with a submap id out of range or from == to").c_str());
+    for (int k = 0; k < 16; k++)
+      if (!std::isfinite(e.relative_pose[k])) return sm_fail(s, B200REG_ERR_ARG, (std::string(what) + ": non-finite relative_pose").c_str());
+  }
+  return B200REG_OK;
+}
+
+// the caller's loop edges appended to the pose graph's loop list: ids (from, to) and relative poses
+void append_loop_edges(const b200sm_loop_edge* loop_edges, int n_loop_edges, std::vector<int>& ids, std::vector<pg::Iso>& rel) {
+  for (int l = 0; l < n_loop_edges; l++) {
+    ids.push_back(loop_edges[l].from);
+    ids.push_back(loop_edges[l].to);
+    rel.push_back(pg::iso_from_colmajor16(loop_edges[l].relative_pose));
+  }
+}
+
+// a caller's poses (16 column-major per submap), when given, are finite
+bool finite_poses(const double* poses_colmajor16, size_t n_sub) {
+  if (poses_colmajor16)
+    for (size_t k = 0; k < 16 * n_sub; k++)
+      if (!std::isfinite(poses_colmajor16[k])) return false;
+  return true;
+}
+
 void upload_frame(b200sm_t s, const float* points, size_t n, size_t stride, long intensity_off) {
   s->upload.ensure(n);
   // one H2D copy per frame; the unpack pass also moves the points into the robot frame when a sensor transform is set, and
@@ -497,13 +548,9 @@ int update_map(b200sm_t s, const float* final_T, const double* position, const d
   s->n_targeted = total;
   s->launches += 1;
   // the new submap keeps the FILTERED, untransformed cloud and the pose (:465-481)
-  std::unique_ptr<Submap> sub(new Submap());
-  sub->cloud = s->arena.alloc(std::max<size_t>(m, 1));
-  sub->n = m;
-  if (m) B200_CUDA(cudaMemcpyAsync(sub->cloud, filtered, m * sizeof(float4), cudaMemcpyDeviceToDevice, s->stream));
-  pose_to_matrix_d(position, quat, sub->pose);
-  sub->distance = s->latest_distance;
-  s->submaps.push_back(std::move(sub));
+  double pose[16];
+  pose_to_matrix_d(position, quat, pose);
+  s->submaps.push_back(new_submap(s->arena, filtered, m, pose, s->latest_distance, s->stream));
   s->target_pending = true;
   return B200REG_OK;
 }
@@ -533,11 +580,8 @@ int adopt_target(b200sm_t s, b200reg_t reg, int is_gicp) {
 void sim_trans(b200sm_t s, float* T_row, float* sim_col) {
   double M[16];
   pose_to_matrix_d(s->position, s->quat, M);
-  for (int r = 0; r < 4; r++)
-    for (int c = 0; c < 4; c++) {
-      T_row[r * 4 + c] = (float)M[r * 4 + c];
-      sim_col[c * 4 + r] = (float)M[r * 4 + c];
-    }
+  for (int k = 0; k < 16; k++) T_row[k] = (float)M[k];
+  row_to_col(M, sim_col);
 }
 
 // publishMapAndPose's pose (:391-398): position and quaternion of a column-major float final transformation
@@ -559,8 +603,7 @@ int register_frame(b200sm_t s, b200reg_t reg, bool use_odom, float* final_col) {
   sim_trans(s, T_row, sim_col);
   if (use_odom) {  // sim_trans * previous_odom_mat_.inverse() * odom_mat, then previous_odom_mat_ = odom_mat
     odom_guess_f(T_row, s->previous_odom_mat, s->odom_mat);
-    for (int r = 0; r < 4; r++)
-      for (int c = 0; c < 4; c++) sim_col[c * 4 + r] = T_row[r * 4 + c];
+    row_to_col(T_row, sim_col);
   }
   rc = b200reg_align(reg, sim_col, final_col);
   if (rc != B200REG_OK) {
@@ -578,8 +621,7 @@ void write_pose(b200sm_t s, double* pose7_out) {
 }
 
 bool valid_frame_args(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes) {
-  return s && reg && points && n != 0 && stride_bytes >= 12 && (stride_bytes % 4) == 0 &&
-         (intensity_offset_bytes < 0 || (intensity_offset_bytes % 4) == 0);
+  return s && reg && points && n != 0 && valid_layout(stride_bytes, intensity_offset_bytes);
 }
 
 int read_back(b200sm_t s, const float4* d, size_t n, float* out, size_t cap, size_t* n_out) {
@@ -650,11 +692,8 @@ int b200sm_set_initial_pose(b200sm_t s, const double* position3, const double* q
 
 int b200sm_set_scan(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes,
                     size_t* n_filtered) {
-  if (!s || !reg || !points || n == 0 || stride_bytes < 12 || (stride_bytes % 4) != 0 ||
-      (intensity_offset_bytes >= 0 && (intensity_offset_bytes % 4) != 0))
-    return B200REG_ERR_ARG;
-  if (s->seg_first.size() > 1) return sm_fail(s, B200REG_ERR_ARG, "set_scan: the session holds a merged map of several recordings");
-  if (s->loaded) return sm_fail(s, B200REG_ERR_ARG, "set_scan: the session holds a map loaded by b200sm_load_session");
+  if (!valid_frame_args(s, reg, points, n, stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
+  if (const int rc = refuse_backend_map(s, "set_scan"); rc != B200REG_OK) return rc;
   return sm_guarded(s, [&]() {
     upload_frame(s, points, n, stride_bytes, intensity_offset_bytes);
     const int rc = set_source_from_scan(s, reg);
@@ -666,12 +705,10 @@ int b200sm_set_scan(b200sm_t s, b200reg_t reg, const float* points, size_t n, si
 int b200sm_update_map(b200sm_t s, b200reg_t reg, const float* final_T_colmajor16, const double* position3, const double* quat_xyzw,
                       int adopt_now) {
   if (!s || !final_T_colmajor16 || !position3 || !quat_xyzw) return B200REG_ERR_ARG;
-  if (s->seg_first.size() > 1) return sm_fail(s, B200REG_ERR_ARG, "update_map: the session holds a merged map of several recordings");
-  if (s->loaded) return sm_fail(s, B200REG_ERR_ARG, "update_map: the session holds a map loaded by b200sm_load_session");
+  if (const int rc = refuse_backend_map(s, "update_map"); rc != B200REG_OK) return rc;
   return sm_guarded(s, [&]() {
     float T[16];
-    for (int r = 0; r < 4; r++)
-      for (int c = 0; c < 4; c++) T[r * 4 + c] = final_T_colmajor16[c * 4 + r];
+    col_to_row(final_T_colmajor16, T);
     if (!s->submaps.empty()) {  // updateMap :471: latest_distance_ += trans_ (distance travelled since the last submap)
       const double dx = position3[0] - s->previous_position[0], dy = position3[1] - s->previous_position[1],
                    dz = position3[2] - s->previous_position[2];
@@ -692,8 +729,7 @@ int b200sm_update_map(b200sm_t s, b200reg_t reg, const float* final_T_colmajor16
 int b200sm_receive_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes,
                          double* pose7_out, float* final_T_colmajor16_out, int* map_updated) {
   if (!valid_frame_args(s, reg, points, n, stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
-  if (s->seg_first.size() > 1) return sm_fail(s, B200REG_ERR_ARG, "receive_cloud: the session holds a merged map of several recordings");
-  if (s->loaded) return sm_fail(s, B200REG_ERR_ARG, "receive_cloud: the session holds a map loaded by b200sm_load_session");
+  if (const int rc = refuse_backend_map(s, "receive_cloud"); rc != B200REG_OK) return rc;
   return sm_guarded(s, [&]() {
     if (map_updated) *map_updated = 0;
     const bool use_odom = s->odom_armed;  // armed for this frame only, like the de-skew
@@ -724,8 +760,7 @@ int b200sm_receive_cloud(b200sm_t s, b200reg_t reg, const float* points, size_t 
       for (int k = 0; k < 3; k++) s->previous_position[k] = pos[k];
       s->latest_distance += s->trans;  // updateMap :471
       float F_row[16];
-      for (int r = 0; r < 4; r++)
-        for (int c = 0; c < 4; c++) F_row[r * 4 + c] = final_col[c * 4 + r];
+      col_to_row(final_col, F_row);
       rc = update_map(s, F_row, s->position, s->quat);
       if (rc != B200REG_OK) return rc;
       if (map_updated) *map_updated = 1;
@@ -751,9 +786,7 @@ int b200sm_get_submap(b200sm_t s, size_t index, float* out_xyzi, size_t capacity
   if (!s || index >= s->submaps.size()) return B200REG_ERR_ARG;
   return sm_guarded(s, [&]() {
     const Submap& sub = *s->submaps[index];
-    if (pose_colmajor16)
-      for (int r = 0; r < 4; r++)
-        for (int c = 0; c < 4; c++) pose_colmajor16[c * 4 + r] = sub.pose[r * 4 + c];
+    if (pose_colmajor16) row_to_col(sub.pose, pose_colmajor16);
     if (distance) *distance = sub.distance;
     return read_back(s, sub.cloud, sub.n, out_xyzi, capacity, n);
   });
@@ -860,8 +893,7 @@ int loop_evaluate(b200sm_t s, b200reg_t reg, const LoopCandidate& cand, const Su
   if (fitness < threshold_loop_closure_score) {  // :232-246: loop edge (id_min, newest), relative pose from^-1 * (final * init)
     out->accepted = 1;
     double F[16], to[16], rel[16];
-    for (int r = 0; r < 4; r++)
-      for (int c = 0; c < 4; c++) F[r * 4 + c] = (double)fin[c * 4 + r];
+    col_to_row(fin, F);
     for (int r = 0; r < 4; r++)
       for (int c = 0; c < 4; c++) {
         double a = 0;
@@ -877,8 +909,7 @@ int loop_evaluate(b200sm_t s, b200reg_t reg, const LoopCandidate& cand, const Su
         for (int k = 0; k < 4; k++) a += inv[r * 4 + k] * to[k * 4 + c];
         rel[r * 4 + c] = a;
       }
-    for (int r = 0; r < 4; r++)
-      for (int c = 0; c < 4; c++) out->relative_pose[c * 4 + r] = rel[r * 4 + c];
+    row_to_col(rel, out->relative_pose);
   }
   return B200REG_OK;
 }
@@ -952,21 +983,16 @@ int b200sm_search_loop_all(b200sm_t s, b200reg_t reg, float voxel_leaf_size, dou
 // point appends one to the session so that b200sm_search_loop / _all work on device-resident copies there too.
 int b200sm_import_submap(b200sm_t s, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes,
                          const double* pose_colmajor16, double distance) {
-  if (!s || (!points && n) || !pose_colmajor16 || stride_bytes < 12 || (stride_bytes % 4) != 0 ||
-      (intensity_offset_bytes >= 0 && intensity_offset_bytes % 4 != 0))
-    return B200REG_ERR_ARG;
+  if (!s || (!points && n) || !pose_colmajor16 || !valid_layout(stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
   return sm_guarded(s, [&]() {
-    std::unique_ptr<Submap> sub(new Submap());
-    sub->cloud = s->arena.alloc(std::max<size_t>(n, 1));
-    sub->n = n;
+    double pose[16];
+    col_to_row(pose_colmajor16, pose);
+    std::unique_ptr<Submap> sub = new_submap(s->arena, nullptr, n, pose, distance, s->stream);
     if (n) {
       s->uploader.upload(points, n, stride_bytes, intensity_offset_bytes, 0.0f, sub->cloud, s->stream);
       B200_CUDA(cudaStreamSynchronize(s->stream));  // the caller may reuse its buffer
       s->launches += 1;
     }
-    for (int r = 0; r < 4; r++)
-      for (int c = 0; c < 4; c++) sub->pose[r * 4 + c] = pose_colmajor16[c * 4 + r];
-    sub->distance = distance;
     s->latest_distance = distance;
     s->submaps.push_back(std::move(sub));
     return (int)B200REG_OK;
@@ -980,23 +1006,13 @@ int b200sm_pose_adjust(b200sm_t s, int num_adjacent_pose_cnstraints, const b200s
   if (!s || !poses_out || num_adjacent_pose_cnstraints < 1 || max_iterations < 0 || n_loop_edges < 0 || (n_loop_edges && !loop_edges))
     return B200REG_ERR_ARG;
   const int n = (int)s->submaps.size();
-  for (int l = 0; l < n_loop_edges; l++) {
-    const b200sm_loop_edge& e = loop_edges[l];
-    if (e.from < 0 || e.from >= n || e.to < 0 || e.to >= n || e.from == e.to)
-      return sm_fail(s, B200REG_ERR_ARG, "pose_adjust: loop edge with a submap id out of range or from == to");
-    for (int k = 0; k < 16; k++)
-      if (!std::isfinite(e.relative_pose[k])) return sm_fail(s, B200REG_ERR_ARG, "pose_adjust: non-finite relative_pose");
-  }
+  if (const int rc = check_loop_edges(s, loop_edges, n_loop_edges, n, "pose_adjust"); rc != B200REG_OK) return rc;
   return sm_guarded(s, [&]() {
     std::vector<pg::Iso> X(n);
     for (int i = 0; i < n; i++) X[i] = pg::iso_from_rowmajor16(s->submaps[i]->pose);
-    std::vector<int> ids(2 * (size_t)n_loop_edges);
-    std::vector<pg::Iso> rel(n_loop_edges);
-    for (int l = 0; l < n_loop_edges; l++) {
-      ids[2 * l] = loop_edges[l].from;
-      ids[2 * l + 1] = loop_edges[l].to;
-      rel[l] = pg::iso_from_colmajor16(loop_edges[l].relative_pose);
-    }
+    std::vector<int> ids;
+    std::vector<pg::Iso> rel;
+    append_loop_edges(loop_edges, n_loop_edges, ids, rel);
     const std::vector<pg::Edge> edges = pg::build_edges(X, num_adjacent_pose_cnstraints, s->seg_first, ids.data(), rel.data(), n_loop_edges);
     const pg::LmResult r = pg::optimize(X, edges, max_iterations);
     for (int i = 0; i < n; i++) pg::iso_to_colmajor16(X[i], poses_out + 16 * (size_t)i);
@@ -1022,30 +1038,57 @@ size_t map_points(b200sm_t s) {
   return total;
 }
 
+// The table of a launch over submaps [first, size) whose blocks serve `tile` points each: entry r is submap ids[r], whose
+// first tile is first_tile[r]. An empty submap owns no tile (with skip_empty, no entry either). A submap of 2^32 points or
+// more, and more than 2^31 - 1 tiles in all, are refused with the caller's messages.
+struct SubmapTiles {
+  std::vector<size_t> ids;
+  std::vector<unsigned> first_tile;
+  unsigned long long tiles = 0;
+};
+int submap_tiles(b200sm_t s, size_t first, size_t tile, bool skip_empty, const char* too_big, const char* too_many, SubmapTiles* t) {
+  for (size_t i = first; i < s->submaps.size(); i++) {
+    const size_t n = s->submaps[i]->n;
+    if (n == 0 && skip_empty) continue;
+    if (n > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, too_big);
+    t->ids.push_back(i);
+    t->first_tile.push_back((unsigned)t->tiles);
+    t->tiles += (n + tile - 1) / tile;
+  }
+  if (t->tiles > 0x7fffffffull) return sm_fail(s, B200REG_ERR_ARG, too_many);
+  return B200REG_OK;
+}
+
+// the float pose of submap k, 3x4 row-major: the caller's column-major one (poses_colmajor16 + 16 k) if given, else the
+// session's, cast to float (affine.matrix().cast<float>())
+void submap_pose_f(b200sm_t s, size_t k, const double* poses_colmajor16, float* T) {
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 4; c++)
+      T[r * 4 + c] = poses_colmajor16 ? (float)poses_colmajor16[16 * k + c * 4 + r] : (float)s->submaps[k]->pose[r * 4 + c];
+}
+
 // publishMap (sm.cpp:529-552) / modified_map (gbs.cpp:321-368): every submap through its pose cast to float, concatenated in
 // submap order, in one launch into s->assembled (total = map_points(s) > 0). Enqueue only.
 int assemble_on_device(b200sm_t s, const double* poses_colmajor16, size_t total) {
   const int n_sub = (int)s->submaps.size();
+  SubmapTiles t;
+  const int rc = submap_tiles(s, 0, ASSEMBLE_TILE, false, "assemble_map: a submap of 2^32 points or more",
+                              "assemble_map: map too large for one launch", &t);
+  if (rc != B200REG_OK) return rc;
   std::vector<AssembleEntry> table(n_sub);
-  unsigned long long tiles = 0;
   for (int i = 0; i < n_sub; i++) {
     const Submap& sub = *s->submaps[i];
     AssembleEntry& e = table[i];
     e.cloud = sub.cloud;
     e.out_offset = i ? table[i - 1].out_offset + table[i - 1].n : 0;
-    if (sub.n > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "assemble_map: a submap of 2^32 points or more");
     e.n = (unsigned)sub.n;
-    e.first_tile = (unsigned)tiles;
-    tiles += (sub.n + ASSEMBLE_TILE - 1) / ASSEMBLE_TILE;
-    for (int r = 0; r < 3; r++)
-      for (int c = 0; c < 4; c++)
-        e.T.m[r * 4 + c] = poses_colmajor16 ? (float)poses_colmajor16[16 * (size_t)i + c * 4 + r] : (float)sub.pose[r * 4 + c];
+    e.first_tile = t.first_tile[i];
+    submap_pose_f(s, i, poses_colmajor16, e.T.m);
   }
-  if (tiles > 0x7fffffffull) return sm_fail(s, B200REG_ERR_ARG, "assemble_map: map too large for one launch");
   s->assemble_table.ensure(n_sub);
   s->assembled.ensure(total);
   B200_CUDA(cudaMemcpyAsync(s->assemble_table.ptr, table.data(), n_sub * sizeof(AssembleEntry), cudaMemcpyHostToDevice, s->stream));
-  assemble_map_kernel<<<(unsigned)tiles, ASSEMBLE_THREADS, 0, s->stream>>>(s->assemble_table.ptr, n_sub, s->assembled.ptr);
+  assemble_map_kernel<<<(unsigned)t.tiles, ASSEMBLE_THREADS, 0, s->stream>>>(s->assemble_table.ptr, n_sub, s->assembled.ptr);
   B200_CUDA(cudaGetLastError());
   s->launches += 1;
   return (int)B200REG_OK;
@@ -1078,10 +1121,53 @@ int b200sm_assemble_map(b200sm_t s, const double* poses_colmajor16, float* out_x
 
 namespace {
 
-// pcl::io::savePCDFileASCII of the device cloud pts[0 .. total) (total > 0): formatted on the device, its text copied out
-// chunk by chunk into two pinned buffers in turn. Chunk c + 1 is encoded and copied (one stream: encode, copy, encode,
-// ...) while this thread writes chunk c; a buffer is refilled only after its previous chunk has been written. `what`
-// prefixes the error messages.
+// One whole file: `head`, then body_bytes bytes of `body`. nullptr once it is written and closed, else what failed
+// ("cannot open " or "writing "), with errno as the failing call left it.
+const char* write_file(const std::string& path, const std::string& head, const void* body = nullptr, size_t body_bytes = 0) {
+  FILE* fp = std::fopen(path.c_str(), "wb");
+  if (!fp) return "cannot open ";
+  bool ok = std::fwrite(head.data(), 1, head.size(), fp) == head.size() && (body_bytes == 0 || std::fwrite(body, 1, body_bytes, fp) == body_bytes);
+  ok = (std::fclose(fp) == 0) && ok;
+  return ok ? nullptr : "writing ";
+}
+
+// Pieces [0, n) (n > 0) of device data written to files through the session's two pinned staging buffers in turn
+// (`most` bytes each): piece p + 1 is copied while this thread writes piece p, and a buffer is refilled only after its
+// previous piece has been written. enqueue(p, buf) puts piece p into `buf` on the session's stream; write(p, buf) writes
+// it once it has arrived and returns B200REG_OK or an error code. On every return no copy into the staging buffers is
+// left in flight and `fp`, the file the callbacks write, is closed.
+template <typename Enqueue, typename Write>
+int write_staged(b200sm_t s, size_t n, size_t most, FILE*& fp, Enqueue&& enqueue, Write&& write) {
+  cudaEvent_t copied[2] = {nullptr, nullptr};
+  struct Cleanup {
+    cudaEvent_t* ev;
+    FILE** fp;
+    cudaStream_t st;
+    ~Cleanup() {
+      cudaStreamSynchronize(st);
+      for (int b = 0; b < 2; b++)
+        if (ev[b]) cudaEventDestroy(ev[b]);
+      if (*fp) std::fclose(*fp);
+    }
+  } cleanup{copied, &fp, s->stream};
+  for (auto& st : s->pcd_staging) st.ensure(most);
+  for (cudaEvent_t& e : copied) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  auto put = [&](size_t p) {
+    enqueue(p, s->pcd_staging[p & 1].ptr);
+    B200_CUDA(cudaEventRecord(copied[p & 1], s->stream));
+  };
+  put(0);
+  for (size_t p = 0; p < n; p++) {
+    if (p + 1 < n) put(p + 1);  // its buffer held piece p - 1, already written
+    B200_CUDA(cudaEventSynchronize(copied[p & 1]));
+    const int rc = write(p, s->pcd_staging[p & 1].ptr);
+    if (rc != B200REG_OK) return rc;
+  }
+  return (int)B200REG_OK;
+}
+
+// pcl::io::savePCDFileASCII of the device cloud pts[0 .. total) (total > 0): formatted on the device chunk by chunk
+// (one stream: encode, copy, encode, ...) and written by write_staged. `what` prefixes the error messages.
 int write_pcd_ascii(b200sm_t s, const float4* pts, size_t total, const char* path, const char* what, size_t* n_points, size_t* n_bytes) {
   PcdEncoder& E = s->pcd;
   const int launches_before = E.launches;
@@ -1095,48 +1181,29 @@ int write_pcd_ascii(b200sm_t s, const float4* pts, size_t total, const char* pat
   }
   if (n_points) *n_points = total;
   if (n_bytes) *n_bytes = file_bytes;
-  for (auto& st : s->pcd_staging) st.ensure(most);
   FILE* fp = std::fopen(path, "wb");
   if (!fp) {
     s->err = std::string(what) + ": cannot open " + path + ": " + std::strerror(errno);
     return (int)B200REG_ERR_IO;
   }
-  cudaEvent_t copied[2] = {nullptr, nullptr};
-  auto finish = [&](int code) {
-    for (cudaEvent_t& e : copied)
-      if (e) cudaEventDestroy(e);
-    if (std::fclose(fp) != 0 && code == B200REG_OK) {
-      s->err = std::string(what) + ": writing " + path + ": " + std::strerror(errno);
-      return (int)B200REG_ERR_IO;
-    }
-    return code;
+  const size_t chunks = E.chunk_bytes.size();
+  auto enqueue = [&](size_t c, char* buf) {
+    E.encode_chunk(pts, total, c, s->stream);
+    s->launches += 1;
+    B200_CUDA(cudaMemcpyAsync(buf, E.text.ptr, E.chunk_bytes[c], cudaMemcpyDeviceToHost, s->stream));
   };
-  try {
-    for (cudaEvent_t& e : copied) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    const size_t chunks = E.chunk_bytes.size();
-    auto enqueue = [&](size_t c) {
-      E.encode_chunk(pts, total, c, s->stream);
-      s->launches += 1;
-      B200_CUDA(cudaMemcpyAsync(s->pcd_staging[c & 1].ptr, E.text.ptr, E.chunk_bytes[c], cudaMemcpyDeviceToHost, s->stream));
-      B200_CUDA(cudaEventRecord(copied[c & 1], s->stream));
-    };
-    enqueue(0);
-    bool ok = std::fwrite(header.data(), 1, header.size(), fp) == header.size();
-    for (size_t c = 0; c < chunks && ok; c++) {
-      if (c + 1 < chunks) enqueue(c + 1);  // its buffer held chunk c - 1, already written
-      B200_CUDA(cudaEventSynchronize(copied[c & 1]));
-      ok = std::fwrite(s->pcd_staging[c & 1].ptr, 1, E.chunk_bytes[c], fp) == E.chunk_bytes[c];
+  auto write = [&](size_t c, const char* buf) {
+    bool ok = c > 0 || std::fwrite(header.data(), 1, header.size(), fp) == header.size();
+    ok = ok && std::fwrite(buf, 1, E.chunk_bytes[c], fp) == E.chunk_bytes[c];
+    if (ok && c + 1 == chunks) {
+      ok = std::fclose(fp) == 0;
+      fp = nullptr;
     }
-    if (!ok) {
-      s->err = std::string(what) + ": writing " + path + ": " + std::strerror(errno);
-      B200_CUDA(cudaStreamSynchronize(s->stream));  // no copy into the staging buffers is left in flight
-      return finish(B200REG_ERR_IO);
-    }
-  } catch (...) {
-    finish(B200REG_ERR_CUDA);
-    throw;
-  }
-  return finish(B200REG_OK);
+    if (ok) return (int)B200REG_OK;
+    s->err = std::string(what) + ": writing " + path + ": " + std::strerror(errno);
+    return (int)B200REG_ERR_IO;
+  };
+  return write_staged(s, chunks, most, fp, enqueue, write);
 }
 
 }  // namespace
@@ -1232,8 +1299,7 @@ int b200sm_odom_next_scan(b200sm_t s, const double* translation3, const double* 
 
 int b200sm_imu_adjust_distortion(b200sm_t s, float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes,
                                  double scan_time) {
-  if (!s || (!points && n) || stride_bytes < 12 || (stride_bytes % 4) != 0 || (intensity_offset_bytes >= 0 && intensity_offset_bytes % 4 != 0))
-    return B200REG_ERR_ARG;
+  if (!s || (!points && n) || !valid_layout(stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
   return sm_guarded(s, [&]() {
     if (n == 0) return (int)B200REG_OK;
     s->upload.ensure(n);
@@ -1423,9 +1489,7 @@ int b200sm_set_prior_map_pcd(b200sm_t s, const char* path, size_t* n_points) {
 }
 
 int b200sm_set_prior_map(b200sm_t s, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes) {
-  if (!s || !points || n == 0 || stride_bytes < 12 || (stride_bytes % 4) != 0 ||
-      (intensity_offset_bytes >= 0 && (intensity_offset_bytes % 4) != 0))
-    return B200REG_ERR_ARG;
+  if (!s || !points || n == 0 || !valid_layout(stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
   if (n > CUT_MAX_POINTS) return sm_fail(s, B200REG_ERR_ARG, "set_prior_map: more than 2^32 - 1 points");
   return sm_guarded(s, [&]() {
     s->prior_incoming.ensure(n);
@@ -1635,23 +1699,23 @@ int sc_ensure(b200sm_t s) {
     std::swap(norms.cap, s->sc_norms.cap);
     s->sc_cap = cap;
   }
+  // an empty submap owns no tile: its descriptor is all zero
+  SubmapTiles t;
+  const int rc = submap_tiles(s, s->sc_built, SC_BUILD_TILE, true, "scan_context: a submap of 2^32 points or more",
+                              "scan_context: too many points for one launch", &t);
+  if (rc != B200REG_OK) return rc;
   std::vector<ScBuildEntry> table;
-  unsigned long long tiles = 0;
-  for (size_t i = s->sc_built; i < n_sub; i++) {
-    const Submap& sub = *s->submaps[i];
-    if (sub.n == 0) continue;  // an empty submap owns no tile: its descriptor is all zero
-    if (sub.n > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "scan_context: a submap of 2^32 points or more");
-    table.push_back({sub.cloud, (unsigned)sub.n, (unsigned)tiles, (unsigned)i, 0u});
-    tiles += (sub.n + SC_BUILD_TILE - 1) / SC_BUILD_TILE;
+  for (size_t r = 0; r < t.ids.size(); r++) {
+    const Submap& sub = *s->submaps[t.ids[r]];
+    table.push_back({sub.cloud, (unsigned)sub.n, t.first_tile[r], (unsigned)t.ids[r], 0u});
   }
-  if (tiles > 0x7fffffffull) return sm_fail(s, B200REG_ERR_ARG, "scan_context: too many points for one launch");
   const size_t first = s->sc_built, count = n_sub - s->sc_built;
   B200_CUDA(cudaMemsetAsync(s->sc_keys.ptr + first * nb, 0, count * nb * sizeof(uint32_t), s->stream));
   if (!table.empty()) {
     s->sc_build_table.ensure(table.size());
     B200_CUDA(cudaMemcpyAsync(s->sc_build_table.ptr, table.data(), table.size() * sizeof(ScBuildEntry), cudaMemcpyHostToDevice,
                               s->stream));
-    sc_build_launch(s->sc_build_table.ptr, (int)table.size(), (unsigned)tiles, s->sc_keys.ptr, s->sc_tables.ptr, p.num_rings,
+    sc_build_launch(s->sc_build_table.ptr, (int)table.size(), (unsigned)t.tiles, s->sc_keys.ptr, s->sc_tables.ptr, p.num_rings,
                     p.num_sectors, (float)p.lidar_height, s->stream);
     s->launches += 1;
   }
@@ -1834,13 +1898,7 @@ int b200sm_merge_session(b200sm_t dst, b200sm_t src, b200reg_t reg, const b200sm
   if (nA == 0 || nB == 0) return sm_fail(dst, B200REG_ERR_ARG, "merge_session: an empty session");
   if ((unsigned long long)nA * nB > MERGE_MAX_PAIRS) return sm_fail(dst, B200REG_ERR_ARG, "merge_session: more than 2^28 pairs");
   const int n_all = (int)(nA + nB);
-  for (int l = 0; l < n_loop_edges; l++) {
-    const b200sm_loop_edge& e = loop_edges[l];
-    if (e.from < 0 || e.from >= n_all || e.to < 0 || e.to >= n_all || e.from == e.to)
-      return sm_fail(dst, B200REG_ERR_ARG, "merge_session: loop edge with a submap id out of range or from == to");
-    for (int k = 0; k < 16; k++)
-      if (!std::isfinite(e.relative_pose[k])) return sm_fail(dst, B200REG_ERR_ARG, "merge_session: non-finite relative_pose");
-  }
+  if (const int rc = check_loop_edges(dst, loop_edges, n_loop_edges, n_all, "merge_session"); rc != B200REG_OK) return rc;
   return sm_guarded(dst, [&]() {
     *n_rows = 0;
     std::memset(result, 0, sizeof(*result));
@@ -1938,8 +1996,7 @@ int b200sm_merge_session(b200sm_t dst, b200sm_t src, b200reg_t reg, const b200sm
         e.db = B.distance;
         std::memcpy(e.Pa, A.pose, sizeof(e.Pa));
         std::memcpy(e.Pb, B.pose, sizeof(e.Pb));
-        for (int r = 0; r < 4; r++)
-          for (int k = 0; k < 4; k++) e.Z[r * 4 + k] = row.place.loop.relative_pose[k * 4 + r];
+        col_to_row(row.place.loop.relative_pose, e.Z);
         acc.push_back(e);
         acc_row.push_back((int)q);
       }
@@ -1965,19 +2022,14 @@ int b200sm_merge_session(b200sm_t dst, b200sm_t src, b200reg_t reg, const b200sm
     std::vector<int> segs = dst->seg_first;  // dst's segments, then src's (src may itself be a merged map)
     for (int f : src->seg_first) segs.push_back((int)nA + f);
     const int n_loops = n_loop_edges + (int)in.size();
-    std::vector<int> ids(2 * (size_t)n_loops);
-    std::vector<pg::Iso> rel(n_loops);
-    for (int l = 0; l < n_loop_edges; l++) {
-      ids[2 * l] = loop_edges[l].from;
-      ids[2 * l + 1] = loop_edges[l].to;
-      rel[l] = pg::iso_from_colmajor16(loop_edges[l].relative_pose);
-    }
+    std::vector<int> ids;
+    std::vector<pg::Iso> rel;
+    append_loop_edges(loop_edges, n_loop_edges, ids, rel);
     for (size_t k = 0; k < in.size(); k++) {
       const MergeEdge& e = acc[in[k]];
-      const int l = n_loop_edges + (int)k;
-      ids[2 * l] = e.a;
-      ids[2 * l + 1] = (int)nA + e.b;
-      rel[l] = pg::iso_from_rowmajor16(e.Z);
+      ids.push_back(e.a);
+      ids.push_back((int)nA + e.b);
+      rel.push_back(pg::iso_from_rowmajor16(e.Z));
     }
     const std::vector<pg::Edge> edges = pg::build_edges(X, p.num_adjacent_pose_cnstraints, segs, ids.data(), rel.data(), n_loops);
     const pg::LmResult r = pg::optimize(X, edges, p.max_iterations);
@@ -1986,13 +2038,7 @@ int b200sm_merge_session(b200sm_t dst, b200sm_t src, b200reg_t reg, const b200sm
     std::vector<std::unique_ptr<Submap>> added;
     for (size_t b = 0; b < nB; b++) {
       const Submap& B = *src->submaps[b];
-      std::unique_ptr<Submap> sub(new Submap());
-      sub->cloud = dst->arena.alloc(std::max<size_t>(B.n, 1));
-      sub->n = B.n;
-      if (B.n) B200_CUDA(cudaMemcpyAsync(sub->cloud, B.cloud, B.n * sizeof(float4), cudaMemcpyDeviceToDevice, dst->stream));
-      std::memcpy(sub->pose, Xb.data() + 16 * b, sizeof(sub->pose));
-      sub->distance = d_last + B.distance;
-      added.push_back(std::move(sub));
+      added.push_back(new_submap(dst->arena, B.cloud, B.n, Xb.data() + 16 * b, d_last + B.distance, dst->stream));
     }
     B200_CUDA(cudaStreamSynchronize(dst->stream));
     for (auto& sub : added) dst->submaps.push_back(std::move(sub));
@@ -2002,8 +2048,7 @@ int b200sm_merge_session(b200sm_t dst, b200sm_t src, b200reg_t reg, const b200sm
       for (int i = 0; i < n_all; i++) pg::iso_to_colmajor16(X[i], poses_out + 16 * (size_t)i);
     result->merged = 1;
     result->first_submap = (int)nA;
-    for (int rr = 0; rr < 4; rr++)
-      for (int cc = 0; cc < 4; cc++) result->T[cc * 4 + rr] = T[rr * 4 + cc];
+    row_to_col(T, result->T);
     result->adjust.chi2_initial = r.chi2_initial;
     result->adjust.chi2_final = r.chi2_final;
     result->adjust.iterations = r.iterations;
@@ -2053,17 +2098,8 @@ bool sio_make_dir(const std::string& d) {
   return errno == EEXIST && stat(d.c_str(), &st) == 0 && S_ISDIR(st.st_mode);
 }
 
-bool sio_write_text(const std::string& path, const std::string& text) {
-  FILE* fp = std::fopen(path.c_str(), "wb");
-  if (!fp) return false;
-  const bool ok = std::fwrite(text.data(), 1, text.size(), fp) == text.size();
-  return (std::fclose(fp) == 0) && ok;
-}
-
-// Every submap file: the binary PCD header, then the submap's float4 rows as they are on the device. The rows come to the
-// host in pieces of at most SIO_PIECE_BYTES through the two pinned staging buffers in turn, and piece p + 1 is copied
-// while this thread writes piece p (write_pcd_ascii's scheme); a buffer is refilled only after its previous piece has
-// been written. An empty submap is a header alone.
+// Every submap file: the binary PCD header, then the submap's float4 rows as they are on the device, in pieces of at most
+// SIO_PIECE_BYTES through write_staged. An empty submap is a header alone.
 int sio_write_submaps(b200sm_t s, const std::string& sub_dir, unsigned long long* bytes) {
   struct Piece {
     size_t sub, first, count;  // points
@@ -2081,32 +2117,14 @@ int sio_write_submaps(b200sm_t s, const std::string& sub_dir, unsigned long long
       first += c;
     } while (first < n);
   }
-  for (auto& st : s->pcd_staging) st.ensure(most);
-  cudaEvent_t copied[2] = {nullptr, nullptr};
   FILE* fp = nullptr;
-  struct Cleanup {  // on every return: no copy into the staging buffers left in flight, no file left open
-    cudaEvent_t* ev;
-    FILE** fp;
-    cudaStream_t st;
-    ~Cleanup() {
-      cudaStreamSynchronize(st);
-      for (int b = 0; b < 2; b++)
-        if (ev[b]) cudaEventDestroy(ev[b]);
-      if (*fp) std::fclose(*fp);
-    }
-  } cleanup{copied, &fp, s->stream};
-  for (cudaEvent_t& e : copied) B200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  auto enqueue = [&](size_t p) {
+  std::string path;
+  auto enqueue = [&](size_t p, char* buf) {
     const Piece& q = pieces[p];
     if (q.count)
-      B200_CUDA(cudaMemcpyAsync(s->pcd_staging[p & 1].ptr, s->submaps[q.sub]->cloud + q.first, q.count * sizeof(float4),
-                                cudaMemcpyDeviceToHost, s->stream));
-    B200_CUDA(cudaEventRecord(copied[p & 1], s->stream));
+      B200_CUDA(cudaMemcpyAsync(buf, s->submaps[q.sub]->cloud + q.first, q.count * sizeof(float4), cudaMemcpyDeviceToHost, s->stream));
   };
-  enqueue(0);
-  std::string path;
-  for (size_t p = 0; p < pieces.size(); p++) {
-    if (p + 1 < pieces.size()) enqueue(p + 1);  // its buffer held piece p - 1, already written
+  auto write = [&](size_t p, const char* buf) {
     const Piece& q = pieces[p];
     const size_t n = s->submaps[q.sub]->n;
     if (q.first == 0) {
@@ -2118,18 +2136,17 @@ int sio_write_submaps(b200sm_t s, const std::string& sub_dir, unsigned long long
         return sio_io_fail(s, "save_session: writing " + path + ": " + std::strerror(errno));
       *bytes += header.size();
     }
-    B200_CUDA(cudaEventSynchronize(copied[p & 1]));
     const size_t b = q.count * sizeof(float4);
-    if (b && std::fwrite(s->pcd_staging[p & 1].ptr, 1, b, fp) != b)
-      return sio_io_fail(s, "save_session: writing " + path + ": " + std::strerror(errno));
+    if (b && std::fwrite(buf, 1, b, fp) != b) return sio_io_fail(s, "save_session: writing " + path + ": " + std::strerror(errno));
     *bytes += b;
     if (q.first + q.count == n) {
       const int rc = std::fclose(fp);
       fp = nullptr;
       if (rc != 0) return sio_io_fail(s, "save_session: writing " + path + ": " + std::strerror(errno));
     }
-  }
-  return (int)B200REG_OK;
+    return (int)B200REG_OK;
+  };
+  return write_staged(s, pieces.size(), most, fp, enqueue, write);
 }
 
 bool sio_session_empty(b200sm_t s) { return s->submaps.empty() && !s->d_scan && !s->initial_cloud_received && !s->loaded; }
@@ -2145,16 +2162,8 @@ int b200sm_save_session(b200sm_t s, const char* dir, int num_adjacent_pose_cnstr
              : B200REG_ERR_ARG;
   const size_t n = s->submaps.size();
   if (n == 0) return sm_fail(s, B200REG_ERR_ARG, "save_session: the session has no submaps");
-  for (int l = 0; l < n_loop_edges; l++) {
-    const b200sm_loop_edge& e = loop_edges[l];
-    if (e.from < 0 || e.from >= (int)n || e.to < 0 || e.to >= (int)n || e.from == e.to)
-      return sm_fail(s, B200REG_ERR_ARG, "save_session: loop edge with a submap id out of range or from == to");
-    for (int k = 0; k < 16; k++)
-      if (!std::isfinite(e.relative_pose[k])) return sm_fail(s, B200REG_ERR_ARG, "save_session: non-finite relative_pose");
-  }
-  if (adjusted_poses_colmajor16)
-    for (size_t k = 0; k < 16 * n; k++)
-      if (!std::isfinite(adjusted_poses_colmajor16[k])) return sm_fail(s, B200REG_ERR_ARG, "save_session: non-finite adjusted pose");
+  if (const int rc = check_loop_edges(s, loop_edges, n_loop_edges, (int)n, "save_session"); rc != B200REG_OK) return rc;
+  if (!finite_poses(adjusted_poses_colmajor16, n)) return sm_fail(s, B200REG_ERR_ARG, "save_session: non-finite adjusted pose");
   return sm_guarded(s, [&]() {
     sio::Manifest m;
     m.sc = s->sc;
@@ -2166,8 +2175,7 @@ int b200sm_save_session(b200sm_t s, const char* dir, int num_adjacent_pose_cnstr
       const Submap& sub = *s->submaps[i];
       m.points[i] = sub.n;
       m.distance[i] = sub.distance;
-      for (int r = 0; r < 4; r++)
-        for (int c = 0; c < 4; c++) m.pose[16 * i + c * 4 + r] = sub.pose[r * 4 + c];
+      row_to_col(sub.pose, m.pose.data() + 16 * i);
     }
     m.k = num_adjacent_pose_cnstraints;
     m.loops.resize(n_loop_edges);
@@ -2188,9 +2196,9 @@ int b200sm_save_session(b200sm_t s, const char* dir, int num_adjacent_pose_cnstr
     int rc = sio_write_submaps(s, sub_dir, &bytes);
     if (rc != B200REG_OK) return rc;
     const std::string g2o = sio::write_g2o(m), text = sio::write_manifest(m);
-    if (!sio_write_text(d + "/pose_graph.g2o", g2o))
+    if (write_file(d + "/pose_graph.g2o", g2o))
       return sio_io_fail(s, "save_session: writing " + d + "/pose_graph.g2o: " + std::strerror(errno));
-    if (!sio_write_text(tmp, text)) {
+    if (write_file(tmp, text)) {
       const int e = errno;
       std::remove(tmp.c_str());
       return sio_io_fail(s, "save_session: writing " + tmp + ": " + std::strerror(e));
@@ -2256,16 +2264,11 @@ int b200sm_load_session(b200sm_t s, const char* dir, b200sm_session_io_info* inf
                                                std::to_string(m.points[i])).c_str());
       struct stat st;
       if (stat(file.c_str(), &st) == 0) bytes += (unsigned long long)st.st_size;
-      std::unique_ptr<Submap> sub(new Submap());
-      sub->cloud = arena.alloc(std::max<size_t>(got, 1));
-      sub->n = got;
+      double pose[16];
+      col_to_row(m.pose.data() + 16 * i, pose);
       // stream-ordered before the next file's upload into `rows`
-      if (got) B200_CUDA(cudaMemcpyAsync(sub->cloud, rows.ptr, got * sizeof(float4), cudaMemcpyDeviceToDevice, s->stream));
-      for (int r = 0; r < 4; r++)
-        for (int c = 0; c < 4; c++) sub->pose[r * 4 + c] = m.pose[16 * i + c * 4 + r];
-      sub->distance = m.distance[i];
+      subs.push_back(new_submap(arena, rows.ptr, got, pose, m.distance[i], s->stream));
       pts += got;
-      subs.push_back(std::move(sub));
     }
     B200_CUDA(cudaStreamSynchronize(s->stream));
     // (3) what b200sm_import_submap of every submap in order gives, then the segments and the Scan Context parameters
@@ -2345,22 +2348,21 @@ int b200sm_build_occupancy_grid(b200sm_t s, const double* poses_colmajor16, cons
   if (const char* why = og_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_occupancy_grid: ") + why).c_str());
   const size_t n_sub = s->submaps.size();
   if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_occupancy_grid: the session has no submaps");
-  if (poses_colmajor16)
-    for (size_t k = 0; k < 16 * n_sub; k++)
-      if (!std::isfinite(poses_colmajor16[k])) return sm_fail(s, B200REG_ERR_ARG, "build_occupancy_grid: a non-finite pose entry");
-  // every submap's float pose and ray origin, and the entries of the submaps that have points
+  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, "build_occupancy_grid: a non-finite pose entry");
+  // the tiles of the submaps that have points (an empty submap's origin alone widens the grid)
+  SubmapTiles t;
+  const int rc = submap_tiles(s, 0, OG_TILE, true, "build_occupancy_grid: a submap of 2^32 points or more",
+                              "build_occupancy_grid: too many points for one launch", &t);
+  if (rc != B200REG_OK) return rc;
+  const std::vector<size_t>& ids = t.ids;
+  // every submap's float pose and ray origin
   std::vector<OgEntry> all(n_sub);
   std::vector<int> bounds(4 * n_sub);
   for (size_t k = 0; k < n_sub; k++) {
     const Submap& sub = *s->submaps[k];
-    if (sub.n > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_occupancy_grid: a submap of 2^32 points or more");
     OgEntry& e = all[k];
     std::memset(&e, 0, sizeof(e));
-    double P[16];
-    for (int r = 0; r < 4; r++)
-      for (int col = 0; col < 4; col++)
-        P[col * 4 + r] = poses_colmajor16 ? poses_colmajor16[16 * k + col * 4 + r] : sub.pose[r * 4 + col];
-    og_pose_f(P, e.T);
+    submap_pose_f(s, k, poses_colmajor16, e.T);
     long long o[3];
     if (!og_origin(c, p, e.T, o)) {
       s->err = "build_occupancy_grid: the sensor origin of submap " + std::to_string(k) +
@@ -2378,16 +2380,10 @@ int b200sm_build_occupancy_grid(b200sm_t s, const double* poses_colmajor16, cons
   return sm_guarded(s, [&]() {
     // K14a over the submaps with points: one launch, one read-back of the bounds and counts
     std::vector<OgEntry> table;
-    std::vector<size_t> ids;
-    unsigned long long tiles = 0;
-    for (size_t k = 0; k < n_sub; k++) {
-      if (all[k].n == 0) continue;  // an empty submap owns no tile: its origin alone widens the grid
-      all[k].first_tile = (unsigned)tiles;
-      tiles += (all[k].n + OG_TILE - 1) / OG_TILE;
-      table.push_back(all[k]);
-      ids.push_back(k);
+    for (size_t r = 0; r < ids.size(); r++) {
+      table.push_back(all[ids[r]]);
+      table.back().first_tile = t.first_tile[r];
     }
-    if (tiles > 0x7fffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_occupancy_grid: too many points for one launch");
     std::vector<int> tb(4 * table.size());
     for (size_t r = 0; r < ids.size(); r++) std::memcpy(&tb[4 * r], &bounds[4 * ids[r]], 4 * sizeof(int));
     unsigned long long ctr[OG_CTR_COUNT] = {};
@@ -2398,7 +2394,7 @@ int b200sm_build_occupancy_grid(b200sm_t s, const double* poses_colmajor16, cons
       s->og_bounds.ensure(tb.size());
       B200_CUDA(cudaMemcpyAsync(s->og_table.ptr, table.data(), table.size() * sizeof(OgEntry), cudaMemcpyHostToDevice, s->stream));
       B200_CUDA(cudaMemcpyAsync(s->og_bounds.ptr, tb.data(), tb.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
-      og_bounds_launch(s->og_table.ptr, (int)table.size(), (unsigned)tiles, c, s->og_bounds.ptr, s->og_counters.ptr, s->stream);
+      og_bounds_launch(s->og_table.ptr, (int)table.size(), (unsigned)t.tiles, c, s->og_bounds.ptr, s->og_counters.ptr, s->stream);
       s->launches += 1;
       B200_CUDA(cudaMemcpyAsync(tb.data(), s->og_bounds.ptr, tb.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
     }
@@ -2532,18 +2528,12 @@ int b200sm_save_occupancy_map(b200sm_t s, const char* pgm_path, const char* yaml
     const OgParams& p = s->og_params;
     const std::string head = og_pgm_header(s->og_width, s->og_height, p.resolution);
     const std::string yaml = og_yaml(pgm_path, p.resolution, s->og_origin, p.occupied_thresh, p.free_thresh);
-    auto write = [&](const char* path, const std::string& a, const unsigned char* b, size_t nb) {
-      FILE* f = std::fopen(path, "wb");
-      if (!f) {
-        s->err = std::string("save_occupancy_map: cannot open ") + path + ": " + std::strerror(errno);
-        return false;
-      }
-      bool ok = std::fwrite(a.data(), 1, a.size(), f) == a.size() && (nb == 0 || std::fwrite(b, 1, nb, f) == nb);
-      ok = (std::fclose(f) == 0) && ok;
-      if (!ok) s->err = std::string("save_occupancy_map: writing ") + path + ": " + std::strerror(errno);
-      return ok;
+    auto fail = [&](const char* path, const char* why) {
+      s->err = std::string("save_occupancy_map: ") + why + path + ": " + std::strerror(errno);
+      return (int)B200REG_ERR_IO;
     };
-    if (!write(pgm_path, head, image.data(), cells) || !write(yaml_path, yaml, nullptr, 0)) return (int)B200REG_ERR_IO;
+    if (const char* why = write_file(pgm_path, head, image.data(), cells)) return fail(pgm_path, why);
+    if (const char* why = write_file(yaml_path, yaml)) return fail(yaml_path, why);
     return (int)B200REG_OK;
   });
 }
@@ -2583,22 +2573,21 @@ int b200sm_build_static_map(b200sm_t s, const double* poses_colmajor16, const b2
   if (const char* why = sm_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_static_map: ") + why).c_str());
   const size_t n_sub = s->submaps.size();
   if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_static_map: the session has no submaps");
-  if (poses_colmajor16)
-    for (size_t k = 0; k < 16 * n_sub; k++)
-      if (!std::isfinite(poses_colmajor16[k])) return sm_fail(s, B200REG_ERR_ARG, "build_static_map: a non-finite pose entry");
+  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, "build_static_map: a non-finite pose entry");
+  SubmapTiles t;
+  const int rc = submap_tiles(s, 0, SM_TILE, true, "build_static_map: a submap of 2^32 points or more",
+                              "build_static_map: too many points for one launch", &t);
+  if (rc != B200REG_OK) return rc;
+  const std::vector<size_t>& ids = t.ids;
+  const unsigned long long tiles = t.tiles;
   // the entries of the submaps with points (empty ones own no tile), in submap order
   std::vector<SmEntry> table;
-  std::vector<size_t> ids;
-  unsigned long long tiles = 0, total = 0;
+  unsigned long long total = 0;
   for (size_t k = 0; k < n_sub; k++) {
     const Submap& sub = *s->submaps[k];
-    if (sub.n > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_static_map: a submap of 2^32 points or more");
     SmEntry e;
     std::memset(&e, 0, sizeof(e));
-    double P[16];
-    for (int r = 0; r < 4; r++)
-      for (int col = 0; col < 4; col++) P[col * 4 + r] = poses_colmajor16 ? poses_colmajor16[16 * k + col * 4 + r] : sub.pose[r * 4 + col];
-    og_pose_f(P, e.T);
+    submap_pose_f(s, k, poses_colmajor16, e.T);
     if (!sm_origin(c, p, e.T, e.o)) {
       s->err = "build_static_map: the sensor origin of submap " + std::to_string(k) + " lies beyond 2^30 voxels";
       return (int)B200REG_ERR_ARG;
@@ -2607,10 +2596,8 @@ int b200sm_build_static_map(b200sm_t s, const double* poses_colmajor16, const b2
     if (sub.n == 0) continue;
     e.cloud = sub.cloud;
     e.n = (unsigned)sub.n;
-    e.first_tile = (unsigned)tiles;
-    tiles += (sub.n + SM_TILE - 1) / SM_TILE;
+    e.first_tile = t.first_tile[table.size()];
     table.push_back(e);
-    ids.push_back(k);
   }
   if (total > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_static_map: a map of 2^32 points or more");
   const int n_entries = (int)table.size();

@@ -9,18 +9,6 @@
 namespace b200 {
 namespace {
 
-// the entry of tile `tile`: the last one whose first tile (K15c: first tile in the batch) is <= tile
-template <bool kBatch>
-__device__ __forceinline__ int sm_entry_of(const SmEntry* __restrict__ table, int n_entries, unsigned tile) {
-  int lo = 0, hi = n_entries - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if ((kBatch ? table[mid].batch_tile : table[mid].first_tile) <= tile) lo = mid;
-    else hi = mid - 1;
-  }
-  return lo;
-}
-
 // the linear index of voxel (x, y, z) in the box; false outside it (the differences in int64: voxel indices reach 2^30 + 2^14)
 __device__ __forceinline__ bool sm_lin(const SmBox& b, int x, int y, int z, unsigned* lin) {
   const long long wx = (long long)x - b.lo[0], wy = (long long)y - b.lo[1], wz = (long long)z - b.lo[2];
@@ -52,7 +40,7 @@ __device__ __forceinline__ void sm_set(uint32_t* bits, unsigned r, unsigned n_vo
 // then one lane per warp widens the entry's bounds with atomicMin / atomicMax.
 __global__ void __launch_bounds__(SM_THREADS) sm_bounds_kernel(const SmEntry* __restrict__ table, int n_entries, SmConst c,
                                                                int* __restrict__ bounds, unsigned long long* __restrict__ counters) {
-  const int k = sm_entry_of<false>(table, n_entries, blockIdx.x);
+  const int k = entry_of(table, n_entries, blockIdx.x, &SmEntry::first_tile);
   const SmEntry& e = table[k];
   const unsigned base = (blockIdx.x - e.first_tile) * (unsigned)SM_TILE + threadIdx.x;
   int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
@@ -99,7 +87,7 @@ __global__ void __launch_bounds__(SM_THREADS) sm_bounds_kernel(const SmEntry* __
 // K15b. The endpoint voxel of every ray into the rank index.
 __global__ void __launch_bounds__(SM_THREADS) sm_mark_kernel(const SmEntry* __restrict__ table, int n_entries, SmConst c, SmBox box,
                                                              RankWord* __restrict__ index, unsigned long long* __restrict__ counters) {
-  const int k = sm_entry_of<false>(table, n_entries, blockIdx.x);
+  const int k = entry_of(table, n_entries, blockIdx.x, &SmEntry::first_tile);
   const SmEntry& e = table[k];
   const unsigned base = (blockIdx.x - e.first_tile) * (unsigned)SM_TILE + threadIdx.x;
   unsigned tripped = 0;
@@ -128,7 +116,7 @@ __global__ void __launch_bounds__(SM_THREADS) sm_walk_kernel(const SmEntry* __re
                                                              const RankWord* __restrict__ index, unsigned n_voxels,
                                                              unsigned long long words_per, uint32_t* __restrict__ scratch,
                                                              unsigned long long* __restrict__ counters) {
-  const int k = sm_entry_of<true>(table, n_entries, blockIdx.x);
+  const int k = entry_of(table, n_entries, blockIdx.x, &SmEntry::batch_tile);
   const SmEntry& e = table[k];
   uint32_t* hit = scratch + 2ull * (unsigned long long)k * words_per;
   uint32_t* fre = hit + words_per;
@@ -249,7 +237,7 @@ __global__ void __launch_bounds__(SM_THREADS) sm_compact_kernel(const SmEntry* _
                                                                 float4* __restrict__ out, unsigned long long* __restrict__ counters) {
   constexpr int W = SM_THREADS / 32;
   __shared__ unsigned warp_count[SM_PER_THREAD][W];
-  const int k = sm_entry_of<false>(table, n_entries, blockIdx.x);
+  const int k = entry_of(table, n_entries, blockIdx.x, &SmEntry::first_tile);
   const SmEntry& e = table[k];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const unsigned base = (blockIdx.x - e.first_tile) * (unsigned)SM_TILE + threadIdx.x;
