@@ -827,6 +827,71 @@ int b200sm_localize_global(b200sm_t s, b200reg_t reg, const float* points, size_
  * (16 floats, column-major), scores and hits; any pointer may be NULL. The session keeps this grid in host memory (80 bytes per
  * hypothesis, about 1.3 GB at the 2^24 cap) until the next such call or until it is destroyed. */
 int b200sm_get_global_search(b200sm_t s, size_t capacity, size_t* n, float* poses_colmajor16, double* scores, long long* hits);
+/* Relocalisation anywhere in the prior map ("kidnapped robot"): no position is assumed (NDT and GICP handles). The map's
+ * rows in the height band [z_min, z_max] are projected into a 2D occupancy grid of `resolution` cells over the map's whole
+ * extent, with a max-pyramid of num_levels levels (kept in the session until the prior map, resolution, the band or
+ * num_levels changes). The frame's filtered scan (upload, sensor transform, armed de-skew, range filter,
+ * VoxelGrid(vg_size_for_input) + setInputSource, as b200sm_localize_init) is rotated to each of yaw_steps headings about the
+ * current pose's rotation and height, and an exact branch-and-bound search over (heading, cell) counts the scan points
+ * that land in occupied cells (csrc/relocalize.hpp states every definition). The answer is the first top_k tiles (the
+ * 2^(num_levels-1)-cell squares of the grid, over all headings) ranked by their best leaf (score descending, leaf index
+ * ascending) among those scoring >= max(1, ceil(min_score * m)), m the projected scan points. For each row in rank order:
+ * the map is cut around the leaf's cell corner, handed over as target (NDT: the grid check first), align(guess) and
+ * getFitnessScore() (no max range): bitwise setInputTarget(cut) / setInputSource(filtered) / align(guess) /
+ * getFitnessScore(). The row with status OK, converged and fitness < accept_fitness that has the lowest fitness (the lowest
+ * row on a tie) becomes the pose; out->best = that row or -1 (pose unchanged). The cut is then stale, so the next
+ * b200sm_localize_cloud cuts around the pose. rows needs capacity >= top_k.
+ * params NULL: the defaults below. A bad parameter, capacity < top_k, or a limit (W * H > 2^28 cells, the pyramid over 2^32
+ * bytes, yaw_steps * W * H >= 2^40, over 2^32 roots, m >= 2^24 or yaw_steps * m > 2^26, a level's stored nodes over 2^26):
+ * B200REG_ERR_ARG, found before the refinement, with the pose, the cut and the engine's target unchanged. No prior map:
+ * B200REG_ERR_NO_TARGET. m = 0, no projected map row or no tile reaching the threshold: B200REG_OK, no rows, best = -1.
+ * The limits that depend on yaw_steps (leaves, roots) are checked by every call, before its search launches anything.
+ * Memory the session keeps: the pyramid, (W + 2^h - 1) * (H + 2^h - 1) bytes for each level h < num_levels (the margins
+ * grow as 4^h: 6 W H + 57 (W + H) + 1245 bytes at 6 levels, but about 1.4 GB at 16 levels even for a 1 x 1 grid); the
+ * offsets table (8 * yaw_steps * m bytes); 8 bytes per tile on the device (TW * TH tiles, every cell a tile at num_levels
+ * = 1: 2 GB at the 2^28-cell limit); the largest frontier (16 bytes per stored node, its score included) and the roots'
+ * scores (4 bytes per root, kept when there are at most 2^26 roots). A call also holds 8 host bytes per tile, 16 when
+ * num_levels > 1. A node calls this at start-up, or when b200sm_localize_cloud's fitness says it is lost, then
+ * b200sm_localize_cloud frame by frame. */
+typedef struct b200sm_relocalize_params {
+  double resolution;      /* > 0, metres per cell (default 0.25)                                                    */
+  double z_min, z_max;    /* finite, z_min < z_max: the height band of map rows and rotated scan points (0.3, 3.0)   */
+  int yaw_steps;          /* 1..4096 headings 2 pi k / yaw_steps about the current rotation (360)                    */
+  int num_levels;         /* 1..16 pyramid levels; 1 is the exhaustive search (6)                                    */
+  double min_score;       /* [0, 1]: a tile's best must score >= ceil(min_score * m) (0.3)                           */
+  int top_k;              /* 1..64 tiles refined (4)                                                                 */
+  double accept_fitness;  /* > 0: a refined row is adopted only below this fitness (1.0)                             */
+} b200sm_relocalize_params;
+typedef struct b200sm_relocalize_row {
+  int yaw_index, cell_i, cell_j;  /* the tile's best leaf: heading, cell relative to the grid's origin cell          */
+  int score;                      /* its score (projected scan points on occupied cells)                             */
+  float guess[16];                /* R_k and the cell's lower corner at the current z, column-major                  */
+  float final_T[16];              /* align()'s result, column-major                                                   */
+  double fitness;                 /* getFitnessScore()                                                                */
+  double trans_probability;       /* NDT: getTransformationProbability(); GICP: 0                                     */
+  int converged, iterations, status, pad;
+} b200sm_relocalize_row;
+typedef struct b200sm_relocalize_result {
+  long long width, height;        /* W, H cells                                                                       */
+  int origin_cell[2];             /* i0, j0: cell (0, 0) covers [i0, i0 + 1) * resolution x [j0, j0 + 1) * resolution */
+  long long m, t0, t;             /* projected scan points, the score threshold T0, the search's threshold T           */
+  unsigned long long leaves;      /* yaw_steps * W * H                                                                */
+  long long nodes[16];            /* nodes scored per level by the expansion; level num_levels - 1: the roots          */
+  int n_rows, best;
+  int pyramid_builds;             /* pyramids the session has built                                                   */
+  float search_ms;                /* device time of the search's launches (CUDA events around each run of launches
+                                     between two host waits, summed; the waits and the pyramid build excluded)        */
+} b200sm_relocalize_result;
+int b200sm_relocalize(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes,
+                      const b200sm_relocalize_params* params, b200sm_relocalize_row* rows, size_t capacity,
+                      b200sm_relocalize_result* out);
+/* Level `level` of the last pyramid: the byte of cell (i, j), i, j in [1 - 2^level, W) x [1 - 2^level, H), at
+ * (j + 2^level - 1) * width + (i + 2^level - 1); *width = W + 2^level - 1, *height likewise (0 x 0 for an empty grid);
+ * min(capacity, width * height) bytes into out (may be NULL). No pyramid or level outside it: B200REG_ERR_ARG. */
+int b200sm_get_relocalize_grid(b200sm_t s, int level, unsigned char* out, size_t capacity, long long* width, long long* height);
+/* score_level of `count` nodes (heading, i, j triples, any i, j) with the last relocalize search's discretised scan. No
+ * search since the pyramid was built, a heading outside it or a level outside the pyramid: B200REG_ERR_ARG. */
+int b200sm_relocalize_score_nodes(b200sm_t s, int level, long long count, const int* k_i_j, int* scores);
 int b200sm_get_localize_stats(b200sm_t s, b200sm_localize_stats* out);
 /* read-back of the current cut (the newest one, pending or adopted), like b200sm_get_targeted */
 int b200sm_get_cut(b200sm_t s, float* out_xyzi, size_t capacity, size_t* n);

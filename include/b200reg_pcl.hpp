@@ -463,6 +463,18 @@ class ScanMatcherSession {
     hits.resize(n);
     check(b200sm_get_global_search(s_.get(), n, &n, poses.data(), scores.data(), hits.data()));
   }
+  // relocalisation anywhere in the prior map (b200sm_relocalize; params NULL: the defaults): the refined rows in rank order;
+  // returns the adopted row or -1 (pose unchanged)
+  int relocalize(b200reg_t reg, const float* points, size_t n, size_t stride, long intensity_offset, const b200sm_relocalize_params* params,
+                 std::vector<b200sm_relocalize_row>& rows, b200sm_relocalize_result* info = nullptr) {
+    const int top_k = params ? params->top_k : 4;
+    rows.resize(top_k > 0 ? (size_t)top_k : 1);
+    b200sm_relocalize_result r{};
+    check(b200sm_relocalize(s_.get(), reg, points, n, stride, intensity_offset, params, rows.data(), rows.size(), &r));
+    rows.resize((size_t)r.n_rows);
+    if (info) *info = r;
+    return r.best;
+  }
   // ---- place recognition (b200sm_search_loop_place): a loop search by Scan Context that does not trust the drifted poses
   void setScanContextParams(const b200sm_scan_context_params* p) { check(b200sm_set_scan_context_params(s_.get(), p)); }
   // descriptor of submap `index`: num_rings * num_sectors floats, ring-major

@@ -48,6 +48,7 @@ SYMBOLS = [
     "b200sm_set_prior_map_pcd", "b200sm_set_prior_map", "b200sm_set_localization_params", "b200sm_localize_cloud",
     "b200sm_localize_init", "b200sm_get_localize_stats", "b200sm_get_cut", "b200reg_ndt_score_poses",
     "b200sm_localize_global", "b200sm_get_global_search",
+    "b200sm_relocalize", "b200sm_get_relocalize_grid", "b200sm_relocalize_score_nodes",
     "b200sm_set_scan_context_params", "b200sm_get_scan_context", "b200sm_search_loop_place", "b200sm_get_place_scores",
     "b200sm_build_occupancy_grid", "b200sm_get_occupancy_grid", "b200sm_save_occupancy_map",
     "b200sm_build_static_map", "b200sm_get_static_map", "b200sm_get_map_voxels", "b200sm_save_static_map_pcd_ascii",
@@ -156,6 +157,27 @@ class SmGlobalSearch(C.Structure):
 class SmGlobalResult(C.Structure):
     _fields_ = [("n_hypotheses", C.c_longlong), ("hits_total", C.c_longlong), ("n_refined", C.c_int), ("best", C.c_int),
                 ("score_ms", C.c_float)]
+
+
+class SmRelocalizeParams(C.Structure):
+    _fields_ = [("resolution", C.c_double), ("z_min", C.c_double), ("z_max", C.c_double), ("yaw_steps", C.c_int),
+                ("num_levels", C.c_int), ("min_score", C.c_double), ("top_k", C.c_int), ("accept_fitness", C.c_double)]
+
+
+RELOCALIZE_DEFAULTS = dict(resolution=0.25, z_min=0.3, z_max=3.0, yaw_steps=360, num_levels=6, min_score=0.3, top_k=4,
+                           accept_fitness=1.0)
+
+
+class SmRelocalizeRow(C.Structure):
+    _fields_ = [("yaw_index", C.c_int), ("cell_i", C.c_int), ("cell_j", C.c_int), ("score", C.c_int), ("guess", C.c_float * 16),
+                ("final_T", C.c_float * 16), ("fitness", C.c_double), ("trans_probability", C.c_double), ("converged", C.c_int),
+                ("iterations", C.c_int), ("status", C.c_int), ("pad", C.c_int)]
+
+
+class SmRelocalizeResult(C.Structure):
+    _fields_ = [("width", C.c_longlong), ("height", C.c_longlong), ("origin_cell", C.c_int * 2), ("m", C.c_longlong),
+                ("t0", C.c_longlong), ("t", C.c_longlong), ("leaves", C.c_ulonglong), ("nodes", C.c_longlong * 16),
+                ("n_rows", C.c_int), ("best", C.c_int), ("pyramid_builds", C.c_int), ("search_ms", C.c_float)]
 
 
 class SweepResult(C.Structure):
@@ -290,6 +312,10 @@ def lib() -> C.CDLL:
     L.b200reg_ndt_score_poses.argtypes = [vp, i, vp, vp, vp]
     L.b200sm_localize_global.argtypes = [vp, vp, vp, sz, sz, C.c_long, C.POINTER(SmGlobalSearch), vp, vp, C.POINTER(SmGlobalResult)]
     L.b200sm_get_global_search.argtypes = [vp, sz, C.POINTER(sz), vp, vp, vp]
+    L.b200sm_relocalize.argtypes = [vp, vp, vp, sz, sz, C.c_long, C.POINTER(SmRelocalizeParams), C.POINTER(SmRelocalizeRow), sz,
+                                    C.POINTER(SmRelocalizeResult)]
+    L.b200sm_get_relocalize_grid.argtypes = [vp, i, vp, sz, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]
+    L.b200sm_relocalize_score_nodes.argtypes = [vp, i, C.c_longlong, vp, vp]
     L.b200sm_set_scan_context_params.argtypes = [vp, C.POINTER(SmScanContextParams)]
     L.b200sm_get_scan_context.argtypes = [vp, sz, vp, sz]
     L.b200sm_search_loop_place.argtypes = [vp, vp, f, d, d, i, d, i, vp, sz, C.POINTER(sz), C.POINTER(sz)]

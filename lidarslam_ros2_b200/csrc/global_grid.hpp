@@ -52,18 +52,10 @@ inline long long global_grid_count(double radius, double step, int yaw_steps, in
   return p * yaw_steps;
 }
 
-// The hypotheses of a valid spec around the pose (position, quaternion x y z w), 16 floats each, column-major. Hypothesis
-// k = position_index * yaw_steps + m: translation (cx + a, cy + b, z0), rotation Rz(theta_m) * R0 with R0 the rotation of
-// pose_to_matrix_d (the session's sim_trans), theta_m = 2 pi m / yaw_steps, products summed left to right in double, then
-// cast to float.
-inline void global_grid_build(const double* position, const double* quat, double radius, double step, int yaw_steps,
-                              std::vector<float>& poses) {
-  std::vector<int> ij;
-  const long long n_pos = global_grid_positions(radius, step, &ij);
-  poses.assign((size_t)(n_pos < 0 ? 0 : n_pos) * (size_t)yaw_steps * 16, 0.0f);
-  double M[16];
-  pose_to_matrix_d(position, quat, M);
-  std::vector<double> rot((size_t)yaw_steps * 9);
+// The rotations Rz(theta_m) * R0 for m = 0 .. yaw_steps - 1, row-major 3x3 in double: R0 the rotation of the row-major M,
+// theta_m = 2 pi m / yaw_steps, products summed left to right. b200sm_localize_global and b200sm_relocalize share them.
+inline void global_yaw_rotations(const double* M, int yaw_steps, std::vector<double>& rot) {
+  rot.assign((size_t)yaw_steps * 9, 0.0);
   for (int m = 0; m < yaw_steps; m++) {
     const double th = 2.0 * 3.141592653589793 * (double)m / (double)yaw_steps;  // math.pi
     const double c = std::cos(th), s = std::sin(th);
@@ -72,6 +64,20 @@ inline void global_grid_build(const double* position, const double* quat, double
       for (int col = 0; col < 3; col++)
         rot[(size_t)m * 9 + r * 3 + col] = Rz[r * 3 + 0] * M[0 * 4 + col] + Rz[r * 3 + 1] * M[1 * 4 + col] + Rz[r * 3 + 2] * M[2 * 4 + col];
   }
+}
+
+// The hypotheses of a valid spec around the pose (position, quaternion x y z w), 16 floats each, column-major. Hypothesis
+// k = position_index * yaw_steps + m: translation (cx + a, cy + b, z0), rotation global_yaw_rotations' R_m with R0 the
+// rotation of pose_to_matrix_d (the session's sim_trans), cast to float.
+inline void global_grid_build(const double* position, const double* quat, double radius, double step, int yaw_steps,
+                              std::vector<float>& poses) {
+  std::vector<int> ij;
+  const long long n_pos = global_grid_positions(radius, step, &ij);
+  poses.assign((size_t)(n_pos < 0 ? 0 : n_pos) * (size_t)yaw_steps * 16, 0.0f);
+  double M[16];
+  pose_to_matrix_d(position, quat, M);
+  std::vector<double> rot;
+  global_yaw_rotations(M, yaw_steps, rot);
   for (long long q = 0; q < n_pos; q++) {
     const double t[3] = {M[3] + (double)ij[2 * q] * step, M[7] + (double)ij[2 * q + 1] * step, M[11]};
     for (int m = 0; m < yaw_steps; m++) {

@@ -25,6 +25,7 @@
 // The submaps (sensor-frame, voxel-filtered) and the targeted cloud never leave the GPU; read-back entry points exist for
 // the parity tests and for the node's publishers.
 #include <cerrno>
+#include <cfloat>
 #include <climits>
 #include <cmath>
 #include <cstdio>
@@ -43,6 +44,7 @@
 #include "occupancy.cuh"
 #include "place_recognition.cuh"
 #include "pose_graph.hpp"
+#include "relocalize.cuh"
 #include "scan_context.hpp"
 #include "sensor_frame.hpp"
 #include "session_io.hpp"
@@ -317,6 +319,8 @@ struct b200sm_session {
   std::vector<float> global_poses;
   std::vector<double> global_scores;
   std::vector<long long> global_hits;
+  // relocalisation (b200sm_relocalize): the pyramid of the prior map, the last search's offsets and frontier
+  Relocalizer reloc;
   // place recognition (b200sm_search_loop_place): descriptors of submaps [0, sc_built) in slots of sc_keys (keys while being
   // built, then the descriptor's floats) and their column norms; room for sc_cap submaps
   ScParams sc;
@@ -1367,6 +1371,7 @@ int install_prior_map(b200sm_t s, size_t n) {
   std::swap(s->prior_map.cap, s->prior_incoming.cap);
   s->prior_incoming.release();
   s->n_prior = n;
+  s->reloc.invalidate();
   s->cut_stale = true;
   s->cut_pending = false;
   s->n_cuts = 0;
@@ -1632,6 +1637,131 @@ int b200sm_get_global_search(b200sm_t s, size_t capacity, size_t* n, float* pose
   if (scores && m) std::memcpy(scores, s->global_scores.data(), m * sizeof(double));
   if (hits && m) std::memcpy(hits, s->global_hits.data(), m * sizeof(long long));
   return B200REG_OK;
+}
+
+int b200sm_relocalize(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes,
+                      const b200sm_relocalize_params* params, b200sm_relocalize_row* rows, size_t capacity,
+                      b200sm_relocalize_result* out) {
+  if (!valid_frame_args(s, reg, points, n, stride_bytes, intensity_offset_bytes) || !rows) return B200REG_ERR_ARG;
+  RlParams p;
+  if (params) {
+    p.resolution = params->resolution;
+    p.z_min = params->z_min;
+    p.z_max = params->z_max;
+    p.yaw_steps = params->yaw_steps;
+    p.num_levels = params->num_levels;
+    p.min_score = params->min_score;
+    p.top_k = params->top_k;
+    p.accept_fitness = params->accept_fitness;
+  }
+  if (!rl_params_valid(p))
+    return sm_fail(s, B200REG_ERR_ARG, "relocalize: resolution must be finite and > 0, z_min < z_max finite, yaw_steps in 1..4096, "
+                                       "num_levels in 1..16, min_score in [0, 1], top_k in 1..64 and accept_fitness finite and > 0");
+  if (capacity < (size_t)p.top_k) return sm_fail(s, B200REG_ERR_ARG, "relocalize: fewer rows than top_k");
+  int kind = B200REG_NDT;
+  b200reg_get_kind(reg, &kind);
+  return sm_guarded(s, [&]() {
+    b200sm_relocalize_result res;
+    std::memset(&res, 0, sizeof(res));
+    res.best = -1;
+    if (out) *out = res;
+    if (s->n_prior == 0) return sm_fail(s, B200REG_ERR_NO_TARGET, "relocalize: no prior map");
+    upload_frame(s, points, n, stride_bytes, intensity_offset_bytes);
+    int rc = set_source_from_scan(s, reg);
+    if (rc != B200REG_OK) return rc;
+    std::string why;
+    const int before = s->reloc.launches;
+    rc = s->reloc.ensure_pyramid(s->prior_map.ptr, s->n_prior, p, why, s->stream);
+    s->launches += s->reloc.launches - before;
+    if (rc != B200REG_OK) return sm_fail(s, rc, ("relocalize: " + why).c_str());
+    const RlGrid g = s->reloc.grid;
+    std::vector<double> rot_d;
+    std::vector<float> rot_f;
+    rl_rotations(s->position, s->quat, p.yaw_steps, rot_d, rot_f);
+    const double z0 = s->position[2];
+    RlSearchInfo info;
+    const int before_search = s->reloc.launches;
+    rc = s->reloc.search(s->d_filtered, s->n_filtered, rot_f, z0, p, info, why, s->stream);
+    s->launches += s->reloc.launches - before_search;
+    res.width = g.W;
+    res.height = g.H;
+    res.origin_cell[0] = g.i0;
+    res.origin_cell[1] = g.j0;
+    res.m = info.m;
+    res.t0 = info.t0;
+    res.t = info.t;
+    res.leaves = (unsigned long long)p.yaw_steps * (unsigned long long)g.W * (unsigned long long)g.H;
+    for (int h = 0; h < RL_MAX_LEVELS; h++) res.nodes[h] = info.nodes[h];
+    res.pyramid_builds = s->reloc.builds;
+    res.search_ms = info.ms;
+    if (out) *out = res;
+    if (rc != B200REG_OK) return sm_fail(s, rc, ("relocalize: " + why).c_str());
+    // the refinement: each row registered against the cut around its cell, the engine's plain calls
+    const int n_rows = (int)info.tiles.size();
+    for (int r = 0; r < n_rows; r++) {
+      b200sm_relocalize_row& row = rows[r];
+      std::memset(&row, 0, sizeof(row));
+      const long long idx = rl_key_index(info.keys[(size_t)r]);
+      row.yaw_index = (int)(idx / (g.W * g.H));
+      row.cell_i = (int)(idx % g.W);
+      row.cell_j = (int)((idx / g.W) % g.H);
+      row.score = (int)rl_key_score(info.keys[(size_t)r]);
+      rl_guess(rot_d.data() + 9 * (size_t)row.yaw_index, g, p.resolution, z0, row.cell_i, row.cell_j, row.guess);
+      const double cx = (double)((long long)g.i0 + row.cell_i) * p.resolution, cy = (double)((long long)g.j0 + row.cell_j) * p.resolution;
+      row.status = make_cut(s, cx, cy);
+      if (row.status == B200REG_OK && kind == B200REG_NDT) {
+        row.status = b200reg_check_target_grid_device(reg, s->cut.ptr, s->n_cut);
+        if (row.status != B200REG_OK) s->err = std::string("relocalize: ") + b200reg_last_error(reg);
+      }
+      if (row.status == B200REG_OK) {
+        row.status = hand_over_target(s, reg, kind == B200REG_GICP, s->cut.ptr, s->n_cut, "relocalize: the cut is empty after VoxelGrid",
+                                      &s->n_cut_target);
+        if (row.status == B200REG_OK) s->cut_pending = false;
+      }
+      if (row.status == B200REG_OK) row.status = b200reg_adopt_source_device(reg, s->d_filtered, s->n_filtered);
+      if (row.status == B200REG_OK) row.status = b200reg_align(reg, row.guess, row.final_T);
+      if (row.status == B200REG_OK) row.status = b200reg_get_fitness_score(reg, DBL_MAX, &row.fitness);
+      if (row.status != B200REG_OK) {
+        if (row.status == B200REG_ERR_CUDA) return sm_fail(s, row.status, ("relocalize: " + std::string(b200reg_last_error(reg))).c_str());
+        continue;
+      }
+      b200reg_has_converged(reg, &row.converged);
+      b200reg_stats st;
+      if (b200reg_get_stats(reg, &st) == B200REG_OK) row.iterations = st.iterations;
+      if (kind == B200REG_NDT) b200reg_ndt_get_transformation_probability(reg, &row.trans_probability);
+    }
+    if (n_rows > 0) s->cut_stale = true;  // the rows replaced the cut and the target: the next frame cuts around the pose
+    int best = -1;
+    for (int r = 0; r < n_rows; r++)
+      if (rows[r].status == B200REG_OK && rows[r].converged && rows[r].fitness < p.accept_fitness &&
+          (best < 0 || rows[r].fitness < rows[best].fitness))
+        best = r;
+    if (best >= 0) adopt_pose(s, rows[best].final_T);
+    res.n_rows = n_rows;
+    res.best = best;
+    if (out) *out = res;
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_relocalize_grid(b200sm_t s, int level, unsigned char* out, size_t capacity, long long* width, long long* height) {
+  if (!s) return B200REG_ERR_ARG;
+  return sm_guarded(s, [&]() {
+    std::string why;
+    const int rc = s->reloc.read_level(level, out, capacity, width, height, why, s->stream);
+    if (rc != B200REG_OK) return sm_fail(s, rc, why.c_str());
+    return rc;
+  });
+}
+
+int b200sm_relocalize_score_nodes(b200sm_t s, int level, long long count, const int* k_i_j, int* scores) {
+  if (!s) return B200REG_ERR_ARG;
+  return sm_guarded(s, [&]() {
+    std::string why;
+    const int rc = s->reloc.score_nodes(level, count, k_i_j, scores, why, s->stream);
+    if (rc != B200REG_OK) return sm_fail(s, rc, why.c_str());
+    return rc;
+  });
 }
 
 int b200sm_get_localize_stats(b200sm_t s, b200sm_localize_stats* out) {

@@ -162,6 +162,48 @@ class ScanMatcher:
         self._check(self._lib.b200sm_get_global_search(self._h, H, C.byref(n), _ptr(poses), _ptr(scores), _ptr(hits)))
         return poses.reshape(H, 4, 4).transpose(0, 2, 1).copy(), scores, hits
 
+    def relocalize(self, points, **params):
+        """The pose anywhere in the prior map (b200sm_relocalize; NDT or GICP): an exact branch-and-bound (x, y, yaw) search of
+        the filtered scan over the map's 2D projection, the best tiles refined against the map cut around them; the
+        converged row with the lowest fitness under accept_fitness becomes the pose. `params` override
+        _capi.RELOCALIZE_DEFAULTS (resolution, z_min, z_max, yaw_steps, num_levels, min_score, top_k, accept_fitness).
+        Returns (best row or -1, rows (dicts), info dict)."""
+        p = _as_cloud(points)
+        n, w = p.shape
+        kw = dict(_capi.RELOCALIZE_DEFAULTS, **params)
+        spec = _capi.SmRelocalizeParams(float(kw["resolution"]), float(kw["z_min"]), float(kw["z_max"]), int(kw["yaw_steps"]),
+                                        int(kw["num_levels"]), float(kw["min_score"]), int(kw["top_k"]), float(kw["accept_fitness"]))
+        cap = max(int(kw["top_k"]), 1)
+        rows = (_capi.SmRelocalizeRow * cap)()
+        out = _capi.SmRelocalizeResult()
+        self._check(self._lib.b200sm_relocalize(self._h, self.registration._h, _ptr(p), n, 4 * w, 12 if w >= 4 else -1,
+                                                C.byref(spec), rows, cap, C.byref(out)))
+        res = [{"yaw_index": r.yaw_index, "cell": (r.cell_i, r.cell_j), "score": r.score,
+                "guess": np.array(r.guess, dtype=np.float32).reshape(4, 4).T.copy(),
+                "final": np.array(r.final_T, dtype=np.float32).reshape(4, 4).T.copy(), "fitness": float(r.fitness),
+                "trans_probability": float(r.trans_probability), "converged": bool(r.converged), "iterations": int(r.iterations),
+                "status": int(r.status)} for r in rows[:out.n_rows]]
+        info = dict(width=int(out.width), height=int(out.height), origin_cell=(int(out.origin_cell[0]), int(out.origin_cell[1])),
+                    m=int(out.m), t0=int(out.t0), t=int(out.t), leaves=int(out.leaves), nodes=[int(v) for v in out.nodes],
+                    pyramid_builds=int(out.pyramid_builds), search_ms=float(out.search_ms))
+        return int(out.best), res, info
+
+    def relocalizeGrid(self, level: int = 0) -> np.ndarray:
+        """Level `level` of the relocalisation pyramid: (H + 2^level - 1, W + 2^level - 1) uint8, row r / column c holding cell
+        (c - 2^level + 1, r - 2^level + 1) of the grid."""
+        w, h = C.c_longlong(0), C.c_longlong(0)
+        self._check(self._lib.b200sm_get_relocalize_grid(self._h, int(level), None, 0, C.byref(w), C.byref(h)))
+        out = np.zeros((h.value, w.value), dtype=np.uint8)
+        self._check(self._lib.b200sm_get_relocalize_grid(self._h, int(level), _ptr(out), out.size, C.byref(w), C.byref(h)))
+        return out
+
+    def relocalizeScoreNodes(self, level: int, nodes) -> np.ndarray:
+        """score_level of (heading, i, j) nodes with the last relocalize search's discretised scan, int32."""
+        kij = np.ascontiguousarray(np.asarray(nodes, dtype=np.int32).reshape(-1, 3))
+        out = np.zeros(len(kij), dtype=np.int32)
+        self._check(self._lib.b200sm_relocalize_score_nodes(self._h, int(level), len(kij), _ptr(kij), _ptr(out)))
+        return out
+
     def localizeStats(self) -> dict:
         st = _capi.SmLocalizeStats()
         self._check(self._lib.b200sm_get_localize_stats(self._h, C.byref(st)))
