@@ -14,6 +14,10 @@
  *  - 4x4 matrices are 16 floats COLUMN-MAJOR — exactly Eigen::Matrix4f::data().
  *  - clouds are (const float* base, size_t n, size_t stride_bytes) with x,y,z at byte offsets 0,4,8 of every
  *    point: pass pcl::PointCloud<PointXYZI>::points.data() with stride 32 (PointXYZ: 16).
+ *  - a record layout (stride_bytes[, intensity_offset_bytes]) is valid when stride_bytes >= 12 and is a multiple of 4,
+ *    and the intensity offset is either negative (no intensity) or a multiple of 4 with offset + 4 <= stride_bytes (the
+ *    intensity float lies inside the record: PointXYZI's 16, a PointCloud2 intensity field's offset). Any other layout
+ *    is refused with B200REG_ERR_ARG before anything is copied or launched, and the handle or session is unchanged.
  *  - the library copies what it needs to the GPU inside set_input_*; caller memory (host or device) may be freed or
  *    overwritten on return. A device buffer must be complete (its producer stream synchronised) at the call.
  *  - one handle = one CUDA stream + its device buffers; a handle is used from one host thread at a time,
@@ -165,7 +169,9 @@ int b200reg_ndt_set_batch_slots(b200reg_t h, int slots);
 /* ---- pcl::VoxelGrid<PointXYZI>::filter (sm.cpp:266-269,311-314,325-328,444-447; gbs.cpp:225-226) ------ */
 /* Centroid downsample of all fields (x,y,z,intensity). intensity_offset_bytes < 0: no intensity field.
  * out: same point layout as in (stride_bytes), capacity in points; *m = number of output points (ascending
- * leaf index). If the grid would overflow int32 the input is returned unchanged (PCL behaviour). */
+ * leaf index). Each output record gets x, y, z, the intensity (when there is one) and, for strides >= 16 whose bytes
+ * 12-15 are not the intensity, PointXYZ's padding float data[3] = 1; its other bytes are not written.
+ * If the grid would overflow int32 the input records are returned unchanged (PCL behaviour). */
 int b200reg_voxelgrid(int device, const float* in, size_t n, size_t stride_bytes, long intensity_offset_bytes,
                       float leaf, float* out, size_t out_capacity, size_t* m);
 

@@ -611,9 +611,7 @@ int b200reg_get_aligned(b200reg_t h, float* out, size_t stride_bytes) {
 // ---- VoxelGrid ---------------------------------------------------------------------------------------------
 int b200reg_voxelgrid(int device, const float* in, size_t n, size_t stride_bytes, long intensity_offset_bytes, float leaf,
                       float* out, size_t out_capacity, size_t* m) {
-  if (!in || !out || !m || stride_bytes < 12 || (stride_bytes % 4) != 0 || !(leaf > 0) ||
-      (intensity_offset_bytes >= 0 && (intensity_offset_bytes % 4) != 0))
-    return B200REG_ERR_ARG;  // float fields: records and offsets are 4-byte aligned
+  if (!in || !out || !m || !valid_record_layout(stride_bytes, intensity_offset_bytes) || !(leaf > 0)) return B200REG_ERR_ARG;
   static std::mutex mu;
   std::lock_guard<std::mutex> lock(mu);
   try {
@@ -653,14 +651,17 @@ int b200reg_voxelgrid(int device, const float* in, size_t n, size_t stride_bytes
     B200_CUDA(cudaMemcpyAsync(F.staging.ptr, F.out.ptr, mm * sizeof(float4), cudaMemcpyDeviceToHost, s));
     B200_CUDA(cudaStreamSynchronize(s));
     size_t k = std::min(mm, out_capacity);
+    // x, y, z, the intensity, and PointXYZ's padding float data[3] = 1 when bytes 12-15 are not the intensity; every
+    // other byte of the caller's records is left as it was
+    const bool pad = stride_bytes >= 16 && intensity_offset_bytes != 12;
     for (size_t i = 0; i < k; i++) {
       float* f = reinterpret_cast<float*>(ob + i * stride_bytes);
       const float4 v = F.staging.ptr[i];
       f[0] = v.x;
       f[1] = v.y;
       f[2] = v.z;
+      if (pad) f[3] = 1.0f;
       if (intensity_offset_bytes >= 0) *reinterpret_cast<float*>(ob + i * stride_bytes + intensity_offset_bytes) = v.w;
-      if (stride_bytes >= 32 || (stride_bytes >= 16 && intensity_offset_bytes != 12)) f[3] = 1.0f;
     }
     *m = mm;
     return B200REG_OK;

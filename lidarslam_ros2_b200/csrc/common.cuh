@@ -87,6 +87,15 @@ inline void row_to_col(const S* r, D* c) {
     for (int j = 0; j < 4; j++) c[j * 4 + i] = static_cast<D>(r[i * 4 + j]);
 }
 
+// A caller's host records: x, y, z float32 at bytes 0, 4, 8 of every `stride_bytes`-byte record (4-byte fields, so the
+// stride is a multiple of 4), and an intensity float at `intensity_offset_bytes` when that is >= 0. The intensity must lie
+// inside the record: the unpack kernels read, and VoxelGrid's write-back writes, 4 bytes at that offset of every record.
+inline bool valid_record_layout(size_t stride_bytes, long intensity_offset_bytes) {
+  return stride_bytes >= 12 && (stride_bytes % 4) == 0 &&
+         (intensity_offset_bytes < 0 ||
+          ((intensity_offset_bytes % 4) == 0 && (size_t)intensity_offset_bytes + 4 <= stride_bytes));
+}
+
 // ---- small PTX helpers ------------------------------------------------------------------------------
 #ifdef __CUDACC__
 __device__ __forceinline__ unsigned ld_relaxed_gpu(const unsigned* p) {

@@ -155,11 +155,13 @@ void mark_grid_cells(const float4* pts, size_t n, const GridGeom& g, RankWord* t
 
 Bounds decode_bounds(const unsigned* res6) {
   Bounds b;
-  b.any = !(res6[0] == 0xffffffffu && res6[3] == 0u);
   for (int a = 0; a < 3; a++) {
     b.mn[a] = ordered_to_float(res6[a]);
     b.mx[a] = ordered_to_float(res6[3 + a]);
   }
+  // no finite point: either initial value is still there — the upload's {0xffffffff, 0} (both decode to NaN) or
+  // cloud_bounds' inverted {FLT_MAX, -FLT_MAX} — and min <= max fails
+  b.any = b.mn[0] <= b.mx[0];
   return b;
 }
 
@@ -191,11 +193,18 @@ Bounds grid_bounds(const float4* pts, size_t n, const Bounds* known_bounds, Devi
 bool make_grid_geom(const Bounds& b, float leaf, GridGeom& g) {
   g.leaf = leaf;
   g.inv_leaf = 1.0f / leaf;
-  // voxel_grid_covariance_omp_impl.hpp:75-84 — float products, int64 casts
-  long long dx = static_cast<long long>((b.mx[0] - b.mn[0]) * g.inv_leaf) + 1;
-  long long dy = static_cast<long long>((b.mx[1] - b.mn[1]) * g.inv_leaf) + 1;
-  long long dz = static_cast<long long>((b.mx[2] - b.mn[2]) * g.inv_leaf) + 1;
-  if (dx * dy * dz > static_cast<long long>(INT32_MAX)) return false;
+  // voxel_grid_covariance_omp_impl.hpp:75-84 — float products, int64 casts, dx * dy * dz > INT32_MAX refused. A float
+  // product of 2^31 or more (inf for a range near FLT_MAX), or a bound whose leaf index is not an int, already means
+  // overflow: refusing it first keeps the casts defined (the reference's would not be), and dx * dy cannot wrap.
+  constexpr float kIntLimit = 2147483648.0f;
+  long long d[3];
+  for (int a = 0; a < 3; a++) {
+    const float p = (b.mx[a] - b.mn[a]) * g.inv_leaf;
+    if (!(p < kIntLimit) || !(std::fabs(b.mn[a] * g.inv_leaf) < kIntLimit) || !(std::fabs(b.mx[a] * g.inv_leaf) < kIntLimit))
+      return false;
+    d[a] = static_cast<long long>(p) + 1;
+  }
+  if (d[0] * d[1] > static_cast<long long>(INT32_MAX) || d[0] * d[1] * d[2] > static_cast<long long>(INT32_MAX)) return false;
   for (int a = 0; a < 3; a++) {
     g.min_b[a] = static_cast<int>(std::floor(b.mn[a] * g.inv_leaf));
     g.max_b[a] = static_cast<int>(std::floor(b.mx[a] * g.inv_leaf));

@@ -118,8 +118,9 @@ using namespace b200;
 // a host cloud: uploaded once, measured, then each chunk encoded and copied to its place in `out` (up to capacity)
 extern "C" int b200reg_encode_pcd_ascii(int device, const float* base, size_t n, size_t stride_bytes, long intensity_offset_bytes,
                                         char* out, size_t capacity, size_t* n_bytes) {
-  if (!base || n == 0 || !n_bytes || (!out && capacity) || stride_bytes < 12 || (stride_bytes % 4) != 0 ||
-      intensity_offset_bytes < 0 || (intensity_offset_bytes % 4) != 0 || (size_t)intensity_offset_bytes + 4 > stride_bytes)
+  // the file's intensity column is always written, so the records must carry one
+  if (!base || n == 0 || !n_bytes || (!out && capacity) || intensity_offset_bytes < 0 ||
+      !valid_record_layout(stride_bytes, intensity_offset_bytes))
     return B200REG_ERR_ARG;
   struct State {
     cudaStream_t stream = nullptr;

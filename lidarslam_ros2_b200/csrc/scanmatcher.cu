@@ -398,11 +398,6 @@ int sm_fail(b200sm_t s, int code, const char* msg) {
   return code;
 }
 
-// the record layout the uploader reads: x, y, z first, 4-byte fields; no intensity when the offset is negative
-bool valid_layout(size_t stride_bytes, long intensity_offset_bytes) {
-  return stride_bytes >= 12 && (stride_bytes % 4) == 0 && (intensity_offset_bytes < 0 || (intensity_offset_bytes % 4) == 0);
-}
-
 // A session of several segments or loaded from disk is a backend's map: the frontend's calls are refused on it. `what`
 // prefixes the message.
 int refuse_backend_map(b200sm_t s, const char* what) {
@@ -625,7 +620,7 @@ void write_pose(b200sm_t s, double* pose7_out) {
 }
 
 bool valid_frame_args(b200sm_t s, b200reg_t reg, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes) {
-  return s && reg && points && n != 0 && valid_layout(stride_bytes, intensity_offset_bytes);
+  return s && reg && points && n != 0 && valid_record_layout(stride_bytes, intensity_offset_bytes);
 }
 
 int read_back(b200sm_t s, const float4* d, size_t n, float* out, size_t cap, size_t* n_out) {
@@ -987,7 +982,7 @@ int b200sm_search_loop_all(b200sm_t s, b200reg_t reg, float voxel_leaf_size, dou
 // point appends one to the session so that b200sm_search_loop / _all work on device-resident copies there too.
 int b200sm_import_submap(b200sm_t s, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes,
                          const double* pose_colmajor16, double distance) {
-  if (!s || (!points && n) || !pose_colmajor16 || !valid_layout(stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
+  if (!s || (!points && n) || !pose_colmajor16 || !valid_record_layout(stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
   return sm_guarded(s, [&]() {
     double pose[16];
     col_to_row(pose_colmajor16, pose);
@@ -1303,7 +1298,7 @@ int b200sm_odom_next_scan(b200sm_t s, const double* translation3, const double* 
 
 int b200sm_imu_adjust_distortion(b200sm_t s, float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes,
                                  double scan_time) {
-  if (!s || (!points && n) || !valid_layout(stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
+  if (!s || (!points && n) || !valid_record_layout(stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
   return sm_guarded(s, [&]() {
     if (n == 0) return (int)B200REG_OK;
     s->upload.ensure(n);
@@ -1494,7 +1489,7 @@ int b200sm_set_prior_map_pcd(b200sm_t s, const char* path, size_t* n_points) {
 }
 
 int b200sm_set_prior_map(b200sm_t s, const float* points, size_t n, size_t stride_bytes, long intensity_offset_bytes) {
-  if (!s || !points || n == 0 || !valid_layout(stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
+  if (!s || !points || n == 0 || !valid_record_layout(stride_bytes, intensity_offset_bytes)) return B200REG_ERR_ARG;
   if (n > CUT_MAX_POINTS) return sm_fail(s, B200REG_ERR_ARG, "set_prior_map: more than 2^32 - 1 points");
   return sm_guarded(s, [&]() {
     s->prior_incoming.ensure(n);

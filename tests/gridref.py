@@ -35,7 +35,14 @@ def leaf_geometry(points, leaf):
     mn, mx = p.min(axis=0), p.max(axis=0)
     leaf = F32(leaf)
     inv = F32(1.0) / leaf
-    d = [int(F32(mx[a] - mn[a]) * inv) + 1 for a in range(3)]  # float product, truncating int64 cast
+    with np.errstate(over="ignore"):
+        span = [F32(F32(mx[a] - mn[a]) * inv) for a in range(3)]
+        # a float product of 2^31 or more (inf near FLT_MAX), or a bound whose leaf index is not an int, overflows the
+        # grid before any cast
+        if not all(s < 2.0**31 and abs(F32(mn[a] * inv)) < 2.0**31 and abs(F32(mx[a] * inv)) < 2.0**31
+                   for a, s in enumerate(span)):
+            return dict(leaf=leaf, inv_leaf=inv, mn=mn, mx=mx, dxyz=None, overflow=True)
+    d = [int(s) + 1 for s in span]  # float product, truncating int64 cast
     g = dict(leaf=leaf, inv_leaf=inv, mn=mn, mx=mx, dxyz=tuple(d), overflow=d[0] * d[1] * d[2] > INT32_MAX)
     if g["overflow"]:
         return g
