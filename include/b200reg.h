@@ -644,6 +644,61 @@ int b200sm_get_occupancy_grid(b200sm_t s, signed char* data, unsigned* hits, uns
  * nav2's map_saver's as its documentation states it; csrc/occupancy_grid.hpp's text is the contract. No grid built yet:
  * B200REG_ERR_ARG. A file that cannot be opened or written: B200REG_ERR_IO. */
 int b200sm_save_occupancy_map(b200sm_t s, const char* pgm_path, const char* yaml_path);
+/* ---- 2.5D elevation and traversability map, for a navigation stack on non-flat ground ---------------------------------
+ * No counterpart in the reference. The occupancy grid's band is fixed in the map frame, so a ramp rising into it reads as
+ * an obstacle and a drop below it as free; this map follows the ground instead. Every submap's points are the points
+ * b200sm_assemble_map(s, poses_colmajor16, ...) returns, skipped by the occupancy grid's rule (non-finite, or horizontally
+ * beyond max_range from the submap's sensor origin), on the occupancy grid's lattice. Each cell keeps its point count n,
+ * its lowest height lo and its surface height h: the highest point no more than `clearance` above lo (points higher up
+ * are overhangs: canopy, a bridge deck). A cell with n >= min_points is observed. Over the observed cells within
+ * window_cells of an observed cell: step = max h - min h, the least-squares plane's slope and the RMS of the residuals to
+ * it (roughness). The cell is unknown (-1) with fewer than min_cells such cells or collinear ones; lethal (100) when the
+ * step, slope or roughness passes its limit; otherwise round-half-up of 99 * the largest of the three ratios to their
+ * limits. Integer statistics, exact int64 moment sums and a fixed double formula make it bitwise deterministic; the exact
+ * definitions are in csrc/elevation_map.hpp, DESIGN.md section 7b describes the build. NDT and GICP sessions alike; no
+ * registration handle is involved. */
+typedef struct b200sm_elevation_params {
+  double resolution;        /* metres per cell, finite, > 0; default 0.1                                               */
+  double max_range;         /* finite, > 0: points farther (horizontally) from the sensor are skipped; default 100;
+                               max_range / resolution <= 2^14                                                         */
+  double sensor_origin[3];  /* LiDAR position in the robot frame, as for b200sm_build_occupancy_grid; default 0         */
+  double clearance;         /* metres above a cell's lowest point that still count as its surface, >= 0; default 2    */
+  int min_points;           /* points that make a cell observed, >= 1; default 2                                      */
+  int window_cells;         /* window radius r in cells, 1..8; default 3 (a 7 x 7 window)                              */
+  int min_cells;            /* observed cells a window needs, 3..(2r + 1)^2; default 6                                */
+  double max_slope;         /* degrees, in (0, 90); default 20                                                         */
+  double max_step;          /* metres, > 0; default 0.15                                                               */
+  double max_roughness;     /* metres (RMS), > 0; default 0.05                                                         */
+  double occupied_thresh, free_thresh; /* image: value >= rint(100 occupied_thresh) -> 0, <= rint(100 free_thresh) -> 254,
+                               else 205; 0 <= free_thresh < occupied_thresh <= 1; defaults 0.65, 0.25                  */
+} b200sm_elevation_params;
+typedef struct b200sm_elevation_info {
+  unsigned width, height;            /* cells                                                                      */
+  double origin[2], resolution;      /* map-frame corner of cell (0, 0), as map_server's YAML origin               */
+  unsigned long long n_points, n_skipped, n_overhang; /* points used / skipped / above a cell's clearance            */
+  unsigned long long n_observed;     /* cells with n >= min_points                                                  */
+  unsigned long long n_lethal, n_traversable, n_unknown; /* cells of value 100 / 0..99 / -1                         */
+} b200sm_elevation_info;
+/* Build the map from every submap at its own pose (poses_colmajor16 NULL) or at the given 16 * n_submaps doubles. params
+ * NULL: the defaults. A parameter out of range, a non-finite pose entry, a sensor origin beyond 2^30 cells, no submaps,
+ * no non-skipped point or a grid of more than 2^28 cells: B200REG_ERR_ARG, checked before the grid is allocated (the
+ * extent is measured on the device first). A height extent (highest minus lowest non-skipped point) of 2^24 cells or
+ * more: B200REG_ERR_ARG, checked after the statistics pass, before the window pass. After any refusal the previous map
+ * stays. The session keeps the map until the next build or destroy: 34 bytes per cell (n, lo, h, step, tan_slope,
+ * roughness, value, image byte; 9.1 GB at the 2^28-cell cap), and a build holds the new map beside the old one until it
+ * succeeds. info may be NULL. */
+int b200sm_build_elevation_map(b200sm_t s, const double* poses_colmajor16, const b200sm_elevation_params* params,
+                               b200sm_elevation_info* info);
+/* The last map, row-major from cell (0, 0): min(capacity, width * height) cells of each non-NULL array. n: points per
+ * cell; h and lo: surface and lowest height in fixed point (metres * 2^16 / resolution, floor), 0x8080808080808080 and
+ * 0x7f7f7f7f7f7f7f7f in a cell without points; step (metres), tan_slope, roughness (metres): NaN in an unknown cell;
+ * value: -1, 0..99 or 100. No map built yet: B200REG_ERR_ARG. */
+int b200sm_get_elevation_map(b200sm_t s, unsigned* n, long long* h, long long* lo, float* step, float* tan_slope, float* roughness,
+                             signed char* value, size_t capacity);
+/* The map_server pair of the last map, in b200sm_save_occupancy_map's format: 0 where the value is lethal or at least
+ * occupied_thresh, 254 where it is at most free_thresh, 205 elsewhere and where unknown. No map built yet:
+ * B200REG_ERR_ARG. A file that cannot be opened or written: B200REG_ERR_IO. */
+int b200sm_save_traversability_map(b200sm_t s, const char* pgm_path, const char* yaml_path);
 /* ---- static map: the map without what moved while it was recorded ---------------------------------------------------
  * No counterpart in the reference. Every submap's points are rays from its sensor origin through a 3D voxel grid: the
  * endpoint is the point b200sm_assemble_map(s, poses_colmajor16, ...) returns for it, the origin the same float pose

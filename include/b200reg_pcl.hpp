@@ -564,6 +564,29 @@ class ScanMatcherSession {
   void saveOccupancyMap(const std::string& pgm_path, const std::string& yaml_path) {
     check(b200sm_save_occupancy_map(s_.get(), pgm_path.c_str(), yaml_path.c_str()));
   }
+  // ---- elevation / traversability map for non-flat ground (b200sm_build_elevation_map): poses empty = the submaps' own,
+  // else 16 doubles per submap, column-major; p nullptr = the defaults
+  b200sm_elevation_info buildElevationMap(const std::vector<double>& poses_colmajor16 = {}, const b200sm_elevation_params* p = nullptr) {
+    b200sm_elevation_info info{};
+    check(b200sm_build_elevation_map(s_.get(), poses_colmajor16.empty() ? nullptr : poses_colmajor16.data(), p, &info));
+    el_cells_ = (size_t)info.width * info.height;
+    return info;
+  }
+  // the last map, row-major from cell (0, 0): values (-1, 0..99, 100) and, where asked for, surface heights (fixed point),
+  // tangents of the slope, and roughness (metres)
+  void elevationMap(std::vector<signed char>& value, std::vector<long long>* h = nullptr, std::vector<float>* tan_slope = nullptr,
+                    std::vector<float>* roughness = nullptr) {
+    value.resize(el_cells_);
+    if (h) h->resize(el_cells_);
+    if (tan_slope) tan_slope->resize(el_cells_);
+    if (roughness) roughness->resize(el_cells_);
+    check(b200sm_get_elevation_map(s_.get(), nullptr, h ? h->data() : nullptr, nullptr, nullptr, tan_slope ? tan_slope->data() : nullptr,
+                                   roughness ? roughness->data() : nullptr, value.data(), el_cells_));
+  }
+  // nav2 map_server's pgm + yaml of the last map, next to the occupancy grid's
+  void saveTraversabilityMap(const std::string& pgm_path, const std::string& yaml_path) {
+    check(b200sm_save_traversability_map(s_.get(), pgm_path.c_str(), yaml_path.c_str()));
+  }
   // ---- static map (b200sm_build_static_map): the map without what moved while it was recorded; poses empty = the
   // submaps' own, else 16 doubles per submap, column-major (b200sm_pose_adjust's output); p nullptr = the defaults
   b200sm_static_map_info buildStaticMap(const std::vector<double>& poses_colmajor16 = {}, const b200sm_static_map_params* p = nullptr) {
@@ -611,6 +634,7 @@ class ScanMatcherSession {
   }
   std::shared_ptr<b200sm_session> s_;
   size_t og_cells_ = 0;  // cells of the last grid this adapter built
+  size_t el_cells_ = 0;  // cells of the last elevation map this adapter built
   size_t sm_sub_ = 0;    // submaps at the last static-map build of this adapter
 };
 

@@ -51,6 +51,7 @@ SYMBOLS = [
     "b200sm_relocalize", "b200sm_get_relocalize_grid", "b200sm_relocalize_score_nodes",
     "b200sm_set_scan_context_params", "b200sm_get_scan_context", "b200sm_search_loop_place", "b200sm_get_place_scores",
     "b200sm_build_occupancy_grid", "b200sm_get_occupancy_grid", "b200sm_save_occupancy_map",
+    "b200sm_build_elevation_map", "b200sm_get_elevation_map", "b200sm_save_traversability_map",
     "b200sm_build_static_map", "b200sm_get_static_map", "b200sm_get_map_voxels", "b200sm_save_static_map_pcd_ascii",
     "b200sm_merge_session", "b200sm_get_merge_scores", "b200sm_get_segments",
     "b200sm_save_session", "b200sm_load_session", "b200sm_get_session_graph",
@@ -84,6 +85,20 @@ class SmOccupancyInfo(C.Structure):
     _fields_ = [("width", C.c_uint), ("height", C.c_uint), ("origin", C.c_double * 2), ("resolution", C.c_double),
                 ("n_rays", C.c_ulonglong), ("n_skipped", C.c_ulonglong), ("n_batches", C.c_int), ("n_occupied", C.c_ulonglong),
                 ("n_free", C.c_ulonglong), ("n_unknown", C.c_ulonglong)]
+
+
+class SmElevationParams(C.Structure):
+    _fields_ = [("resolution", C.c_double), ("max_range", C.c_double), ("sensor_origin", C.c_double * 3),
+                ("clearance", C.c_double), ("min_points", C.c_int), ("window_cells", C.c_int), ("min_cells", C.c_int),
+                ("max_slope", C.c_double), ("max_step", C.c_double), ("max_roughness", C.c_double),
+                ("occupied_thresh", C.c_double), ("free_thresh", C.c_double)]
+
+
+class SmElevationInfo(C.Structure):
+    _fields_ = [("width", C.c_uint), ("height", C.c_uint), ("origin", C.c_double * 2), ("resolution", C.c_double),
+                ("n_points", C.c_ulonglong), ("n_skipped", C.c_ulonglong), ("n_overhang", C.c_ulonglong),
+                ("n_observed", C.c_ulonglong), ("n_lethal", C.c_ulonglong), ("n_traversable", C.c_ulonglong),
+                ("n_unknown", C.c_ulonglong)]
 
 
 class SmStaticMapParams(C.Structure):
@@ -323,6 +338,9 @@ def lib() -> C.CDLL:
     L.b200sm_build_occupancy_grid.argtypes = [vp, vp, C.POINTER(SmOccupancyParams), C.POINTER(SmOccupancyInfo)]
     L.b200sm_get_occupancy_grid.argtypes = [vp, vp, vp, vp, sz]
     L.b200sm_save_occupancy_map.argtypes = [vp, C.c_char_p, C.c_char_p]
+    L.b200sm_build_elevation_map.argtypes = [vp, vp, C.POINTER(SmElevationParams), C.POINTER(SmElevationInfo)]
+    L.b200sm_get_elevation_map.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, sz]
+    L.b200sm_save_traversability_map.argtypes = [vp, C.c_char_p, C.c_char_p]
     L.b200sm_build_static_map.argtypes = [vp, vp, C.POINTER(SmStaticMapParams), C.POINTER(SmStaticMapInfo)]
     L.b200sm_get_static_map.argtypes = [vp, vp, sz, C.POINTER(sz), vp]
     L.b200sm_get_map_voxels.argtypes = [vp, vp, vp, vp, vp, sz, C.POINTER(sz)]

@@ -17,7 +17,8 @@
 //   doPoseAdjustment: modified_map / modified_map_array                                     :321-368   -> b200sm_assemble_map
 //   doPoseAdjustment: savePCDFileASCII("map.pcd", modified_map)                             :369       -> b200sm_save_map_pcd_ascii
 // The 2D occupancy grid of the map for a navigation stack (b200sm_build_occupancy_grid, csrc/occupancy_grid.hpp) has no
-// counterpart in the reference: nav2's map_server pair is written next to map.pcd.
+// counterpart in the reference: nav2's map_server pair is written next to map.pcd. Nor has the elevation /
+// traversability map for non-flat ground (b200sm_build_elevation_map, csrc/elevation_map.hpp), saved as a second such pair.
 // Removing what moved while the map was recorded (b200sm_build_static_map, csrc/static_map.hpp) has no counterpart in the
 // reference either: the static map is saved as PCD in place of map.pcd.
 // Localising in a saved map has no counterpart in the reference: b200sm_set_prior_map* keep the map on the device and
@@ -38,6 +39,7 @@
 
 #include "../../include/b200reg.h"
 #include "deskew.hpp"
+#include "elevation.cuh"
 #include "engine.hpp"
 #include "global_grid.hpp"
 #include "map_cut.hpp"
@@ -247,6 +249,17 @@ using namespace b200;
 extern "C" int b200reg_adopt_source_device(b200reg_t h, const void* dev, size_t n);  // capi.cu (library-internal)
 extern "C" float b200reg_last_score_ms(b200reg_t h);                                 // capi.cu (library-internal)
 
+// One elevation map (b200sm_build_elevation_map): its layers on the device, its parameters and its info.
+struct ElevationMap {
+  DeviceBuffer<uint32_t> n;
+  DeviceBuffer<long long> lo, top;
+  DeviceBuffer<float> step, tan_slope, roughness;
+  DeviceBuffer<signed char> value;
+  DeviceBuffer<unsigned char> image;
+  ElParams params;
+  b200sm_elevation_info info{};
+};
+
 struct b200sm_session {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -351,6 +364,13 @@ struct b200sm_session {
   OgParams og_params;
   unsigned og_width = 0, og_height = 0;
   double og_origin[2] = {0, 0};
+  // elevation map (b200sm_build_elevation_map): the per-call table, bounds, counters and height extent, and the last map
+  // built, kept until the next build succeeds
+  DeviceBuffer<OgEntry> el_table;
+  DeviceBuffer<int> el_bounds;
+  DeviceBuffer<unsigned long long> el_counters;
+  DeviceBuffer<long long> el_zrange;
+  std::unique_ptr<ElevationMap> el;
   // static map (b200sm_build_static_map): the per-call table, bounds, counters and tile counts, the walks' bitmap scratch,
   // and the last build (rank index over the box, hits, frees and flags per occupied voxel, the static map), kept until
   // the next build
@@ -2461,6 +2481,27 @@ OgParams og_params_from(const b200sm_occupancy_params* p) {
   return q;
 }
 
+// nav2 map_server's pair of a trinary image on the device, W x H, top row first (the occupancy grid and the
+// traversability map alike); `what` prefixes the error message
+int save_map_pair(b200sm_t s, const char* what, const unsigned char* image_dev, unsigned W, unsigned H, double resolution,
+                  const double* origin, double occupied_thresh, double free_thresh, const char* pgm_path, const char* yaml_path) {
+  return sm_guarded(s, [&]() {
+    const size_t cells = (size_t)W * H;
+    std::vector<unsigned char> image(cells);
+    B200_CUDA(cudaMemcpyAsync(image.data(), image_dev, cells, cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    const std::string head = og_pgm_header(W, H, resolution);
+    const std::string yaml = og_yaml(pgm_path, resolution, origin, occupied_thresh, free_thresh);
+    auto fail = [&](const char* path, const char* why) {
+      s->err = std::string(what) + why + path + ": " + std::strerror(errno);
+      return (int)B200REG_ERR_IO;
+    };
+    if (const char* why = write_file(pgm_path, head, image.data(), cells)) return fail(pgm_path, why);
+    if (const char* why = write_file(yaml_path, yaml)) return fail(yaml_path, why);
+    return (int)B200REG_OK;
+  });
+}
+
 }  // namespace
 
 extern "C" {
@@ -2645,22 +2686,183 @@ int b200sm_get_occupancy_grid(b200sm_t s, signed char* data, unsigned* hits, uns
 int b200sm_save_occupancy_map(b200sm_t s, const char* pgm_path, const char* yaml_path) {
   if (!s || !pgm_path || !yaml_path) return B200REG_ERR_ARG;
   if (!s->og_built) return sm_fail(s, B200REG_ERR_ARG, "save_occupancy_map: no grid has been built");
+  const OgParams& p = s->og_params;
+  return save_map_pair(s, "save_occupancy_map: ", s->og_image.ptr, s->og_width, s->og_height, p.resolution, s->og_origin,
+                       p.occupied_thresh, p.free_thresh, pgm_path, yaml_path);
+}
+
+}  // extern "C"
+
+// ---- elevation / traversability map: surface heights under the clearance, slope, step and roughness over a window
+// (csrc/elevation_map.hpp, csrc/elevation.cu) ----
+namespace {
+
+ElParams el_params_from(const b200sm_elevation_params* p) {
+  ElParams q;
+  if (p) {
+    q.resolution = p->resolution;
+    q.max_range = p->max_range;
+    for (int k = 0; k < 3; k++) q.sensor_origin[k] = p->sensor_origin[k];
+    q.clearance = p->clearance;
+    q.min_points = p->min_points;
+    q.window_cells = p->window_cells;
+    q.min_cells = p->min_cells;
+    q.max_slope = p->max_slope;
+    q.max_step = p->max_step;
+    q.max_roughness = p->max_roughness;
+    q.occupied_thresh = p->occupied_thresh;
+    q.free_thresh = p->free_thresh;
+  }
+  return q;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b200sm_build_elevation_map(b200sm_t s, const double* poses_colmajor16, const b200sm_elevation_params* params,
+                               b200sm_elevation_info* info) {
+  if (!s) return B200REG_ERR_ARG;
+  const ElParams p = el_params_from(params);
+  ElConst c;
+  if (const char* why = el_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_elevation_map: ") + why).c_str());
+  const size_t n_sub = s->submaps.size();
+  if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_elevation_map: the session has no submaps");
+  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, "build_elevation_map: a non-finite pose entry");
+  SubmapTiles t;
+  const int rc = submap_tiles(s, 0, OG_TILE, true, "build_elevation_map: a submap of 2^32 points or more",
+                              "build_elevation_map: too many points for one launch", &t);
+  if (rc != B200REG_OK) return rc;
+  // the submaps with points: float pose and horizontal origin (the band is the whole line, so zo plays no part)
+  std::vector<OgEntry> table(t.ids.size());
+  for (size_t r = 0; r < t.ids.size(); r++) {
+    const size_t k = t.ids[r];
+    OgEntry& e = table[r];
+    std::memset(&e, 0, sizeof(e));
+    submap_pose_f(s, k, poses_colmajor16, e.T);
+    if (!el_origin(c, p, e.T, &e.xo, &e.yo)) {
+      s->err = "build_elevation_map: the sensor origin of submap " + std::to_string(k) + " lies beyond 2^30 cells";
+      return (int)B200REG_ERR_ARG;
+    }
+    e.cloud = s->submaps[k]->cloud;
+    e.n = (unsigned)s->submaps[k]->n;
+    e.first_tile = t.first_tile[r];
+  }
+  if (table.empty()) return sm_fail(s, B200REG_ERR_ARG, "build_elevation_map: no submap has points");
   return sm_guarded(s, [&]() {
-    const size_t cells = (size_t)s->og_width * s->og_height;
-    std::vector<unsigned char> image(cells);
-    B200_CUDA(cudaMemcpyAsync(image.data(), s->og_image.ptr, cells, cudaMemcpyDeviceToHost, s->stream));
+    // K14a: the extent of the non-skipped points, bounds starting empty; one read-back
+    std::vector<int> tb(4 * table.size());
+    for (size_t r = 0; r < table.size(); r++) {
+      tb[4 * r] = tb[4 * r + 1] = INT_MAX;
+      tb[4 * r + 2] = tb[4 * r + 3] = INT_MIN;
+    }
+    unsigned long long ctr[EL_CTR_COUNT] = {};
+    s->el_counters.ensure(EL_CTR_COUNT);
+    s->el_table.ensure(table.size());
+    s->el_bounds.ensure(tb.size());
+    B200_CUDA(cudaMemsetAsync(s->el_counters.ptr, 0, EL_CTR_COUNT * sizeof(unsigned long long), s->stream));
+    B200_CUDA(cudaMemcpyAsync(s->el_table.ptr, table.data(), table.size() * sizeof(OgEntry), cudaMemcpyHostToDevice, s->stream));
+    B200_CUDA(cudaMemcpyAsync(s->el_bounds.ptr, tb.data(), tb.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
+    og_bounds_launch(s->el_table.ptr, (int)table.size(), (unsigned)t.tiles, c.og, s->el_bounds.ptr, s->el_counters.ptr, s->stream);
+    B200_CUDA(cudaMemcpyAsync(tb.data(), s->el_bounds.ptr, tb.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaMemcpyAsync(ctr, s->el_counters.ptr, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));
-    const OgParams& p = s->og_params;
-    const std::string head = og_pgm_header(s->og_width, s->og_height, p.resolution);
-    const std::string yaml = og_yaml(pgm_path, p.resolution, s->og_origin, p.occupied_thresh, p.free_thresh);
-    auto fail = [&](const char* path, const char* why) {
-      s->err = std::string("save_occupancy_map: ") + why + path + ": " + std::strerror(errno);
-      return (int)B200REG_ERR_IO;
-    };
-    if (const char* why = write_file(pgm_path, head, image.data(), cells)) return fail(pgm_path, why);
-    if (const char* why = write_file(yaml_path, yaml)) return fail(yaml_path, why);
+    s->launches += 1;
+    if (ctr[EL_CTR_POINTS] == 0) return sm_fail(s, B200REG_ERR_ARG, "build_elevation_map: every point is skipped");
+    int gx0 = INT_MAX, gy0 = INT_MAX, gx1 = INT_MIN, gy1 = INT_MIN;
+    for (size_t r = 0; r < table.size(); r++) {
+      gx0 = std::min(gx0, tb[4 * r]);
+      gy0 = std::min(gy0, tb[4 * r + 1]);
+      gx1 = std::max(gx1, tb[4 * r + 2]);
+      gy1 = std::max(gy1, tb[4 * r + 3]);
+    }
+    const unsigned long long W = (unsigned long long)((long long)gx1 - gx0 + 1), H = (unsigned long long)((long long)gy1 - gy0 + 1);
+    if (W * H > OG_MAX_CELLS) {
+      s->err = "build_elevation_map: a grid of " + std::to_string(W) + " x " + std::to_string(H) + " cells exceeds 2^28 cells";
+      return (int)B200REG_ERR_ARG;
+    }
+    // the new map is built beside the last one, which stays until this build succeeds
+    const size_t cells = (size_t)(W * H);
+    auto m = std::make_unique<ElevationMap>();
+    m->n.ensure(cells);
+    m->lo.ensure(cells);
+    m->top.ensure(cells);
+    m->step.ensure(cells);
+    m->tan_slope.ensure(cells);
+    m->roughness.ensure(cells);
+    m->value.ensure(cells);
+    m->image.ensure(cells);
+    B200_CUDA(cudaMemsetAsync(m->n.ptr, 0, cells * sizeof(uint32_t), s->stream));
+    B200_CUDA(cudaMemsetAsync(m->lo.ptr, 0x7f, cells * sizeof(long long), s->stream));   // EL_LO_EMPTY
+    B200_CUDA(cudaMemsetAsync(m->top.ptr, 0x80, cells * sizeof(long long), s->stream));  // EL_TOP_EMPTY
+    long long zrange[2] = {EL_LO_EMPTY, EL_TOP_EMPTY};
+    s->el_zrange.ensure(2);
+    B200_CUDA(cudaMemcpyAsync(s->el_zrange.ptr, zrange, sizeof(zrange), cudaMemcpyHostToDevice, s->stream));
+    el_lowest_launch(s->el_table.ptr, (int)table.size(), (unsigned)t.tiles, c, gx0, gy0, (unsigned)W, (unsigned)H, m->n.ptr, m->lo.ptr,
+                     s->el_counters.ptr, s->stream);
+    el_top_launch(s->el_table.ptr, (int)table.size(), (unsigned)t.tiles, c, gx0, gy0, (unsigned)W, (unsigned)H, m->lo.ptr, m->top.ptr,
+                  s->el_counters.ptr, s->el_zrange.ptr, s->stream);
+    B200_CUDA(cudaMemcpyAsync(zrange, s->el_zrange.ptr, sizeof(zrange), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    s->launches += 2;
+    if (zrange[1] - zrange[0] >= EL_HEIGHT_EXTENT)
+      return sm_fail(s, B200REG_ERR_ARG, "build_elevation_map: the map's height extent is 2^24 cells or more");
+    el_window_launch(c, (unsigned)W, (unsigned)H, m->n.ptr, m->top.ptr, m->step.ptr, m->tan_slope.ptr, m->roughness.ptr, m->value.ptr,
+                     m->image.ptr, s->el_counters.ptr, s->stream);
+    s->launches += 1;
+    B200_CUDA(cudaMemcpyAsync(ctr, s->el_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    if (ctr[EL_CTR_TRIPPED]) return sm_fail(s, B200REG_ERR_CUDA, "build_elevation_map: a point's cell left the grid");
+    m->params = p;
+    b200sm_elevation_info& in = m->info;
+    in.width = (unsigned)W;
+    in.height = (unsigned)H;
+    in.origin[0] = (double)gx0 * p.resolution;
+    in.origin[1] = (double)gy0 * p.resolution;
+    in.resolution = p.resolution;
+    in.n_points = ctr[EL_CTR_POINTS];
+    in.n_skipped = ctr[EL_CTR_SKIPPED];
+    in.n_overhang = ctr[EL_CTR_OVERHANG];
+    in.n_observed = ctr[EL_CTR_OBSERVED];
+    in.n_lethal = ctr[EL_CTR_LETHAL];
+    in.n_traversable = ctr[EL_CTR_TRAVERSABLE];
+    in.n_unknown = ctr[EL_CTR_UNKNOWN];
+    if (info) *info = in;
+    s->el = std::move(m);
     return (int)B200REG_OK;
   });
+}
+
+int b200sm_get_elevation_map(b200sm_t s, unsigned* n, long long* h, long long* lo, float* step, float* tan_slope, float* roughness,
+                             signed char* value, size_t capacity) {
+  if (!s) return B200REG_ERR_ARG;
+  if (!s->el) return sm_fail(s, B200REG_ERR_ARG, "get_elevation_map: no map has been built");
+  return sm_guarded(s, [&]() {
+    const ElevationMap& m = *s->el;
+    const size_t k = std::min(capacity, (size_t)m.info.width * m.info.height);
+    if (k) {
+      auto get = [&](void* dst, const void* src, size_t bytes) {
+        if (dst) B200_CUDA(cudaMemcpyAsync(dst, src, k * bytes, cudaMemcpyDeviceToHost, s->stream));
+      };
+      get(n, m.n.ptr, sizeof(uint32_t));
+      get(h, m.top.ptr, sizeof(long long));
+      get(lo, m.lo.ptr, sizeof(long long));
+      get(step, m.step.ptr, sizeof(float));
+      get(tan_slope, m.tan_slope.ptr, sizeof(float));
+      get(roughness, m.roughness.ptr, sizeof(float));
+      get(value, m.value.ptr, 1);
+      B200_CUDA(cudaStreamSynchronize(s->stream));
+    }
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_save_traversability_map(b200sm_t s, const char* pgm_path, const char* yaml_path) {
+  if (!s || !pgm_path || !yaml_path) return B200REG_ERR_ARG;
+  if (!s->el) return sm_fail(s, B200REG_ERR_ARG, "save_traversability_map: no map has been built");
+  const ElevationMap& m = *s->el;
+  return save_map_pair(s, "save_traversability_map: ", m.image.ptr, m.info.width, m.info.height, m.params.resolution, m.info.origin,
+                       m.params.occupied_thresh, m.params.free_thresh, pgm_path, yaml_path);
 }
 
 }  // extern "C"

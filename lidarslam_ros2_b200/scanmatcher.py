@@ -533,6 +533,46 @@ class ScanMatcher:
         """nav2 map_server's map.pgm + map.yaml pair of the last grid (trinary)."""
         self._check(self._lib.b200sm_save_occupancy_map(self._h, os.fsencode(pgm_path), os.fsencode(yaml_path)))
 
+    # ---- elevation / traversability map for non-flat ground (b200sm_build_elevation_map, csrc/elevation_map.hpp) ----
+    def buildElevationMap(self, poses=None, resolution: float = 0.1, max_range: float = 100.0, sensor_origin=(0.0, 0.0, 0.0),
+                          clearance: float = 2.0, min_points: int = 2, window_cells: int = 3, min_cells: int = 6,
+                          max_slope: float = 20.0, max_step: float = 0.15, max_roughness: float = 0.05,
+                          occupied_thresh: float = 0.65, free_thresh: float = 0.25) -> dict:
+        """The 2.5D elevation map of every submap at its own pose (poses None) or at `poses` (N, 4, 4), built on the device:
+        per cell the highest point within `clearance` of its lowest one, and over the observed cells within window_cells
+        of it the step, slope (max_slope in degrees) and roughness, classified -1 / 0..99 / 100 (lethal). Returns the
+        build's info as a dict (width, height, origin (x, y), resolution, n_points, n_skipped, n_overhang, n_observed,
+        n_lethal, n_traversable, n_unknown)."""
+        P = None
+        if poses is not None:
+            P = np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(self.numSubmaps(), 4, 4).transpose(0, 2, 1))
+        so = (C.c_double * 3)(*[float(v) for v in sensor_origin])
+        prm = _capi.SmElevationParams(float(resolution), float(max_range), so, float(clearance), int(min_points),
+                                      int(window_cells), int(min_cells), float(max_slope), float(max_step),
+                                      float(max_roughness), float(occupied_thresh), float(free_thresh))
+        info = _capi.SmElevationInfo()
+        self._check(self._lib.b200sm_build_elevation_map(self._h, _ptr(P) if P is not None else None, C.byref(prm),
+                                                         C.byref(info)))
+        self._el = info
+        return _struct_dict(info)
+
+    def elevationMap(self) -> dict:
+        """The last map as (height, width) arrays, row 0 the bottom row: n uint32 (points per cell), h and lo int64 (surface
+        and lowest height in 2^16-per-cell fixed point), step, tan_slope, roughness float32 (metres; NaN where unknown),
+        value int8 (-1, 0..99, 100), and the build's info."""
+        info = getattr(self, "_el", None)
+        W, H = (int(info.width), int(info.height)) if info is not None else (0, 0)
+        out = dict(n=np.empty((H, W), dtype=np.uint32), h=np.empty((H, W), dtype=np.int64), lo=np.empty((H, W), dtype=np.int64),
+                   step=np.empty((H, W), dtype=np.float32), tan_slope=np.empty((H, W), dtype=np.float32),
+                   roughness=np.empty((H, W), dtype=np.float32), value=np.empty((H, W), dtype=np.int8))
+        self._check(self._lib.b200sm_get_elevation_map(self._h, *[_ptr(out[k]) for k in ("n", "h", "lo", "step", "tan_slope",
+                                                                                         "roughness", "value")], W * H))
+        return dict(out, **(_struct_dict(info) if info is not None else {}))
+
+    def saveTraversabilityMap(self, pgm_path, yaml_path):
+        """nav2 map_server's pgm + yaml pair of the last elevation map (trinary: lethal black, traversable white)."""
+        self._check(self._lib.b200sm_save_traversability_map(self._h, os.fsencode(pgm_path), os.fsencode(yaml_path)))
+
     # ---- static map: what moved while the map was recorded removed (b200sm_build_static_map, csrc/static_map.hpp) ----
     def buildStaticMap(self, poses=None, resolution: float = 0.2, max_range: float = 100.0, sensor_origin=(0.0, 0.0, 0.0),
                        ray_fraction: float = 0.85, min_frees: int = 2, dynamic_thresh: float = 0.4) -> dict:
