@@ -755,6 +755,62 @@ int b200sm_get_map_voxels(b200sm_t s, int* ijk3, unsigned* hits, unsigned* frees
  * No build yet, or a static map without points (no file is created): B200REG_ERR_ARG. A file that cannot be opened or
  * written: B200REG_ERR_IO. */
 int b200sm_save_static_map_pcd_ascii(b200sm_t s, const char* path, size_t* n_points, size_t* n_bytes);
+/* ---- map consistency: how crisp the map is, without ground truth ------------------------------------------------------
+ * No counterpart in the reference. The points are those b200sm_assemble_map(s, poses_colmajor16, ...) returns, in map
+ * order; non-finite ones are skipped. Every point whose map index is a multiple of query_stride is a query: its
+ * neighbours are the points within `radius` of it (itself included, 2^16-per-radius fixed point, the radius test exact).
+ * From their covariance Sigma (m^2) come h = 1/2 ln det(2 pi e Sigma), the differential entropy, and plane_var, the
+ * smallest eigenvalue of Sigma. A query is valid with n >= min_neighbors and det Sigma >= (radius / 2^16)^6. MME (Mean
+ * Map Entropy, Razlaw et al. 2015) and MPV (Mean Plane Variance) are their means over the valid queries, per submap and
+ * for the whole map: a crisp map has thin, flat neighbourhoods, and double walls or blur from a bad pose or a wrong loop
+ * edge raise both, so a build before and after b200sm_pose_adjust, or with and without a loop edge, tells which map is
+ * better. Exact integer moment sums, a fixed double formula and integer aggregates make every value bitwise
+ * deterministic; the exact definitions are in csrc/map_consistency.hpp, DESIGN.md section 7b describes the build. The
+ * session's submaps, poses and other products are not changed. NDT and GICP sessions alike. */
+typedef struct b200sm_map_consistency_params {
+  double radius;      /* metres, [0.01, 100]; default 0.5                                                              */
+  int min_neighbors;  /* neighbours (the query included) a valid query needs, >= 4; default 10                          */
+  int query_stride;   /* every query_stride-th point of the map is a query, >= 1; default 1                              */
+} b200sm_map_consistency_params;
+typedef struct b200sm_map_consistency_info {
+  int box_origin[3];                     /* cell (i, j, k) of the box's lower corner; cells are radius on a side      */
+  unsigned box_dims[3];                  /* cells; 0 when no point is finite                                            */
+  unsigned long long n_points, n_skipped; /* the assembled map; its non-finite points                                  */
+  unsigned long long n_cells;            /* occupied cells                                                              */
+  unsigned long long n_queries, n_valid; /* queries; valid ones                                                         */
+  unsigned long long n_neighbors;        /* neighbours over all queries                                                 */
+  unsigned long long n_candidates;       /* points of the 27 cells around each query, summed: the candidates tested    */
+  long long sum_h_q, sum_plane_q;        /* over the valid queries: sum rint(h 2^24), sum rint(plane_var / radius^2 2^30) */
+  double mme, mpv;                       /* Mean Map Entropy (nats), Mean Plane Variance (m^2); NaN without a valid query */
+} b200sm_map_consistency_info;
+typedef struct b200sm_submap_consistency {
+  unsigned long long n_points, n_queries, n_valid, n_neighbors; /* the submap's points; its queries ...                 */
+  long long sum_h_q, sum_plane_q;                               /* as in b200sm_map_consistency_info                    */
+  double mme, mpv;                                              /* its queries' means; NaN without a valid query        */
+} b200sm_submap_consistency;
+/* Build the map's consistency from every submap at its own pose (poses_colmajor16 NULL) or at the given 16 * n_submaps
+ * doubles. params NULL: the defaults. A parameter out of range, a non-finite pose entry, no submaps, a map of 2^31 points
+ * or more, a point whose fixed-point coordinate is 2^46 or more in magnitude (about 2^30 radii), or a box of more than
+ * 2^31 - 1 cells (its dims in the message; at 0.3 m that is about 2 km x 2 km x 50 m): B200REG_ERR_ARG, checked before
+ * anything is sized from the map (the box is measured on the device first, with 72 bytes per submap of tables); the
+ * previous build stays. The session keeps the build until the next one or destroy: 20 bytes per point (n, h, plane_var),
+ * the rank index (8 bytes per 32 box cells), 32 bytes per occupied cell (counts, chunk offsets, the cell list) and 40
+ * bytes per submap; a build also reuses 12 bytes per point of cell-ordered scratch, kept with the session. info may be
+ * NULL. */
+int b200sm_build_map_consistency(b200sm_t s, const double* poses_colmajor16, const b200sm_map_consistency_params* params,
+                                 b200sm_map_consistency_info* info);
+/* The per-point layers of the last build, in map order: min(n_points, capacity) rows of each non-NULL array. n: the
+ * neighbours of a query (0 for other points); h (nats) and plane_var (m^2): NaN (0x7ff8000000000000) for an invalid
+ * query and for every other point. No build yet: B200REG_ERR_ARG. */
+int b200sm_get_map_consistency(b200sm_t s, unsigned* n, double* h, double* plane_var, size_t capacity);
+/* The per-submap rows of the last build: min(n_submaps at the build, capacity) rows. No build yet: B200REG_ERR_ARG. */
+int b200sm_get_submap_consistency(b200sm_t s, b200sm_submap_consistency* rows, size_t capacity);
+/* pcl::io::savePCDFileASCII(path, map) of the assembled map at the build's poses with its intensity replaced by
+ * (float) h, NaN where h is: a heat map of the entropy for a viewer, formatted on the device and written as
+ * b200sm_save_static_map_pcd_ascii writes. n_points, n_bytes (may be NULL) = points and file size. No build yet, a map
+ * without points, or submaps added since the build: B200REG_ERR_ARG. A file that cannot be opened or written:
+ * B200REG_ERR_IO. */
+int b200sm_save_map_consistency_pcd_ascii(b200sm_t s, const char* path, size_t* n_points, size_t* n_bytes);
 /* The same text for a HOST PointXYZI cloud (records as in b200sm_import_submap; intensity_offset_bytes >= 0), formatted
  * on `device`. *n_bytes = size of the whole file content (header and data); min(*n_bytes, capacity) bytes are copied to
  * out, so capacity 0 is a size query. B200REG_ERR_ARG for n == 0, a negative intensity offset, or a stride or offset that

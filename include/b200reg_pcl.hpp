@@ -589,6 +589,14 @@ class ScanMatcherSession {
   }
   // ---- static map (b200sm_build_static_map): the map without what moved while it was recorded; poses empty = the
   // submaps' own, else 16 doubles per submap, column-major (b200sm_pose_adjust's output); p nullptr = the defaults
+  // ---- map consistency (b200sm_build_map_consistency): MME / MPV of the map, per point and per submap; poses empty = the
+  // submaps' own, else 16 doubles per submap, column-major; p nullptr = the defaults
+  b200sm_map_consistency_info buildMapConsistency(const std::vector<double>& poses_colmajor16 = {},
+                                                  const b200sm_map_consistency_params* p = nullptr) {
+    b200sm_map_consistency_info info{};
+    check(b200sm_build_map_consistency(s_.get(), poses_colmajor16.empty() ? nullptr : poses_colmajor16.data(), p, &info));
+    return info;
+  }
   b200sm_static_map_info buildStaticMap(const std::vector<double>& poses_colmajor16 = {}, const b200sm_static_map_params* p = nullptr) {
     b200sm_static_map_info info{};
     check(b200sm_build_static_map(s_.get(), poses_colmajor16.empty() ? nullptr : poses_colmajor16.data(), p, &info));

@@ -53,6 +53,8 @@ SYMBOLS = [
     "b200sm_build_occupancy_grid", "b200sm_get_occupancy_grid", "b200sm_save_occupancy_map",
     "b200sm_build_elevation_map", "b200sm_get_elevation_map", "b200sm_save_traversability_map",
     "b200sm_build_static_map", "b200sm_get_static_map", "b200sm_get_map_voxels", "b200sm_save_static_map_pcd_ascii",
+    "b200sm_build_map_consistency", "b200sm_get_map_consistency", "b200sm_get_submap_consistency",
+    "b200sm_save_map_consistency_pcd_ascii",
     "b200sm_merge_session", "b200sm_get_merge_scores", "b200sm_get_segments",
     "b200sm_save_session", "b200sm_load_session", "b200sm_get_session_graph",
     # include/b200comm.h
@@ -104,6 +106,23 @@ class SmElevationInfo(C.Structure):
 class SmStaticMapParams(C.Structure):
     _fields_ = [("resolution", C.c_double), ("max_range", C.c_double), ("sensor_origin", C.c_double * 3),
                 ("ray_fraction", C.c_double), ("min_frees", C.c_uint), ("dynamic_thresh", C.c_double)]
+
+
+class SmMapConsistencyParams(C.Structure):
+    _fields_ = [("radius", C.c_double), ("min_neighbors", C.c_int), ("query_stride", C.c_int)]
+
+
+class SmMapConsistencyInfo(C.Structure):
+    _fields_ = [("box_origin", C.c_int * 3), ("box_dims", C.c_uint * 3), ("n_points", C.c_ulonglong), ("n_skipped", C.c_ulonglong),
+                ("n_cells", C.c_ulonglong), ("n_queries", C.c_ulonglong), ("n_valid", C.c_ulonglong),
+                ("n_neighbors", C.c_ulonglong), ("n_candidates", C.c_ulonglong), ("sum_h_q", C.c_longlong),
+                ("sum_plane_q", C.c_longlong), ("mme", C.c_double), ("mpv", C.c_double)]
+
+
+class SmSubmapConsistency(C.Structure):
+    _fields_ = [("n_points", C.c_ulonglong), ("n_queries", C.c_ulonglong), ("n_valid", C.c_ulonglong),
+                ("n_neighbors", C.c_ulonglong), ("sum_h_q", C.c_longlong), ("sum_plane_q", C.c_longlong), ("mme", C.c_double),
+                ("mpv", C.c_double)]
 
 
 class SmStaticMapInfo(C.Structure):
@@ -345,6 +364,10 @@ def lib() -> C.CDLL:
     L.b200sm_get_static_map.argtypes = [vp, vp, sz, C.POINTER(sz), vp]
     L.b200sm_get_map_voxels.argtypes = [vp, vp, vp, vp, vp, sz, C.POINTER(sz)]
     L.b200sm_save_static_map_pcd_ascii.argtypes = [vp, C.c_char_p, C.POINTER(sz), C.POINTER(sz)]
+    L.b200sm_build_map_consistency.argtypes = [vp, vp, C.POINTER(SmMapConsistencyParams), C.POINTER(SmMapConsistencyInfo)]
+    L.b200sm_get_map_consistency.argtypes = [vp, vp, vp, vp, sz]
+    L.b200sm_get_submap_consistency.argtypes = [vp, vp, sz]
+    L.b200sm_save_map_consistency_pcd_ascii.argtypes = [vp, C.c_char_p, C.POINTER(sz), C.POINTER(sz)]
     L.b200sm_merge_session.argtypes = [vp, vp, vp, C.POINTER(SmMergeParams), vp, i, vp, sz, C.POINTER(sz), vp,
                                         C.POINTER(SmMergeResult)]
     L.b200sm_get_merge_scores.argtypes = [vp, sz, C.POINTER(sz), C.POINTER(sz), vp, vp]

@@ -20,7 +20,8 @@
 // counterpart in the reference: nav2's map_server pair is written next to map.pcd. Nor has the elevation /
 // traversability map for non-flat ground (b200sm_build_elevation_map, csrc/elevation_map.hpp), saved as a second such pair.
 // Removing what moved while the map was recorded (b200sm_build_static_map, csrc/static_map.hpp) has no counterpart in the
-// reference either: the static map is saved as PCD in place of map.pcd.
+// reference either: the static map is saved as PCD in place of map.pcd. Nor has the map's consistency
+// (b200sm_build_map_consistency, csrc/map_consistency.hpp), a ground-truth-free measure of how crisp the map is.
 // Localising in a saved map has no counterpart in the reference: b200sm_set_prior_map* keep the map on the device and
 // b200sm_localize_cloud registers each frame against a stable cut of it around the pose (csrc/map_cut.hpp).
 // The submaps (sensor-frame, voxel-filtered) and the targeted cloud never leave the GPU; read-back entry points exist for
@@ -38,6 +39,7 @@
 #include <sys/stat.h>
 
 #include "../../include/b200reg.h"
+#include "consistency.cuh"
 #include "deskew.hpp"
 #include "elevation.cuh"
 #include "engine.hpp"
@@ -260,6 +262,21 @@ struct ElevationMap {
   b200sm_elevation_info info{};
 };
 
+// One map-consistency build (b200sm_build_map_consistency): the per-point layers, the cell structures K19c read, the
+// per-submap rows, and what the PCD save needs to assemble the same map again.
+struct MapConsistency {
+  DeviceBuffer<unsigned> n;
+  DeviceBuffer<double> h, plane;
+  DeviceBuffer<RankWord> index;
+  DeviceBuffer<unsigned> start, queries, chunks, qcursor, ocursor, sub_first;
+  DeviceBuffer<int> ijk;
+  DeviceBuffer<unsigned long long> rows;
+  McConst c{};
+  b200sm_map_consistency_info info{};
+  std::vector<b200sm_submap_consistency> sub_rows;
+  std::vector<double> poses;  // the build's poses, 16 column-major doubles per submap
+};
+
 struct b200sm_session {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -389,6 +406,15 @@ struct b200sm_session {
   unsigned long long sm_words = 0;
   b200sm_static_map_info sm_info{};
   std::vector<size_t> sm_offsets;  // n_submaps at the build + 1
+  // map consistency (b200sm_build_map_consistency): the per-call table, bounds and counters, the cell-ordered scratch of
+  // K19b / K19c, the scans' tile sums, and the last build, kept until the next build succeeds
+  DeviceBuffer<McEntry> mc_table;
+  DeviceBuffer<int> mc_bounds;
+  DeviceBuffer<unsigned long long> mc_counters;
+  DeviceBuffer<ushort4> mc_offs;
+  DeviceBuffer<unsigned> mc_idx, mc_tmp;
+  RankIndexScratch mc_scan;
+  std::unique_ptr<MapConsistency> mc;
 };
 
 namespace {
@@ -3112,6 +3138,246 @@ int b200sm_save_static_map_pcd_ascii(b200sm_t s, const char* path, size_t* n_poi
   const size_t total = (size_t)s->sm_info.n_static_points;
   if (total == 0) return sm_fail(s, B200REG_ERR_ARG, "save_static_map_pcd_ascii: the static map has no points");
   return sm_guarded(s, [&]() { return write_pcd_ascii(s, s->sm_static.ptr, total, path, "save_static_map_pcd_ascii", n_points, n_bytes); });
+}
+
+}  // extern "C"
+
+// ---- map consistency: per-point neighbourhood entropy and plane variance (csrc/map_consistency.hpp, csrc/consistency.cu) ----
+namespace {
+
+McParams mc_params_from(const b200sm_map_consistency_params* p) {
+  McParams q;
+  if (p) {
+    q.radius = p->radius;
+    q.min_neighbors = p->min_neighbors;
+    q.query_stride = p->query_stride;
+  }
+  return q;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b200sm_build_map_consistency(b200sm_t s, const double* poses_colmajor16, const b200sm_map_consistency_params* params,
+                                 b200sm_map_consistency_info* info) {
+  if (!s) return B200REG_ERR_ARG;
+  const McParams p = mc_params_from(params);
+  McConst c;
+  if (const char* why = mc_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_map_consistency: ") + why).c_str());
+  const size_t n_sub = s->submaps.size();
+  if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_map_consistency: the session has no submaps");
+  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, "build_map_consistency: a non-finite pose entry");
+  unsigned long long total = 0;
+  for (size_t k = 0; k < n_sub; k++) total += s->submaps[k]->n;
+  if (total > MC_MAX_POINTS) return sm_fail(s, B200REG_ERR_ARG, "build_map_consistency: a map of 2^31 points or more");
+  SubmapTiles t;
+  const int rc = submap_tiles(s, 0, MC_TILE, true, "build_map_consistency: a submap of 2^32 points or more",
+                              "build_map_consistency: too many points for one launch", &t);
+  if (rc != B200REG_OK) return rc;
+  // the entries of the submaps with points, in submap order, and every submap's first map index
+  std::vector<McEntry> table;
+  std::vector<unsigned> sub_first(n_sub);
+  std::vector<double> poses(16 * n_sub);
+  unsigned long long at = 0;
+  for (size_t k = 0; k < n_sub; k++) {
+    const Submap& sub = *s->submaps[k];
+    for (int r = 0; r < 4; r++)
+      for (int col = 0; col < 4; col++)
+        poses[16 * k + col * 4 + r] = poses_colmajor16 ? poses_colmajor16[16 * k + col * 4 + r] : sub.pose[r * 4 + col];
+    sub_first[k] = (unsigned)at;
+    if (sub.n) {
+      McEntry e;
+      std::memset(&e, 0, sizeof(e));
+      e.cloud = sub.cloud;
+      e.n = (unsigned)sub.n;
+      e.first_tile = t.first_tile[table.size()];
+      e.map_offset = (unsigned)at;
+      submap_pose_f(s, k, poses_colmajor16, e.T);
+      table.push_back(e);
+    }
+    at += sub.n;
+  }
+  const int n_entries = (int)table.size();
+  const unsigned tiles = (unsigned)t.tiles;
+  return sm_guarded(s, [&]() {
+    // K19a: one launch, one read-back of the bounds and counts; the refusals it decides come before anything is sized
+    std::vector<int> bounds(6 * table.size());
+    for (size_t r = 0; r < table.size(); r++)
+      for (int a = 0; a < 3; a++) {
+        bounds[6 * r + a] = INT_MAX;
+        bounds[6 * r + 3 + a] = INT_MIN;
+      }
+    unsigned long long ctr[MC_CTR_COUNT] = {};
+    s->mc_counters.ensure(MC_CTR_COUNT);
+    B200_CUDA(cudaMemsetAsync(s->mc_counters.ptr, 0, MC_CTR_COUNT * sizeof(unsigned long long), s->stream));
+    if (n_entries) {
+      s->mc_table.ensure(table.size());
+      s->mc_bounds.ensure(bounds.size());
+      B200_CUDA(cudaMemcpyAsync(s->mc_table.ptr, table.data(), table.size() * sizeof(McEntry), cudaMemcpyHostToDevice, s->stream));
+      B200_CUDA(cudaMemcpyAsync(s->mc_bounds.ptr, bounds.data(), bounds.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
+      mc_bounds_launch(s->mc_table.ptr, n_entries, tiles, c, s->mc_bounds.ptr, s->mc_counters.ptr, s->stream);
+      s->launches += 1;
+      B200_CUDA(cudaMemcpyAsync(bounds.data(), s->mc_bounds.ptr, bounds.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+    }
+    B200_CUDA(cudaMemcpyAsync(ctr, s->mc_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    if (ctr[MC_CTR_RANGE])
+      return sm_fail(s, B200REG_ERR_ARG, "build_map_consistency: a point's fixed-point coordinate is 2^46 or more in magnitude");
+    const unsigned long long used = total - ctr[MC_CTR_SKIPPED];
+    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
+    for (size_t r = 0; r < table.size(); r++)
+      for (int a = 0; a < 3; a++) {
+        lo[a] = std::min(lo[a], bounds[6 * r + a]);
+        hi[a] = std::max(hi[a], bounds[6 * r + 3 + a]);
+      }
+    SmBox box{};
+    unsigned long long cells = 0;
+    if (used && !sm_box(lo, hi, box.dims, &cells)) {
+      s->err = "build_map_consistency: a box of " + std::to_string((long long)hi[0] - lo[0] + 1) + " x " +
+               std::to_string((long long)hi[1] - lo[1] + 1) + " x " + std::to_string((long long)hi[2] - lo[2] + 1) +
+               " cells exceeds 2^31 - 1 cells";
+      return (int)B200REG_ERR_ARG;
+    }
+    if (used)
+      for (int a = 0; a < 3; a++) box.lo[a] = lo[a];
+    // the new build is made beside the last one, which stays until this one succeeds
+    auto m = std::make_unique<MapConsistency>();
+    m->c = c;
+    m->poses = std::move(poses);
+    const size_t np = std::max<size_t>((size_t)total, 1);
+    m->n.ensure(np);
+    m->h.ensure(np);
+    m->plane.ensure(np);
+    m->rows.ensure(MC_ROW_COUNT * n_sub);
+    m->sub_first.ensure(n_sub);
+    B200_CUDA(cudaMemsetAsync(m->rows.ptr, 0, MC_ROW_COUNT * n_sub * sizeof(unsigned long long), s->stream));
+    B200_CUDA(cudaMemcpyAsync(m->sub_first.ptr, sub_first.data(), n_sub * sizeof(unsigned), cudaMemcpyHostToDevice, s->stream));
+    const unsigned long long n_words = (cells + 31) / 32;
+    unsigned n_cells = 0, n_chunks = 0;
+    if (used) {
+      // K19b: the occupied cells' rank index, their counts, the chunks of K19c, and the points in cell order
+      m->index.ensure((size_t)n_words);
+      rank_index_clear(m->index.ptr, (int)n_words, s->stream);
+      mc_mark_launch(s->mc_table.ptr, n_entries, tiles, c, box, m->index.ptr, s->mc_counters.ptr, s->stream);
+      s->mc_scan.total.ensure(1);
+      rank_index_scan_async(m->index.ptr, (size_t)n_words, s->mc_scan, s->mc_scan.total.ptr, s->stream);
+      s->launches += 3;
+      B200_CUDA(cudaMemcpyAsync(&n_cells, s->mc_scan.total.ptr, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaStreamSynchronize(s->stream));
+      const size_t nc = (size_t)n_cells + 1;
+      m->start.ensure(nc);
+      m->queries.ensure(nc);
+      m->chunks.ensure(nc);
+      m->qcursor.ensure(nc);
+      m->ocursor.ensure(nc);
+      m->ijk.ensure(3 * nc);
+      B200_CUDA(cudaMemsetAsync(m->start.ptr, 0, nc * sizeof(unsigned), s->stream));
+      B200_CUDA(cudaMemsetAsync(m->queries.ptr, 0, nc * sizeof(unsigned), s->stream));
+      B200_CUDA(cudaMemsetAsync(m->qcursor.ptr, 0, nc * sizeof(unsigned), s->stream));
+      B200_CUDA(cudaMemsetAsync(m->ocursor.ptr, 0, nc * sizeof(unsigned), s->stream));
+      mc_count_launch(s->mc_table.ptr, n_entries, tiles, c, box, m->index.ptr, m->start.ptr, m->queries.ptr, s->stream);
+      counter_scan_async(m->start.ptr, n_cells, s->mc_tmp, s->stream);
+      mc_chunks_launch(m->queries.ptr, n_cells, m->chunks.ptr, s->stream);
+      counter_scan_async(m->chunks.ptr, n_cells, s->mc_tmp, s->stream);
+      sm_voxel_list_launch(m->index.ptr, n_words, box, n_cells, m->ijk.ptr, s->stream);
+      s->launches += 9;
+      B200_CUDA(cudaMemcpyAsync(&n_chunks, m->chunks.ptr + n_cells, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      s->mc_offs.ensure((size_t)used);
+      s->mc_idx.ensure((size_t)used);
+    }
+    // the scatter also resets every point's layers, skipped ones included
+    mc_scatter_launch(s->mc_table.ptr, n_entries, tiles, c, box, m->index.ptr, m->start.ptr, m->queries.ptr, m->qcursor.ptr,
+                      m->ocursor.ptr, s->mc_offs.ptr, s->mc_idx.ptr, m->n.ptr, m->h.ptr, m->plane.ptr, s->mc_counters.ptr, s->stream);
+    s->launches += tiles ? 1 : 0;
+    B200_CUDA(cudaStreamSynchronize(s->stream));  // n_chunks
+    // K19c + K19d
+    mc_neighbour_launch(m->chunks.ptr, n_chunks, n_cells, m->start.ptr, m->queries.ptr, m->ijk.ptr, box, m->index.ptr, s->mc_offs.ptr,
+                        s->mc_idx.ptr, m->sub_first.ptr, (int)n_sub, c, m->n.ptr, m->h.ptr, m->plane.ptr, m->rows.ptr,
+                        s->mc_counters.ptr, s->stream);
+    s->launches += n_chunks ? 1 : 0;
+    std::vector<unsigned long long> rows(MC_ROW_COUNT * n_sub);
+    B200_CUDA(cudaMemcpyAsync(rows.data(), m->rows.ptr, rows.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaMemcpyAsync(ctr, s->mc_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    if (ctr[MC_CTR_TRIPPED]) return sm_fail(s, B200REG_ERR_CUDA, "build_map_consistency: a cell outside the box or a slot beyond its cell");
+    b200sm_map_consistency_info& I = m->info;
+    for (int a = 0; a < 3; a++) {
+      I.box_origin[a] = box.lo[a];
+      I.box_dims[a] = box.dims[a];
+    }
+    I.n_points = total;
+    I.n_skipped = ctr[MC_CTR_SKIPPED];
+    I.n_cells = n_cells;
+    I.n_candidates = ctr[MC_CTR_CANDIDATES];
+    m->sub_rows.resize(n_sub);
+    for (size_t k = 0; k < n_sub; k++) {
+      const unsigned long long* row = &rows[MC_ROW_COUNT * k];
+      b200sm_submap_consistency& R = m->sub_rows[k];
+      R.n_points = s->submaps[k]->n;
+      R.n_queries = row[MC_ROW_QUERIES];
+      R.n_valid = row[MC_ROW_VALID];
+      R.n_neighbors = row[MC_ROW_NEIGHBORS];
+      R.sum_h_q = (long long)row[MC_ROW_SUM_H];
+      R.sum_plane_q = (long long)row[MC_ROW_SUM_PLANE];
+      R.mme = mc_mme(R.sum_h_q, R.n_valid);
+      R.mpv = mc_mpv(c, R.sum_plane_q, R.n_valid);
+      I.n_queries += R.n_queries;
+      I.n_valid += R.n_valid;
+      I.n_neighbors += R.n_neighbors;
+      I.sum_h_q += R.sum_h_q;
+      I.sum_plane_q += R.sum_plane_q;
+    }
+    I.mme = mc_mme(I.sum_h_q, I.n_valid);
+    I.mpv = mc_mpv(c, I.sum_plane_q, I.n_valid);
+    if (info) *info = I;
+    s->mc = std::move(m);
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_map_consistency(b200sm_t s, unsigned* n, double* h, double* plane_var, size_t capacity) {
+  if (!s) return B200REG_ERR_ARG;
+  if (!s->mc) return sm_fail(s, B200REG_ERR_ARG, "get_map_consistency: no build yet");
+  return sm_guarded(s, [&]() {
+    const MapConsistency& m = *s->mc;
+    const size_t k = std::min(capacity, (size_t)m.info.n_points);
+    if (k) {
+      if (n) B200_CUDA(cudaMemcpyAsync(n, m.n.ptr, k * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      if (h) B200_CUDA(cudaMemcpyAsync(h, m.h.ptr, k * sizeof(double), cudaMemcpyDeviceToHost, s->stream));
+      if (plane_var) B200_CUDA(cudaMemcpyAsync(plane_var, m.plane.ptr, k * sizeof(double), cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaStreamSynchronize(s->stream));
+    }
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_submap_consistency(b200sm_t s, b200sm_submap_consistency* rows, size_t capacity) {
+  if (!s || (!rows && capacity)) return B200REG_ERR_ARG;
+  if (!s->mc) return sm_fail(s, B200REG_ERR_ARG, "get_submap_consistency: no build yet");
+  const std::vector<b200sm_submap_consistency>& r = s->mc->sub_rows;
+  const size_t k = std::min(capacity, r.size());
+  if (k) std::memcpy(rows, r.data(), k * sizeof(b200sm_submap_consistency));
+  return B200REG_OK;
+}
+
+int b200sm_save_map_consistency_pcd_ascii(b200sm_t s, const char* path, size_t* n_points, size_t* n_bytes) {
+  if (!s || !path) return B200REG_ERR_ARG;
+  if (!s->mc) return sm_fail(s, B200REG_ERR_ARG, "save_map_consistency_pcd_ascii: no build yet");
+  const MapConsistency& m = *s->mc;
+  const size_t total = (size_t)m.info.n_points;
+  if (total == 0) return sm_fail(s, B200REG_ERR_ARG, "save_map_consistency_pcd_ascii: the map has no points");
+  size_t now = 0;
+  for (const auto& sub : s->submaps) now += sub->n;
+  if (s->submaps.size() != m.sub_rows.size() || now != total)
+    return sm_fail(s, B200REG_ERR_ARG, "save_map_consistency_pcd_ascii: the session's submaps changed since the build");
+  return sm_guarded(s, [&]() {
+    const int rc = assemble_on_device(s, m.poses.data(), total);
+    if (rc != B200REG_OK) return rc;
+    mc_intensity_launch(s->assembled.ptr, m.h.ptr, total, s->stream);
+    s->launches += 1;
+    return write_pcd_ascii(s, s->assembled.ptr, total, path, "save_map_consistency_pcd_ascii", n_points, n_bytes);
+  });
 }
 
 }  // extern "C"

@@ -622,6 +622,49 @@ class ScanMatcher:
         self._check(self._lib.b200sm_save_static_map_pcd_ascii(self._h, os.fsencode(path), C.byref(n), C.byref(size)))
         return int(n.value), int(size.value)
 
+    # ---- map consistency: neighbourhood entropy and plane variance (b200sm_build_map_consistency, csrc/map_consistency.hpp) ----
+    def buildMapConsistency(self, poses=None, radius: float = 0.5, min_neighbors: int = 10, query_stride: int = 1) -> dict:
+        """How crisp the map of every submap at its own pose (poses None) or at `poses` (N, 4, 4) is, built on the device:
+        per query point the entropy h and plane variance of its neighbours within `radius`, and their means MME and MPV
+        over the valid queries. Returns the build's info as a dict (box_origin, box_dims, n_points, n_skipped, n_cells,
+        n_queries, n_valid, n_neighbors, n_candidates, sum_h_q, sum_plane_q, mme, mpv)."""
+        P = None
+        if poses is not None:
+            P = np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(self.numSubmaps(), 4, 4).transpose(0, 2, 1))
+        prm = _capi.SmMapConsistencyParams(float(radius), int(min_neighbors), int(query_stride))
+        info = _capi.SmMapConsistencyInfo()
+        self._check(self._lib.b200sm_build_map_consistency(self._h, _ptr(P) if P is not None else None, C.byref(prm),
+                                                           C.byref(info)))
+        self._mc = (int(info.n_points), self.numSubmaps())
+        return _struct_dict(info)
+
+    def mapConsistency(self) -> dict:
+        """The per-point layers of the last build in map order: n uint32 (neighbours of a query, 0 otherwise), h float64
+        (nats) and plane_var float64 (m^2), NaN for an invalid query and for every other point."""
+        M = getattr(self, "_mc", (0, 0))[0]
+        out = dict(n=np.empty(M, dtype=np.uint32), h=np.empty(M, dtype=np.float64), plane_var=np.empty(M, dtype=np.float64))
+        self._check(self._lib.b200sm_get_map_consistency(self._h, _ptr(out["n"]), _ptr(out["h"]), _ptr(out["plane_var"]), M))
+        return out
+
+    def submapConsistency(self) -> dict:
+        """The per-submap rows of the last build as arrays of length N (submaps at the build): n_points, n_queries, n_valid,
+        n_neighbors (uint64), sum_h_q, sum_plane_q (int64), mme, mpv (float64, NaN without a valid query)."""
+        N = getattr(self, "_mc", (0, 0))[1]
+        rows = (_capi.SmSubmapConsistency * max(N, 1))()
+        self._check(self._lib.b200sm_get_submap_consistency(self._h, rows, N))
+        out = {}
+        for k, t in _capi.SmSubmapConsistency._fields_:
+            dt = np.float64 if t is C.c_double else (np.int64 if t is C.c_longlong else np.uint64)
+            out[k] = np.array([getattr(rows[i], k) for i in range(N)], dtype=dt)
+        return out
+
+    def saveMapConsistencyPcd(self, path):
+        """pcl::io::savePCDFileASCII(path, map) of the map at the last build's poses with its intensity replaced by h (NaN
+        where invalid), for a heat map in a viewer. Returns (points, file bytes)."""
+        n, size = C.c_size_t(0), C.c_size_t(0)
+        self._check(self._lib.b200sm_save_map_consistency_pcd_ascii(self._h, os.fsencode(path), C.byref(n), C.byref(size)))
+        return int(n.value), int(size.value)
+
     # ---- read-back ----
     def stats(self) -> dict:
         st = _capi.SmStats()
