@@ -811,6 +811,56 @@ int b200sm_get_submap_consistency(b200sm_t s, b200sm_submap_consistency* rows, s
  * without points, or submaps added since the build: B200REG_ERR_ARG. A file that cannot be opened or written:
  * B200REG_ERR_IO. */
 int b200sm_save_map_consistency_pcd_ascii(b200sm_t s, const char* path, size_t* n_points, size_t* n_bytes);
+/* ---- map changes: what changed between two recordings, and the map brought up to date --------------------------------
+ * No counterpart in the reference. The submaps are split into two epochs: BEFORE, submaps [0, split), and AFTER,
+ * [split, n_submaps). The rays, voxels and walks are those of b200sm_build_static_map with the same parameters, but each
+ * voxel counts the submaps that hit and freed it in each epoch separately. In an epoch a voxel is FREE when the static map
+ * would call it dynamic from that epoch's counts, and OCCUPIED when that epoch hit it and it is not free. A voxel is
+ * APPEARED when it is occupied AFTER and free BEFORE, VANISHED when occupied BEFORE and free AFTER, else UNCHANGED. A point
+ * of an AFTER submap in an APPEARED voxel is APPEARED, a point of a BEFORE submap in a VANISHED voxel is VANISHED, every
+ * other point (skipped ones included) UNCHANGED. The updated map is the assembled map without the VANISHED points: save it
+ * and hand it to b200sm_set_prior_map_pcd to localise in the map as it is now. Something that only moves through one
+ * recording is dynamic in that recording, not occupied, so it is never reported as a change. The exact definitions are
+ * in csrc/map_changes.hpp; DESIGN.md section 7b describes the build. Bitwise deterministic; the session's submaps, poses
+ * and other products (the static map included) are not changed. NDT and GICP sessions alike. */
+#define B200SM_CHANGE_UNCHANGED 0
+#define B200SM_CHANGE_APPEARED 1
+#define B200SM_CHANGE_VANISHED 2
+typedef struct b200sm_map_change_info {
+  int box_origin[3];                 /* as in b200sm_static_map_info: the box of both epochs' endpoint voxels           */
+  unsigned box_dims[3];
+  long long split_submap;            /* the first AFTER submap (split_submap -1 resolved)                              */
+  unsigned long long n_rays, n_skipped; /* points cast as rays / not cast                                               */
+  unsigned long long n_voxels, n_appeared_voxels, n_vanished_voxels; /* voxels some endpoint lies in; changed ones      */
+  unsigned long long n_points, n_appeared_points, n_vanished_points; /* the assembled map; its changed points           */
+  unsigned long long n_updated_points; /* the updated map: n_points - n_vanished_points                                 */
+  int n_batches;                     /* launches of the walks; no batch holds submaps of both epochs                    */
+} b200sm_map_change_info;
+/* Build the changes from every submap at its own pose (poses_colmajor16 NULL) or at the given 16 * n_submaps doubles.
+ * params NULL: the static map's defaults. split_submap: the first AFTER submap, in [1, n_submaps); -1 = the first submap
+ * of the session's last segment (after b200sm_merge_session, the merged recording). Refused with B200REG_ERR_ARG, before
+ * anything is sized, the previous build staying: split_submap -1 on a session of one segment, any other value outside
+ * [1, n_submaps), and everything b200sm_build_static_map refuses. The session keeps the build until the next one or
+ * destroy, beside (not in place of) the static map's: the rank index (8 bytes per 32 box voxels), 17 bytes per occupied
+ * voxel (four counts and a label), 1 byte per point (its label) and 16 per point of the updated map; the walks' bitmap
+ * scratch is the static map's. info may be NULL. */
+int b200sm_build_map_changes(b200sm_t s, const double* poses_colmajor16, const b200sm_static_map_params* params, long long split_submap,
+                             b200sm_map_change_info* info);
+/* The label of every point of the last build (B200SM_CHANGE_*), in map order: *n = n_points; min(*n, capacity) bytes are
+ * copied (capacity 0: a size query). No build yet: B200REG_ERR_ARG. */
+int b200sm_get_map_changes(b200sm_t s, unsigned char* labels, size_t capacity, size_t* n);
+/* The occupied voxels of the last build in rank order (as b200sm_get_map_voxels): *n = their number; min(*n, capacity) rows
+ * of each non-NULL array: ijk3 (3 ints), the counts of each epoch, label (B200SM_CHANGE_*). No build yet: B200REG_ERR_ARG. */
+int b200sm_get_change_voxels(b200sm_t s, int* ijk3, unsigned* hits_before, unsigned* frees_before, unsigned* hits_after,
+                             unsigned* frees_after, unsigned char* label, size_t capacity, size_t* n);
+/* The updated map of the last build: x, y, z, intensity floats, in the assembled map's order. *n = its points; min(*n,
+ * capacity) points are copied. offsets (may be NULL) = n_submaps at the build + 1 prefix sums per submap. No build yet:
+ * B200REG_ERR_ARG. */
+int b200sm_get_updated_map(b200sm_t s, float* out_xyzi, size_t capacity, size_t* n, size_t* offsets);
+/* pcl::io::savePCDFileASCII(path, updated map), written as b200sm_save_static_map_pcd_ascii writes. n_points, n_bytes (may
+ * be NULL) = points and file size. No build yet, or an updated map without points (no file is created): B200REG_ERR_ARG.
+ * A file that cannot be opened or written: B200REG_ERR_IO. */
+int b200sm_save_updated_map_pcd_ascii(b200sm_t s, const char* path, size_t* n_points, size_t* n_bytes);
 /* The same text for a HOST PointXYZI cloud (records as in b200sm_import_submap; intensity_offset_bytes >= 0), formatted
  * on `device`. *n_bytes = size of the whole file content (header and data); min(*n_bytes, capacity) bytes are copied to
  * out, so capacity 0 is a size query. B200REG_ERR_ARG for n == 0, a negative intensity offset, or a stride or offset that

@@ -623,6 +623,46 @@ class ScanMatcherSession {
   }
   // PCL's ASCII PCD of the last static map (as saveMapPCDASCII writes the map)
   void saveStaticMapPcd(const std::string& path) { check(b200sm_save_static_map_pcd_ascii(s_.get(), path.c_str(), nullptr, nullptr)); }
+  // ---- map changes (b200sm_build_map_changes): what appeared and vanished between the submaps before split_submap and
+  // those from it on (-1: the last segment's first submap); poses empty = the submaps' own; p nullptr = the defaults
+  b200sm_map_change_info buildMapChanges(const std::vector<double>& poses_colmajor16 = {}, long long split_submap = -1,
+                                         const b200sm_static_map_params* p = nullptr) {
+    b200sm_map_change_info info{};
+    check(b200sm_build_map_changes(s_.get(), poses_colmajor16.empty() ? nullptr : poses_colmajor16.data(), p, split_submap, &info));
+    ch_sub_ = numSubmaps();
+    return info;
+  }
+  // the label of every point of the last build (B200SM_CHANGE_*), in map order
+  void mapChanges(std::vector<unsigned char>& labels) {
+    size_t n = 0;
+    check(b200sm_get_map_changes(s_.get(), nullptr, 0, &n));
+    labels.resize(n);
+    check(b200sm_get_map_changes(s_.get(), labels.data(), n, &n));
+  }
+  // the occupied voxels of the last build in rank order: 3 ints each, the counts of each epoch, the label
+  void changeVoxels(std::vector<int>& ijk3, std::vector<unsigned>& hits_before, std::vector<unsigned>& frees_before,
+                    std::vector<unsigned>& hits_after, std::vector<unsigned>& frees_after, std::vector<unsigned char>& label) {
+    size_t n = 0;
+    check(b200sm_get_change_voxels(s_.get(), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, &n));
+    ijk3.resize(3 * n);
+    hits_before.resize(n);
+    frees_before.resize(n);
+    hits_after.resize(n);
+    frees_after.resize(n);
+    label.resize(n);
+    check(b200sm_get_change_voxels(s_.get(), ijk3.data(), hits_before.data(), frees_before.data(), hits_after.data(), frees_after.data(),
+                                   label.data(), n, &n));
+  }
+  // the last updated map, x y z intensity per point; offsets (when non-null) = per-submap prefix sums (submaps at the build + 1)
+  void updatedMap(std::vector<float>& xyzi, std::vector<size_t>* offsets = nullptr) {
+    size_t n = 0;
+    check(b200sm_get_updated_map(s_.get(), nullptr, 0, &n, nullptr));
+    xyzi.resize(4 * n);
+    if (offsets) offsets->resize(ch_sub_ + 1);
+    check(b200sm_get_updated_map(s_.get(), xyzi.data(), n, &n, offsets ? offsets->data() : nullptr));
+  }
+  // PCL's ASCII PCD of the last updated map: the prior map for setPriorMapPcd next time
+  void saveUpdatedMapPcd(const std::string& path) { check(b200sm_save_updated_map_pcd_ascii(s_.get(), path.c_str(), nullptr, nullptr)); }
   b200sm_localize_stats localizeStats() const {
     b200sm_localize_stats st{};
     check(b200sm_get_localize_stats(s_.get(), &st));
@@ -644,6 +684,7 @@ class ScanMatcherSession {
   size_t og_cells_ = 0;  // cells of the last grid this adapter built
   size_t el_cells_ = 0;  // cells of the last elevation map this adapter built
   size_t sm_sub_ = 0;    // submaps at the last static-map build of this adapter
+  size_t ch_sub_ = 0;    // submaps at the last map-change build of this adapter
 };
 
 }  // namespace b200reg

@@ -55,6 +55,8 @@ SYMBOLS = [
     "b200sm_build_static_map", "b200sm_get_static_map", "b200sm_get_map_voxels", "b200sm_save_static_map_pcd_ascii",
     "b200sm_build_map_consistency", "b200sm_get_map_consistency", "b200sm_get_submap_consistency",
     "b200sm_save_map_consistency_pcd_ascii",
+    "b200sm_build_map_changes", "b200sm_get_map_changes", "b200sm_get_change_voxels", "b200sm_get_updated_map",
+    "b200sm_save_updated_map_pcd_ascii",
     "b200sm_merge_session", "b200sm_get_merge_scores", "b200sm_get_segments",
     "b200sm_save_session", "b200sm_load_session", "b200sm_get_session_graph",
     # include/b200comm.h
@@ -129,6 +131,14 @@ class SmStaticMapInfo(C.Structure):
     _fields_ = [("box_origin", C.c_int * 3), ("box_dims", C.c_uint * 3), ("n_rays", C.c_ulonglong), ("n_skipped", C.c_ulonglong),
                 ("n_voxels", C.c_ulonglong), ("n_dynamic_voxels", C.c_ulonglong), ("n_points", C.c_ulonglong),
                 ("n_static_points", C.c_ulonglong), ("n_batches", C.c_int)]
+
+
+class SmMapChangeInfo(C.Structure):
+    _fields_ = [("box_origin", C.c_int * 3), ("box_dims", C.c_uint * 3), ("split_submap", C.c_longlong),
+                ("n_rays", C.c_ulonglong), ("n_skipped", C.c_ulonglong), ("n_voxels", C.c_ulonglong),
+                ("n_appeared_voxels", C.c_ulonglong), ("n_vanished_voxels", C.c_ulonglong), ("n_points", C.c_ulonglong),
+                ("n_appeared_points", C.c_ulonglong), ("n_vanished_points", C.c_ulonglong),
+                ("n_updated_points", C.c_ulonglong), ("n_batches", C.c_int)]
 
 
 class SmLoopEdge(C.Structure):
@@ -368,6 +378,11 @@ def lib() -> C.CDLL:
     L.b200sm_get_map_consistency.argtypes = [vp, vp, vp, vp, sz]
     L.b200sm_get_submap_consistency.argtypes = [vp, vp, sz]
     L.b200sm_save_map_consistency_pcd_ascii.argtypes = [vp, C.c_char_p, C.POINTER(sz), C.POINTER(sz)]
+    L.b200sm_build_map_changes.argtypes = [vp, vp, C.POINTER(SmStaticMapParams), C.c_longlong, C.POINTER(SmMapChangeInfo)]
+    L.b200sm_get_map_changes.argtypes = [vp, vp, sz, C.POINTER(sz)]
+    L.b200sm_get_change_voxels.argtypes = [vp, vp, vp, vp, vp, vp, vp, sz, C.POINTER(sz)]
+    L.b200sm_get_updated_map.argtypes = [vp, vp, sz, C.POINTER(sz), vp]
+    L.b200sm_save_updated_map_pcd_ascii.argtypes = [vp, C.c_char_p, C.POINTER(sz), C.POINTER(sz)]
     L.b200sm_merge_session.argtypes = [vp, vp, vp, C.POINTER(SmMergeParams), vp, i, vp, sz, C.POINTER(sz), vp,
                                         C.POINTER(SmMergeResult)]
     L.b200sm_get_merge_scores.argtypes = [vp, sz, C.POINTER(sz), C.POINTER(sz), vp, vp]

@@ -44,6 +44,7 @@
 #include "elevation.cuh"
 #include "engine.hpp"
 #include "global_grid.hpp"
+#include "map_changes.cuh"
 #include "map_cut.hpp"
 #include "occupancy.cuh"
 #include "place_recognition.cuh"
@@ -277,6 +278,19 @@ struct MapConsistency {
   std::vector<double> poses;  // the build's poses, 16 column-major doubles per submap
 };
 
+// One map-change build (b200sm_build_map_changes): the rank index over its box, the per-epoch counts and labels per
+// occupied voxel, the label per point, and the updated map with its per-submap offsets.
+struct MapChanges {
+  DeviceBuffer<RankWord> index;
+  DeviceBuffer<uint32_t> hits[2], frees[2];
+  DeviceBuffer<unsigned char> label, point_label;
+  DeviceBuffer<float4> updated;
+  SmBox box{};
+  unsigned long long n_words = 0;
+  b200sm_map_change_info info{};
+  std::vector<size_t> offsets;  // n_submaps at the build + 1
+};
+
 struct b200sm_session {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -415,6 +429,14 @@ struct b200sm_session {
   DeviceBuffer<unsigned> mc_idx, mc_tmp;
   RankIndexScratch mc_scan;
   std::unique_ptr<MapConsistency> mc;
+  // map changes (b200sm_build_map_changes): the per-call table, bounds, counters, first map index per entry and tile
+  // counts, the voxel list of the read-back, and the last build, kept until the next build succeeds. The walks' bitmap
+  // scratch and the rank scan's scratch are the static map's: per-call workspace that no read-back uses.
+  DeviceBuffer<SmEntry> ch_table;
+  DeviceBuffer<int> ch_bounds, ch_ijk;
+  DeviceBuffer<unsigned long long> ch_counters;
+  DeviceBuffer<unsigned> ch_map_first, ch_tiles, ch_tiles_tmp;
+  std::unique_ptr<MapChanges> ch;
 };
 
 namespace {
@@ -2914,6 +2936,130 @@ SmParams sm_params_from(const b200sm_static_map_params* p) {
   return q;
 }
 
+// A build's per-call buffers: the table, the entries' bounds and the counters (n_counters slots, SM_CTR_* first)
+struct SmWork {
+  DeviceBuffer<SmEntry>& table;
+  DeviceBuffer<int>& bounds;
+  DeviceBuffer<unsigned long long>& counters;
+  int n_counters;
+};
+
+// What the front half leaves for the rest of a build
+struct SmFront {
+  SmBox box{};
+  unsigned long long n_words = 0;
+  unsigned n_voxels = 0;
+  int batches = 0;
+};
+
+// The front half the static map and the map changes share: the table's upload, K15a and the box (refused here, before
+// anything is sized from it), then `replacing()` (the caller's last build is about to be overwritten), K15b with the rank
+// scan, and the walks K15c / K15d in batches of consecutive entries. The entries [0, split_entry) fold into hits[0] /
+// frees[0] and, when split_entry < table.size(), the entries [split_entry, table.size()) into hits[1] / frees[1]; no batch
+// crosses split_entry. The counts are sized and zeroed here (one slot when there is no occupied voxel). Must run inside
+// sm_guarded; `what` prefixes the messages.
+template <class Replacing>
+int sm_front_half(b200sm_t s, const char* what, std::vector<SmEntry>& table, unsigned long long tiles, const SmConst& c, SmWork w,
+                  size_t split_entry, DeviceBuffer<RankWord>& index, DeviceBuffer<uint32_t>* hits, DeviceBuffer<uint32_t>* frees,
+                  Replacing&& replacing, SmFront* out) {
+  const int n_entries = (int)table.size();
+  // K15a: one launch, one read-back of the bounds and counts
+  std::vector<int> bounds(6 * table.size());
+  for (size_t r = 0; r < table.size(); r++)
+    for (int a = 0; a < 3; a++) {
+      bounds[6 * r + a] = INT_MAX;
+      bounds[6 * r + 3 + a] = INT_MIN;
+    }
+  unsigned long long ctr[2] = {};
+  w.counters.ensure(w.n_counters);
+  B200_CUDA(cudaMemsetAsync(w.counters.ptr, 0, w.n_counters * sizeof(unsigned long long), s->stream));
+  if (n_entries) {
+    w.table.ensure(table.size());
+    w.bounds.ensure(bounds.size());
+    B200_CUDA(cudaMemcpyAsync(w.table.ptr, table.data(), table.size() * sizeof(SmEntry), cudaMemcpyHostToDevice, s->stream));
+    B200_CUDA(cudaMemcpyAsync(w.bounds.ptr, bounds.data(), bounds.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
+    sm_bounds_launch(w.table.ptr, n_entries, (unsigned)tiles, c, w.bounds.ptr, w.counters.ptr, s->stream);
+    s->launches += 1;
+    B200_CUDA(cudaMemcpyAsync(bounds.data(), w.bounds.ptr, bounds.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+  }
+  B200_CUDA(cudaMemcpyAsync(ctr, w.counters.ptr, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
+  B200_CUDA(cudaStreamSynchronize(s->stream));
+  int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
+  for (size_t r = 0; r < table.size(); r++)
+    for (int a = 0; a < 3; a++) {
+      lo[a] = std::min(lo[a], bounds[6 * r + a]);
+      hi[a] = std::max(hi[a], bounds[6 * r + 3 + a]);
+    }
+  const bool any_ray = ctr[SM_CTR_RAYS] > 0;
+  SmBox box{};
+  unsigned long long cells = 0;
+  if (any_ray && !sm_box(lo, hi, box.dims, &cells)) {
+    s->err = std::string(what) + ": a box of " + std::to_string((long long)hi[0] - lo[0] + 1) + " x " +
+             std::to_string((long long)hi[1] - lo[1] + 1) + " x " + std::to_string((long long)hi[2] - lo[2] + 1) +
+             " voxels exceeds 2^31 - 1 voxels";
+    return (int)B200REG_ERR_ARG;
+  }
+  if (any_ray)
+    for (int a = 0; a < 3; a++) box.lo[a] = lo[a];
+  replacing();
+  const unsigned long long n_words = (cells + 31) / 32;
+  unsigned n_voxels = 0;
+  if (any_ray) {
+    // K15b: the rank index over the box, then the number of occupied voxels
+    index.ensure((size_t)n_words);
+    rank_index_clear(index.ptr, (int)n_words, s->stream);
+    sm_mark_launch(w.table.ptr, n_entries, (unsigned)tiles, c, box, index.ptr, w.counters.ptr, s->stream);
+    s->sm_scan.total.ensure(1);
+    rank_index_scan_async(index.ptr, (size_t)n_words, s->sm_scan, s->sm_scan.total.ptr, s->stream);
+    s->launches += 3;
+    B200_CUDA(cudaMemcpyAsync(&n_voxels, s->sm_scan.total.ptr, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+  }
+  const int n_epochs = split_entry < table.size() ? 2 : 1;
+  const size_t nv = std::max<size_t>(n_voxels, 1);
+  for (int e = 0; e < n_epochs; e++) {
+    hits[e].ensure(nv);
+    frees[e].ensure(nv);
+    B200_CUDA(cudaMemsetAsync(hits[e].ptr, 0, nv * sizeof(uint32_t), s->stream));
+    B200_CUDA(cudaMemsetAsync(frees[e].ptr, 0, nv * sizeof(uint32_t), s->stream));
+  }
+  // K15c / K15d in batches of consecutive submaps of one epoch: every submap's two bitmaps have the same size
+  const unsigned long long words_per = (n_voxels + 31ull) / 32ull;
+  int batches = 0;
+  if (n_voxels > 0) {
+    const size_t per_batch = (size_t)std::max<unsigned long long>(1ull, SM_SCRATCH_WORDS / (2ull * words_per));
+    const size_t largest = std::min(per_batch, table.size());
+    s->sm_scratch.ensure((size_t)(2ull * words_per * largest));
+    for (int e = 0; e < n_epochs; e++) {
+      const size_t r0 = e == 0 ? 0 : split_entry, r1 = e == n_epochs - 1 ? table.size() : split_entry;
+      for (size_t b0 = r0; b0 < r1; b0 += per_batch) {
+        const size_t b1 = std::min(r1, b0 + per_batch);
+        unsigned long long bt = 0;
+        for (size_t r = b0; r < b1; r++) {
+          table[r].batch_tile = (unsigned)bt;
+          bt += (table[r].n + SM_TILE - 1) / SM_TILE;
+        }
+        if (2ull * words_per * (b1 - b0) > s->sm_scratch.cap || b1 > w.table.cap)
+          return sm_fail(s, B200REG_ERR_CUDA, (std::string(what) + ": a walk batch larger than its scratch").c_str());
+        // the previous batch's kernels read the table: this copy is stream-ordered behind them
+        B200_CUDA(cudaMemcpyAsync(w.table.ptr + b0, table.data() + b0, (b1 - b0) * sizeof(SmEntry), cudaMemcpyHostToDevice,
+                                  s->stream));
+        B200_CUDA(cudaMemsetAsync(s->sm_scratch.ptr, 0, 2ull * words_per * (b1 - b0) * sizeof(uint32_t), s->stream));
+        sm_walk_launch(w.table.ptr + b0, (int)(b1 - b0), (unsigned)bt, c, box, index.ptr, n_voxels, words_per, s->sm_scratch.ptr,
+                       w.counters.ptr, s->stream);
+        sm_fold_launch(s->sm_scratch.ptr, (int)(b1 - b0), words_per, n_voxels, hits[e].ptr, frees[e].ptr, s->stream);
+        s->launches += 2;
+        batches++;
+      }
+    }
+  }
+  out->box = box;
+  out->n_words = n_words;
+  out->n_voxels = n_voxels;
+  out->batches = batches;
+  return (int)B200REG_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2955,91 +3101,17 @@ int b200sm_build_static_map(b200sm_t s, const double* poses_colmajor16, const b2
   if (total > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_static_map: a map of 2^32 points or more");
   const int n_entries = (int)table.size();
   return sm_guarded(s, [&]() {
-    // K15a: one launch, one read-back of the bounds and counts
-    std::vector<int> bounds(6 * table.size());
-    for (size_t r = 0; r < table.size(); r++)
-      for (int a = 0; a < 3; a++) {
-        bounds[6 * r + a] = INT_MAX;
-        bounds[6 * r + 3 + a] = INT_MIN;
-      }
+    SmFront f;
+    const int rc = sm_front_half(s, "build_static_map", table, tiles, c, SmWork{s->sm_table, s->sm_bounds, s->sm_counters, SM_CTR_COUNT},
+                                 table.size(), s->sm_index, &s->sm_hits, &s->sm_frees, [&]() { s->sm_built = false; }, &f);
+    if (rc != B200REG_OK) return rc;
+    const SmBox& box = f.box;
+    const unsigned long long n_words = f.n_words;
+    const unsigned n_voxels = f.n_voxels;
+    const int batches = f.batches;
     unsigned long long ctr[SM_CTR_COUNT] = {};
-    s->sm_counters.ensure(SM_CTR_COUNT);
-    B200_CUDA(cudaMemsetAsync(s->sm_counters.ptr, 0, SM_CTR_COUNT * sizeof(unsigned long long), s->stream));
-    if (n_entries) {
-      s->sm_table.ensure(table.size());
-      s->sm_bounds.ensure(bounds.size());
-      B200_CUDA(cudaMemcpyAsync(s->sm_table.ptr, table.data(), table.size() * sizeof(SmEntry), cudaMemcpyHostToDevice, s->stream));
-      B200_CUDA(cudaMemcpyAsync(s->sm_bounds.ptr, bounds.data(), bounds.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
-      sm_bounds_launch(s->sm_table.ptr, n_entries, (unsigned)tiles, c, s->sm_bounds.ptr, s->sm_counters.ptr, s->stream);
-      s->launches += 1;
-      B200_CUDA(cudaMemcpyAsync(bounds.data(), s->sm_bounds.ptr, bounds.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
-    }
-    B200_CUDA(cudaMemcpyAsync(ctr, s->sm_counters.ptr, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
-    B200_CUDA(cudaStreamSynchronize(s->stream));
-    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
-    for (size_t r = 0; r < table.size(); r++)
-      for (int a = 0; a < 3; a++) {
-        lo[a] = std::min(lo[a], bounds[6 * r + a]);
-        hi[a] = std::max(hi[a], bounds[6 * r + 3 + a]);
-      }
-    const bool any_ray = ctr[SM_CTR_RAYS] > 0;
-    SmBox box{};
-    unsigned long long cells = 0;
-    if (any_ray && !sm_box(lo, hi, box.dims, &cells)) {
-      s->err = "build_static_map: a box of " + std::to_string((long long)hi[0] - lo[0] + 1) + " x " +
-               std::to_string((long long)hi[1] - lo[1] + 1) + " x " + std::to_string((long long)hi[2] - lo[2] + 1) +
-               " voxels exceeds 2^31 - 1 voxels";
-      return (int)B200REG_ERR_ARG;
-    }
-    if (any_ray)
-      for (int a = 0; a < 3; a++) box.lo[a] = lo[a];
-    // from here on the previous build is replaced
-    s->sm_built = false;
-    const unsigned long long n_words = (cells + 31) / 32;
-    unsigned n_voxels = 0;
-    if (any_ray) {
-      // K15b: the rank index over the box, then the number of occupied voxels
-      s->sm_index.ensure((size_t)n_words);
-      rank_index_clear(s->sm_index.ptr, (int)n_words, s->stream);
-      sm_mark_launch(s->sm_table.ptr, n_entries, (unsigned)tiles, c, box, s->sm_index.ptr, s->sm_counters.ptr, s->stream);
-      s->sm_scan.total.ensure(1);
-      rank_index_scan_async(s->sm_index.ptr, (size_t)n_words, s->sm_scan, s->sm_scan.total.ptr, s->stream);
-      s->launches += 3;
-      B200_CUDA(cudaMemcpyAsync(&n_voxels, s->sm_scan.total.ptr, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
-      B200_CUDA(cudaStreamSynchronize(s->stream));
-    }
-    const size_t nv = std::max<size_t>(n_voxels, 1);
-    s->sm_hits.ensure(nv);
-    s->sm_frees.ensure(nv);
-    s->sm_dynamic.ensure(nv);
-    B200_CUDA(cudaMemsetAsync(s->sm_hits.ptr, 0, nv * sizeof(uint32_t), s->stream));
-    B200_CUDA(cudaMemsetAsync(s->sm_frees.ptr, 0, nv * sizeof(uint32_t), s->stream));
-    // K15c / K15d in batches of consecutive submaps: every submap's two bitmaps have the same size
-    const unsigned long long words_per = (n_voxels + 31ull) / 32ull;
-    int batches = 0;
+    s->sm_dynamic.ensure(std::max<size_t>(n_voxels, 1));
     if (n_voxels > 0) {
-      const size_t per_batch = (size_t)std::max<unsigned long long>(1ull, SM_SCRATCH_WORDS / (2ull * words_per));
-      const size_t largest = std::min(per_batch, table.size());
-      s->sm_scratch.ensure((size_t)(2ull * words_per * largest));
-      for (size_t b0 = 0; b0 < table.size(); b0 += per_batch) {
-        const size_t b1 = std::min(table.size(), b0 + per_batch);
-        unsigned long long bt = 0;
-        for (size_t r = b0; r < b1; r++) {
-          table[r].batch_tile = (unsigned)bt;
-          bt += (table[r].n + SM_TILE - 1) / SM_TILE;
-        }
-        if (2ull * words_per * (b1 - b0) > s->sm_scratch.cap || b1 > s->sm_table.cap)
-          return sm_fail(s, B200REG_ERR_CUDA, "build_static_map: a walk batch larger than its scratch");
-        // the previous batch's kernels read the table: this copy is stream-ordered behind them
-        B200_CUDA(cudaMemcpyAsync(s->sm_table.ptr + b0, table.data() + b0, (b1 - b0) * sizeof(SmEntry), cudaMemcpyHostToDevice,
-                                  s->stream));
-        B200_CUDA(cudaMemsetAsync(s->sm_scratch.ptr, 0, 2ull * words_per * (b1 - b0) * sizeof(uint32_t), s->stream));
-        sm_walk_launch(s->sm_table.ptr + b0, (int)(b1 - b0), (unsigned)bt, c, box, s->sm_index.ptr, n_voxels, words_per,
-                       s->sm_scratch.ptr, s->sm_counters.ptr, s->stream);
-        sm_fold_launch(s->sm_scratch.ptr, (int)(b1 - b0), words_per, n_voxels, s->sm_hits.ptr, s->sm_frees.ptr, s->stream);
-        s->launches += 2;
-        batches++;
-      }
       // K15e
       sm_classify_launch(s->sm_hits.ptr, s->sm_frees.ptr, n_voxels, c, s->sm_dynamic.ptr, s->sm_counters.ptr, s->stream);
       s->launches += 1;
@@ -3138,6 +3210,210 @@ int b200sm_save_static_map_pcd_ascii(b200sm_t s, const char* path, size_t* n_poi
   const size_t total = (size_t)s->sm_info.n_static_points;
   if (total == 0) return sm_fail(s, B200REG_ERR_ARG, "save_static_map_pcd_ascii: the static map has no points");
   return sm_guarded(s, [&]() { return write_pcd_ascii(s, s->sm_static.ptr, total, path, "save_static_map_pcd_ascii", n_points, n_bytes); });
+}
+
+}  // extern "C"
+
+// ---- map changes: what appeared and vanished between two recordings, and the updated map (csrc/map_changes.hpp,
+// csrc/map_changes.cu, and the static map's front half) ----
+extern "C" {
+
+int b200sm_build_map_changes(b200sm_t s, const double* poses_colmajor16, const b200sm_static_map_params* params, long long split_submap,
+                             b200sm_map_change_info* info) {
+  if (!s) return B200REG_ERR_ARG;
+  const SmParams p = sm_params_from(params);
+  SmConst c;
+  if (const char* why = sm_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_map_changes: ") + why).c_str());
+  const size_t n_sub = s->submaps.size();
+  if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_map_changes: the session has no submaps");
+  unsigned long long split = 0;
+  const unsigned long long last_first = s->seg_first.size() > 1 ? (unsigned long long)s->seg_first.back() : 0ull;
+  if (const char* why = ch_split(split_submap, n_sub, last_first, &split))
+    return sm_fail(s, B200REG_ERR_ARG, (std::string("build_map_changes: ") + why).c_str());
+  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, "build_map_changes: a non-finite pose entry");
+  SubmapTiles t;
+  const int rc = submap_tiles(s, 0, SM_TILE, true, "build_map_changes: a submap of 2^32 points or more",
+                              "build_map_changes: too many points for one launch", &t);
+  if (rc != B200REG_OK) return rc;
+  const std::vector<size_t>& ids = t.ids;
+  const unsigned long long tiles = t.tiles;
+  // the entries of the submaps with points, in submap order, their first map index, and the first AFTER entry
+  std::vector<SmEntry> table;
+  std::vector<unsigned> map_first;
+  size_t split_entry = 0;
+  unsigned long long total = 0;
+  for (size_t k = 0; k < n_sub; k++) {
+    const Submap& sub = *s->submaps[k];
+    SmEntry e;
+    std::memset(&e, 0, sizeof(e));
+    submap_pose_f(s, k, poses_colmajor16, e.T);
+    if (!sm_origin(c, p, e.T, e.o)) {
+      s->err = "build_map_changes: the sensor origin of submap " + std::to_string(k) + " lies beyond 2^30 voxels";
+      return (int)B200REG_ERR_ARG;
+    }
+    if (k == split) split_entry = table.size();
+    const unsigned long long at = total;
+    total += sub.n;
+    if (sub.n == 0) continue;
+    e.cloud = sub.cloud;
+    e.n = (unsigned)sub.n;
+    e.first_tile = t.first_tile[table.size()];
+    table.push_back(e);
+    map_first.push_back((unsigned)at);
+  }
+  if (total > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_map_changes: a map of 2^32 points or more");
+  const int n_entries = (int)table.size();
+  return sm_guarded(s, [&]() {
+    // the new build is made beside the last one, which stays until this one succeeds
+    auto m = std::make_unique<MapChanges>();
+    SmFront f;
+    const int rc = sm_front_half(s, "build_map_changes", table, tiles, c, SmWork{s->ch_table, s->ch_bounds, s->ch_counters, CH_CTR_COUNT},
+                                 split_entry, m->index, m->hits, m->frees, []() {}, &f);
+    if (rc != B200REG_OK) return rc;
+    const unsigned n_voxels = f.n_voxels;
+    const size_t nv = std::max<size_t>(n_voxels, 1);
+    for (int e = 0; e < 2; e++)
+      if (!m->hits[e].ptr) {  // no AFTER submap with points: the front half folded one epoch only
+        m->hits[e].ensure(nv);
+        m->frees[e].ensure(nv);
+        B200_CUDA(cudaMemsetAsync(m->hits[e].ptr, 0, nv * sizeof(uint32_t), s->stream));
+        B200_CUDA(cudaMemsetAsync(m->frees[e].ptr, 0, nv * sizeof(uint32_t), s->stream));
+      }
+    // K20a
+    m->label.ensure(nv);
+    if (n_voxels > 0) {
+      ch_classify_launch(m->hits[CH_BEFORE].ptr, m->frees[CH_BEFORE].ptr, m->hits[CH_AFTER].ptr, m->frees[CH_AFTER].ptr, n_voxels, c,
+                         m->label.ptr, s->ch_counters.ptr, s->stream);
+      s->launches += 1;
+    }
+    // K20b: the point labels and the kept points per tile, scanned into tile offsets; the host reads the total and sizes
+    // the updated map from it
+    m->point_label.ensure(std::max<size_t>((size_t)total, 1));
+    unsigned kept = 0;
+    std::vector<unsigned> tile_off((size_t)tiles + 1, 0);
+    if (tiles) {
+      s->ch_map_first.ensure(map_first.size());
+      B200_CUDA(cudaMemcpyAsync(s->ch_map_first.ptr, map_first.data(), map_first.size() * sizeof(unsigned), cudaMemcpyHostToDevice,
+                                s->stream));
+      s->ch_tiles.ensure((size_t)tiles + 1);
+      ch_label_launch(s->ch_table.ptr, n_entries, (unsigned)tiles, c, f.box, m->index.ptr, m->label.ptr, n_voxels, (int)split_entry,
+                      s->ch_map_first.ptr, m->point_label.ptr, s->ch_tiles.ptr, s->ch_counters.ptr, s->stream);
+      counter_scan_async(s->ch_tiles.ptr, (size_t)tiles, s->ch_tiles_tmp, s->stream);
+      s->launches += 3;
+      B200_CUDA(cudaMemcpyAsync(tile_off.data(), s->ch_tiles.ptr, tile_off.size() * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaStreamSynchronize(s->stream));
+      kept = tile_off[(size_t)tiles];
+    }
+    // K20c
+    m->updated.ensure(std::max<size_t>(kept, 1));
+    if (kept) {
+      ch_write_launch(s->ch_table.ptr, n_entries, (unsigned)tiles, s->ch_map_first.ptr, m->point_label.ptr, s->ch_tiles.ptr, kept,
+                      m->updated.ptr, s->ch_counters.ptr, s->stream);
+      s->launches += 1;
+    }
+    unsigned long long ctr[CH_CTR_COUNT] = {};
+    B200_CUDA(cudaMemcpyAsync(ctr, s->ch_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));  // the host tables go out of scope; the counts are read
+    if (ctr[SM_CTR_TRIPPED])
+      return sm_fail(s, B200REG_ERR_CUDA, "build_map_changes: a voxel outside the box or beyond the rank index, or a point beyond the map");
+    // per-submap offsets: a submap with points starts at its first tile's offset; an empty one where the next one starts
+    m->offsets.assign(n_sub + 1, (size_t)kept);
+    size_t r = table.size();
+    for (size_t k = n_sub; k-- > 0;) {
+      if (r > 0 && ids[r - 1] == k) m->offsets[k] = tile_off[table[--r].first_tile];
+      else m->offsets[k] = m->offsets[k + 1];
+    }
+    m->box = f.box;
+    m->n_words = f.n_words;
+    b200sm_map_change_info& I = m->info;
+    for (int a = 0; a < 3; a++) {
+      I.box_origin[a] = f.box.lo[a];
+      I.box_dims[a] = f.box.dims[a];
+    }
+    I.split_submap = (long long)split;
+    I.n_rays = ctr[SM_CTR_RAYS];
+    I.n_skipped = ctr[SM_CTR_SKIPPED];
+    I.n_voxels = n_voxels;
+    I.n_appeared_voxels = ctr[CH_CTR_APPEARED_VOXELS];
+    I.n_vanished_voxels = ctr[CH_CTR_VANISHED_VOXELS];
+    I.n_points = total;
+    I.n_appeared_points = ctr[CH_CTR_APPEARED_POINTS];
+    I.n_vanished_points = ctr[CH_CTR_VANISHED_POINTS];
+    I.n_updated_points = kept;
+    I.n_batches = f.batches;
+    if (info) *info = I;
+    s->ch = std::move(m);
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_map_changes(b200sm_t s, unsigned char* labels, size_t capacity, size_t* n) {
+  if (!s || (!labels && capacity)) return B200REG_ERR_ARG;
+  if (!s->ch) return sm_fail(s, B200REG_ERR_ARG, "get_map_changes: no build yet");
+  return sm_guarded(s, [&]() {
+    const MapChanges& m = *s->ch;
+    if (n) *n = (size_t)m.info.n_points;
+    const size_t k = std::min(capacity, (size_t)m.info.n_points);
+    if (k) {
+      B200_CUDA(cudaMemcpyAsync(labels, m.point_label.ptr, k, cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaStreamSynchronize(s->stream));
+    }
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_change_voxels(b200sm_t s, int* ijk3, unsigned* hits_before, unsigned* frees_before, unsigned* hits_after,
+                             unsigned* frees_after, unsigned char* label, size_t capacity, size_t* n) {
+  if (!s) return B200REG_ERR_ARG;
+  if (!s->ch) return sm_fail(s, B200REG_ERR_ARG, "get_change_voxels: no build yet");
+  return sm_guarded(s, [&]() {
+    const MapChanges& m = *s->ch;
+    const unsigned n_voxels = (unsigned)m.info.n_voxels;
+    if (n) *n = n_voxels;
+    const size_t k = std::min(capacity, (size_t)n_voxels);
+    if (k == 0) return (int)B200REG_OK;
+    if (ijk3) {
+      s->ch_ijk.ensure(3 * (size_t)n_voxels);
+      sm_voxel_list_launch(m.index.ptr, m.n_words, m.box, n_voxels, s->ch_ijk.ptr, s->stream);
+      s->launches += 1;
+      B200_CUDA(cudaMemcpyAsync(ijk3, s->ch_ijk.ptr, 3 * k * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+    }
+    auto get = [&](unsigned* dst, const DeviceBuffer<uint32_t>& src) {
+      if (dst) B200_CUDA(cudaMemcpyAsync(dst, src.ptr, k * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+    };
+    get(hits_before, m.hits[CH_BEFORE]);
+    get(frees_before, m.frees[CH_BEFORE]);
+    get(hits_after, m.hits[CH_AFTER]);
+    get(frees_after, m.frees[CH_AFTER]);
+    if (label) B200_CUDA(cudaMemcpyAsync(label, m.label.ptr, k, cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_updated_map(b200sm_t s, float* out_xyzi, size_t capacity, size_t* n, size_t* offsets) {
+  if (!s || (!out_xyzi && capacity)) return B200REG_ERR_ARG;
+  if (!s->ch) return sm_fail(s, B200REG_ERR_ARG, "get_updated_map: no build yet");
+  return sm_guarded(s, [&]() {
+    const MapChanges& m = *s->ch;
+    const size_t total = (size_t)m.info.n_updated_points;
+    if (n) *n = total;
+    if (offsets) std::memcpy(offsets, m.offsets.data(), m.offsets.size() * sizeof(size_t));
+    const size_t k = std::min(capacity, total);
+    if (k) {
+      B200_CUDA(cudaMemcpyAsync(out_xyzi, m.updated.ptr, k * sizeof(float4), cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaStreamSynchronize(s->stream));
+    }
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_save_updated_map_pcd_ascii(b200sm_t s, const char* path, size_t* n_points, size_t* n_bytes) {
+  if (!s || !path) return B200REG_ERR_ARG;
+  if (!s->ch) return sm_fail(s, B200REG_ERR_ARG, "save_updated_map_pcd_ascii: no build yet");
+  const size_t total = (size_t)s->ch->info.n_updated_points;
+  if (total == 0) return sm_fail(s, B200REG_ERR_ARG, "save_updated_map_pcd_ascii: the updated map has no points");
+  return sm_guarded(s, [&]() { return write_pcd_ascii(s, s->ch->updated.ptr, total, path, "save_updated_map_pcd_ascii", n_points, n_bytes); });
 }
 
 }  // extern "C"

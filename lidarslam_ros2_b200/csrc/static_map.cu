@@ -9,21 +9,6 @@
 namespace b200 {
 namespace {
 
-// the linear index of voxel (x, y, z) in the box; false outside it (the differences in int64: voxel indices reach 2^30 + 2^14)
-__device__ __forceinline__ bool sm_lin(const SmBox& b, int x, int y, int z, unsigned* lin) {
-  const long long wx = (long long)x - b.lo[0], wy = (long long)y - b.lo[1], wz = (long long)z - b.lo[2];
-  if (wx < 0 || wy < 0 || wz < 0 || wx >= b.dims[0] || wy >= b.dims[1] || wz >= b.dims[2]) return false;
-  *lin = (unsigned)(((unsigned long long)wz * b.dims[1] + (unsigned long long)wy) * b.dims[0] + (unsigned long long)wx);
-  return true;
-}
-
-// the rank of an occupied voxel; false when it is outside the box or not occupied
-__device__ __forceinline__ bool sm_rank(const RankWord* __restrict__ index, const SmBox& b, int x, int y, int z, unsigned* r) {
-  unsigned lin;
-  if (!sm_lin(b, x, y, z, &lin)) return false;
-  return rank_probe(__ldg(reinterpret_cast<const uint2*>(index + (lin >> 5))), lin & 31u, *r);
-}
-
 // set bit r of a bitmap of n_voxels bits, reading first: the rays of a submap cross the voxels near its origin over and over,
 // and a bit that is already set needs no atomic
 __device__ __forceinline__ void sm_set(uint32_t* bits, unsigned r, unsigned n_voxels, unsigned* tripped) {

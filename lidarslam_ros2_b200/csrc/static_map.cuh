@@ -6,6 +6,7 @@
 #include <cstdint>
 
 #include "common.cuh"
+#include "grid_index.cuh"
 #include "static_map.hpp"
 
 namespace b200 {
@@ -25,6 +26,21 @@ struct SmBox {
   int lo[3];
   unsigned dims[3];
 };
+
+// the linear index of voxel (x, y, z) in the box; false outside it (the differences in int64: voxel indices reach 2^30 + 2^14)
+__device__ __forceinline__ bool sm_lin(const SmBox& b, int x, int y, int z, unsigned* lin) {
+  const long long wx = (long long)x - b.lo[0], wy = (long long)y - b.lo[1], wz = (long long)z - b.lo[2];
+  if (wx < 0 || wy < 0 || wz < 0 || wx >= b.dims[0] || wy >= b.dims[1] || wz >= b.dims[2]) return false;
+  *lin = (unsigned)(((unsigned long long)wz * b.dims[1] + (unsigned long long)wy) * b.dims[0] + (unsigned long long)wx);
+  return true;
+}
+
+// the rank of an occupied voxel; false when it is outside the box or not occupied
+__device__ __forceinline__ bool sm_rank(const RankWord* __restrict__ index, const SmBox& b, int x, int y, int z, unsigned* r) {
+  unsigned lin;
+  if (!sm_lin(b, x, y, z, &lin)) return false;
+  return rank_probe(__ldg(reinterpret_cast<const uint2*>(index + (lin >> 5))), lin & 31u, *r);
+}
 
 // counters[] slots
 enum : int { SM_CTR_RAYS = 0, SM_CTR_SKIPPED, SM_CTR_DYNAMIC, SM_CTR_TRIPPED, SM_CTR_COUNT };

@@ -622,6 +622,71 @@ class ScanMatcher:
         self._check(self._lib.b200sm_save_static_map_pcd_ascii(self._h, os.fsencode(path), C.byref(n), C.byref(size)))
         return int(n.value), int(size.value)
 
+    # ---- map changes: what appeared and vanished between two recordings (b200sm_build_map_changes, csrc/map_changes.hpp) ----
+    UNCHANGED, APPEARED, VANISHED = 0, 1, 2
+
+    def buildMapChanges(self, poses=None, split_submap: int = -1, resolution: float = 0.2, max_range: float = 100.0,
+                        sensor_origin=(0.0, 0.0, 0.0), ray_fraction: float = 0.85, min_frees: int = 2,
+                        dynamic_thresh: float = 0.4) -> dict:
+        """What changed between the submaps before split_submap and those from it on (-1: the first submap of the last
+        segment, e.g. the recording mergeSession added), every submap at its own pose (poses None) or at `poses` (N, 4, 4).
+        The rays and parameters are buildStaticMap's; each voxel's hits and frees are counted per epoch, and a voxel
+        occupied in one epoch and free in the other APPEARED or VANISHED. Returns the build's info as a dict (box_origin,
+        box_dims, split_submap, n_rays, n_skipped, n_voxels, n_appeared_voxels, n_vanished_voxels, n_points,
+        n_appeared_points, n_vanished_points, n_updated_points, n_batches)."""
+        P = None
+        if poses is not None:
+            P = np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(self.numSubmaps(), 4, 4).transpose(0, 2, 1))
+        so = (C.c_double * 3)(*[float(v) for v in sensor_origin])
+        prm = _capi.SmStaticMapParams(float(resolution), float(max_range), so, float(ray_fraction), int(min_frees),
+                                      float(dynamic_thresh))
+        info = _capi.SmMapChangeInfo()
+        self._check(self._lib.b200sm_build_map_changes(self._h, _ptr(P) if P is not None else None, C.byref(prm), int(split_submap),
+                                                       C.byref(info)))
+        self._ch_sub = self.numSubmaps()
+        return _struct_dict(info)
+
+    def mapChanges(self) -> np.ndarray:
+        """The label of every point of the last build in map order (M,) uint8: UNCHANGED, APPEARED or VANISHED."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_get_map_changes(self._h, None, 0, C.byref(n)))
+        out = np.empty(max(n.value, 1), dtype=np.uint8)
+        self._check(self._lib.b200sm_get_map_changes(self._h, _ptr(out), n.value, C.byref(n)))
+        return out[:n.value]
+
+    def changeVoxels(self) -> dict:
+        """The occupied voxels of the last build in rank order: ijk (V, 3) int32, hits_before, frees_before, hits_after,
+        frees_after (V,) uint32, label (V,) uint8."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_get_change_voxels(self._h, None, None, None, None, None, None, 0, C.byref(n)))
+        V = n.value
+        out = dict(ijk=np.empty((max(V, 1), 3), dtype=np.int32), label=np.empty(max(V, 1), dtype=np.uint8))
+        for k in ("hits_before", "frees_before", "hits_after", "frees_after"):
+            out[k] = np.empty(max(V, 1), dtype=np.uint32)
+        self._check(self._lib.b200sm_get_change_voxels(self._h, *[_ptr(out[k]) for k in ("ijk", "hits_before", "frees_before",
+                                                                                       "hits_after", "frees_after", "label")],
+                                                        V, C.byref(n)))
+        return {k: v[:V] for k, v in out.items()}
+
+    def updatedMap(self, capacity=None):
+        """The last build's updated map (the assembled map without its VANISHED points): (cloud (M, 4) float32 in the
+        assembled map's order, offsets (N + 1,) int64 per submap, N the submaps at the build). capacity: copy at most that
+        many points."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_get_updated_map(self._h, None, 0, C.byref(n), None))
+        m = n.value if capacity is None else min(int(capacity), n.value)
+        offsets = np.zeros(getattr(self, "_ch_sub", 0) + 1, dtype=np.uint64)
+        out = np.empty((max(m, 1), 4), dtype=np.float32)
+        self._check(self._lib.b200sm_get_updated_map(self._h, _ptr(out), m, C.byref(n), _ptr(offsets)))
+        return out[:m], offsets.astype(np.int64)
+
+    def saveUpdatedMapPcd(self, path):
+        """pcl::io::savePCDFileASCII(path, updated map) of the last build: the prior map to localise in next time
+        (setPriorMapPcd). Returns (points, file bytes)."""
+        n, size = C.c_size_t(0), C.c_size_t(0)
+        self._check(self._lib.b200sm_save_updated_map_pcd_ascii(self._h, os.fsencode(path), C.byref(n), C.byref(size)))
+        return int(n.value), int(size.value)
+
     # ---- map consistency: neighbourhood entropy and plane variance (b200sm_build_map_consistency, csrc/map_consistency.hpp) ----
     def buildMapConsistency(self, poses=None, radius: float = 0.5, min_neighbors: int = 10, query_stride: int = 1) -> dict:
         """How crisp the map of every submap at its own pose (poses None) or at `poses` (N, 4, 4) is, built on the device:
