@@ -861,6 +861,53 @@ int b200sm_get_updated_map(b200sm_t s, float* out_xyzi, size_t capacity, size_t*
  * be NULL) = points and file size. No build yet, or an updated map without points (no file is created): B200REG_ERR_ARG.
  * A file that cannot be opened or written: B200REG_ERR_IO. */
 int b200sm_save_updated_map_pcd_ascii(b200sm_t s, const char* path, size_t* n_points, size_t* n_bytes);
+
+/* ---- surface mesh: a TSDF fused from every submap's rays, extracted by surface nets, saved as binary PLY --------------
+ * No counterpart in the reference. The rays are those of b200sm_build_static_map (its fixed point, origins and skip rule;
+ * the whole ray, no ray_fraction). Each ray walks a band of 2 * truncation around its endpoint through a voxel grid and
+ * adds to every voxel it crosses the signed distance from the voxel's centre to the endpoint along the ray (positive on
+ * the sensor's side, clamped to +-truncation) and one to its weight. A voxel with at least min_weight rays is observed; a
+ * cell of eight observed voxels whose signs differ gets one vertex (the mean of its edges' zero crossings), and every
+ * sign-changing edge between observed voxels whose four cells all have vertices gives two triangles, oriented so their
+ * normals point towards free space. The exact definitions are in csrc/mesh.hpp; DESIGN.md section 7b describes the build.
+ * Bitwise deterministic; the session's submaps, poses and other products are not changed. NDT and GICP sessions alike. */
+typedef struct b200sm_mesh_params {
+  double resolution;        /* metres per voxel, finite, > 0; default 0.2                                             */
+  double truncation;        /* metres, 1 <= truncation / resolution <= 16; default 0.6                                */
+  double max_range;         /* as b200sm_static_map_params.max_range: longer rays are not cast; default 100            */
+  double sensor_origin[3];  /* LiDAR position in the robot frame; default 0                                           */
+  unsigned min_weight;      /* rays a voxel needs to count as observed, >= 1; default 2                               */
+} b200sm_mesh_params;
+typedef struct b200sm_mesh_info {
+  int box_origin[3];                 /* lowest voxel of the band box: the endpoint voxels' box widened on every side   */
+  unsigned box_dims[3];
+  unsigned long long n_points;       /* the assembled map                                                             */
+  unsigned long long n_rays, n_skipped; /* points cast as rays / not cast (as the static map's)                        */
+  unsigned long long n_walked;       /* voxel visits of the band walks                                                */
+  unsigned long long n_band_voxels, n_observed_voxels; /* voxels some walk crosses; those with weight >= min_weight    */
+  unsigned long long n_vertices, n_faces;
+} b200sm_mesh_info;
+/* Build the mesh from every submap at its own pose (poses_colmajor16 NULL) or at the given 16 * n_submaps doubles (e.g.
+ * b200sm_pose_adjust's output). params NULL: the defaults. Refused with B200REG_ERR_ARG, the previous build staying
+ * readable: a parameter out of range, a non-finite pose, a sensor origin beyond 2^30 voxels, no submaps, a map of 2^32
+ * points or more, a band box of more than 2^31 - 1 voxels (all before anything is sized), and 2^32 faces or more (after
+ * they are counted). The session keeps the build until the next successful one or destroy, beside every other product:
+ * the rank index (8 bytes per 32 box voxels), 29 bytes per band voxel (voxel, sum, weight, flag, vertex id), 12 bytes per
+ * vertex and 12 per face, and 4 bytes per 256 band voxels of tile counts. info may be NULL. */
+int b200sm_build_mesh(b200sm_t s, const double* poses_colmajor16, const b200sm_mesh_params* params, b200sm_mesh_info* info);
+/* The last build's mesh: *n_vertices, *n_faces = its sizes; min(*n_vertices, vertex_capacity) vertices (x, y, z floats,
+ * map frame) and min(*n_faces, face_capacity) faces (three vertex ids each, counter-clockwise seen from free space) are
+ * copied (capacity 0: a size query). No build yet: B200REG_ERR_ARG. */
+int b200sm_get_mesh(b200sm_t s, float* xyz, size_t vertex_capacity, size_t* n_vertices, unsigned* faces3, size_t face_capacity,
+                    size_t* n_faces);
+/* The band voxels of the last build in rank order (ascending linear index in the box): *n = their number; min(*n,
+ * capacity) rows of each non-NULL array: ijk3 (3 ints), sdf_sum (the fused signed distances, 2^-16 voxel units), weight
+ * (rays). No build yet: B200REG_ERR_ARG. */
+int b200sm_get_mesh_voxels(b200sm_t s, int* ijk3, long long* sdf_sum, unsigned* weight, size_t capacity, size_t* n);
+/* The last build's mesh as binary little-endian PLY (csrc/mesh.hpp gives the bytes), written in pieces through pinned
+ * staging buffers. n_bytes (may be NULL) = the file size. No build yet, or a mesh without faces (no file is created):
+ * B200REG_ERR_ARG. A file that cannot be opened or written: B200REG_ERR_IO. */
+int b200sm_save_mesh_ply(b200sm_t s, const char* path, size_t* n_bytes);
 /* The same text for a HOST PointXYZI cloud (records as in b200sm_import_submap; intensity_offset_bytes >= 0), formatted
  * on `device`. *n_bytes = size of the whole file content (header and data); min(*n_bytes, capacity) bytes are copied to
  * out, so capacity 0 is a size query. B200REG_ERR_ARG for n == 0, a negative intensity offset, or a stride or offset that

@@ -663,6 +663,37 @@ class ScanMatcherSession {
   }
   // PCL's ASCII PCD of the last updated map: the prior map for setPriorMapPcd next time
   void saveUpdatedMapPcd(const std::string& path) { check(b200sm_save_updated_map_pcd_ascii(s_.get(), path.c_str(), nullptr, nullptr)); }
+
+  // ---- surface mesh (b200sm_build_mesh): a TSDF of every submap's rays, extracted by surface nets; poses empty = the
+  // submaps' own; p nullptr = the defaults
+  b200sm_mesh_info buildMesh(const std::vector<double>& poses_colmajor16 = {}, const b200sm_mesh_params* p = nullptr) {
+    b200sm_mesh_info info{};
+    check(b200sm_build_mesh(s_.get(), poses_colmajor16.empty() ? nullptr : poses_colmajor16.data(), p, &info));
+    return info;
+  }
+  // the last mesh: x y z per vertex (map frame), three vertex ids per face (counter-clockwise seen from free space)
+  void mesh(std::vector<float>& xyz, std::vector<unsigned>& faces3) {
+    size_t nv = 0, nf = 0;
+    check(b200sm_get_mesh(s_.get(), nullptr, 0, &nv, nullptr, 0, &nf));
+    xyz.resize(3 * nv);
+    faces3.resize(3 * nf);
+    check(b200sm_get_mesh(s_.get(), xyz.data(), nv, &nv, faces3.data(), nf, &nf));
+  }
+  // the last build's band voxels in rank order: 3 ints each, the fused signed-distance sum and the ray count
+  void meshVoxels(std::vector<int>& ijk3, std::vector<long long>& sdf_sum, std::vector<unsigned>& weight) {
+    size_t n = 0;
+    check(b200sm_get_mesh_voxels(s_.get(), nullptr, nullptr, nullptr, 0, &n));
+    ijk3.resize(3 * n);
+    sdf_sum.resize(n);
+    weight.resize(n);
+    check(b200sm_get_mesh_voxels(s_.get(), ijk3.data(), sdf_sum.data(), weight.data(), n, &n));
+  }
+  // the last mesh as binary PLY; returns the file's bytes
+  size_t saveMeshPly(const std::string& path) {
+    size_t n = 0;
+    check(b200sm_save_mesh_ply(s_.get(), path.c_str(), &n));
+    return n;
+  }
   b200sm_localize_stats localizeStats() const {
     b200sm_localize_stats st{};
     check(b200sm_get_localize_stats(s_.get(), &st));

@@ -57,6 +57,7 @@ SYMBOLS = [
     "b200sm_save_map_consistency_pcd_ascii",
     "b200sm_build_map_changes", "b200sm_get_map_changes", "b200sm_get_change_voxels", "b200sm_get_updated_map",
     "b200sm_save_updated_map_pcd_ascii",
+    "b200sm_build_mesh", "b200sm_get_mesh", "b200sm_get_mesh_voxels", "b200sm_save_mesh_ply",
     "b200sm_merge_session", "b200sm_get_merge_scores", "b200sm_get_segments",
     "b200sm_save_session", "b200sm_load_session", "b200sm_get_session_graph",
     # include/b200comm.h
@@ -131,6 +132,17 @@ class SmStaticMapInfo(C.Structure):
     _fields_ = [("box_origin", C.c_int * 3), ("box_dims", C.c_uint * 3), ("n_rays", C.c_ulonglong), ("n_skipped", C.c_ulonglong),
                 ("n_voxels", C.c_ulonglong), ("n_dynamic_voxels", C.c_ulonglong), ("n_points", C.c_ulonglong),
                 ("n_static_points", C.c_ulonglong), ("n_batches", C.c_int)]
+
+
+class SmMeshParams(C.Structure):
+    _fields_ = [("resolution", C.c_double), ("truncation", C.c_double), ("max_range", C.c_double),
+                ("sensor_origin", C.c_double * 3), ("min_weight", C.c_uint)]
+
+
+class SmMeshInfo(C.Structure):
+    _fields_ = [("box_origin", C.c_int * 3), ("box_dims", C.c_uint * 3), ("n_points", C.c_ulonglong), ("n_rays", C.c_ulonglong),
+                ("n_skipped", C.c_ulonglong), ("n_walked", C.c_ulonglong), ("n_band_voxels", C.c_ulonglong),
+                ("n_observed_voxels", C.c_ulonglong), ("n_vertices", C.c_ulonglong), ("n_faces", C.c_ulonglong)]
 
 
 class SmMapChangeInfo(C.Structure):
@@ -383,6 +395,10 @@ def lib() -> C.CDLL:
     L.b200sm_get_change_voxels.argtypes = [vp, vp, vp, vp, vp, vp, vp, sz, C.POINTER(sz)]
     L.b200sm_get_updated_map.argtypes = [vp, vp, sz, C.POINTER(sz), vp]
     L.b200sm_save_updated_map_pcd_ascii.argtypes = [vp, C.c_char_p, C.POINTER(sz), C.POINTER(sz)]
+    L.b200sm_build_mesh.argtypes = [vp, vp, C.POINTER(SmMeshParams), C.POINTER(SmMeshInfo)]
+    L.b200sm_get_mesh.argtypes = [vp, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]
+    L.b200sm_get_mesh_voxels.argtypes = [vp, vp, vp, vp, sz, C.POINTER(sz)]
+    L.b200sm_save_mesh_ply.argtypes = [vp, C.c_char_p, C.POINTER(sz)]
     L.b200sm_merge_session.argtypes = [vp, vp, vp, C.POINTER(SmMergeParams), vp, i, vp, sz, C.POINTER(sz), vp,
                                         C.POINTER(SmMergeResult)]
     L.b200sm_get_merge_scores.argtypes = [vp, sz, C.POINTER(sz), C.POINTER(sz), vp, vp]

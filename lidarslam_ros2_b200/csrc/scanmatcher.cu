@@ -45,6 +45,7 @@
 #include "engine.hpp"
 #include "global_grid.hpp"
 #include "map_changes.cuh"
+#include "mesh.cuh"
 #include "map_cut.hpp"
 #include "occupancy.cuh"
 #include "place_recognition.cuh"
@@ -291,6 +292,17 @@ struct MapChanges {
   std::vector<size_t> offsets;  // n_submaps at the build + 1
 };
 
+// One mesh build (b200sm_build_mesh): the rank index over its band box, the band voxels (ijk, sum, weight in rank order),
+// the vertices and the faces.
+struct MeshBuild {
+  DeviceBuffer<RankWord> index;
+  DeviceBuffer<int> ijk;
+  DeviceBuffer<unsigned long long> sum;
+  DeviceBuffer<uint32_t> weight, faces;
+  DeviceBuffer<float> xyz;
+  b200sm_mesh_info info{};
+};
+
 struct b200sm_session {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -437,6 +449,16 @@ struct b200sm_session {
   DeviceBuffer<unsigned long long> ch_counters;
   DeviceBuffer<unsigned> ch_map_first, ch_tiles, ch_tiles_tmp;
   std::unique_ptr<MapChanges> ch;
+  // surface mesh (b200sm_build_mesh): the per-call table, bounds and counters, the per-call workspace of K21c-e (ACTIVE
+  // flags, vertex ids, tile counts and the scans' scratch), and the last build, kept until the next build succeeds
+  DeviceBuffer<SmEntry> ms_table;
+  DeviceBuffer<int> ms_bounds;
+  DeviceBuffer<unsigned long long> ms_counters;
+  DeviceBuffer<unsigned char> ms_active;
+  DeviceBuffer<uint32_t> ms_vid;
+  DeviceBuffer<unsigned> ms_vcounts, ms_fcounts, ms_tiles_tmp;
+  RankIndexScratch ms_scan;
+  std::unique_ptr<MeshBuild> ms;
 };
 
 namespace {
@@ -3414,6 +3436,271 @@ int b200sm_save_updated_map_pcd_ascii(b200sm_t s, const char* path, size_t* n_po
   const size_t total = (size_t)s->ch->info.n_updated_points;
   if (total == 0) return sm_fail(s, B200REG_ERR_ARG, "save_updated_map_pcd_ascii: the updated map has no points");
   return sm_guarded(s, [&]() { return write_pcd_ascii(s, s->ch->updated.ptr, total, path, "save_updated_map_pcd_ascii", n_points, n_bytes); });
+}
+
+}  // extern "C"
+
+// ---- surface mesh: a TSDF fused from every submap's rays, extracted by surface nets, saved as PLY (csrc/mesh.hpp,
+// csrc/mesh.cu, and the static map's rays and bounds) ----
+namespace {
+
+MsParams ms_params_from(const b200sm_mesh_params* p) {
+  MsParams q;
+  if (p) {
+    q.resolution = p->resolution;
+    q.truncation = p->truncation;
+    q.max_range = p->max_range;
+    for (int k = 0; k < 3; k++) q.sensor_origin[k] = p->sensor_origin[k];
+    q.min_weight = p->min_weight;
+  }
+  return q;
+}
+
+constexpr size_t MS_PLY_PIECE = 1u << 20;  // vertices or faces per piece of the PLY write (12 MiB of staging)
+
+}  // namespace
+
+extern "C" {
+
+int b200sm_build_mesh(b200sm_t s, const double* poses_colmajor16, const b200sm_mesh_params* params, b200sm_mesh_info* info) {
+  if (!s) return B200REG_ERR_ARG;
+  const MsParams p = ms_params_from(params);
+  MsConst c;
+  if (const char* why = ms_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_mesh: ") + why).c_str());
+  const size_t n_sub = s->submaps.size();
+  if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_mesh: the session has no submaps");
+  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, "build_mesh: a non-finite pose entry");
+  SubmapTiles t;
+  const int rc = submap_tiles(s, 0, SM_TILE, true, "build_mesh: a submap of 2^32 points or more", "build_mesh: too many points for one launch",
+                              &t);
+  if (rc != B200REG_OK) return rc;
+  const unsigned long long tiles = t.tiles;
+  std::vector<SmEntry> table;
+  unsigned long long total = 0;
+  for (size_t k = 0; k < n_sub; k++) {
+    const Submap& sub = *s->submaps[k];
+    SmEntry e;
+    std::memset(&e, 0, sizeof(e));
+    submap_pose_f(s, k, poses_colmajor16, e.T);
+    if (!ms_origin(c, p, e.T, e.o)) {
+      s->err = "build_mesh: the sensor origin of submap " + std::to_string(k) + " lies beyond 2^30 voxels";
+      return (int)B200REG_ERR_ARG;
+    }
+    total += sub.n;
+    if (sub.n == 0) continue;
+    e.cloud = sub.cloud;
+    e.n = (unsigned)sub.n;
+    e.first_tile = t.first_tile[table.size()];
+    table.push_back(e);
+  }
+  if (total > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_mesh: a map of 2^32 points or more");
+  const int n_entries = (int)table.size();
+  return sm_guarded(s, [&]() {
+    // the new build is made beside the last one, which stays until this one succeeds
+    auto m = std::make_unique<MeshBuild>();
+    unsigned long long ctr[MS_CTR_COUNT] = {};
+    s->ms_counters.ensure(MS_CTR_COUNT);
+    B200_CUDA(cudaMemsetAsync(s->ms_counters.ptr, 0, sizeof(ctr), s->stream));
+    // K15a: the endpoint voxels' bounds and the ray counts, one read-back
+    std::vector<int> bounds(6 * table.size());
+    for (size_t r = 0; r < table.size(); r++)
+      for (int a = 0; a < 3; a++) {
+        bounds[6 * r + a] = INT_MAX;
+        bounds[6 * r + 3 + a] = INT_MIN;
+      }
+    if (n_entries) {
+      s->ms_table.ensure(table.size());
+      s->ms_bounds.ensure(bounds.size());
+      B200_CUDA(cudaMemcpyAsync(s->ms_table.ptr, table.data(), table.size() * sizeof(SmEntry), cudaMemcpyHostToDevice, s->stream));
+      B200_CUDA(cudaMemcpyAsync(s->ms_bounds.ptr, bounds.data(), bounds.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
+      sm_bounds_launch(s->ms_table.ptr, n_entries, (unsigned)tiles, c.sm, s->ms_bounds.ptr, s->ms_counters.ptr, s->stream);
+      s->launches += 1;
+      B200_CUDA(cudaMemcpyAsync(bounds.data(), s->ms_bounds.ptr, bounds.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+    }
+    B200_CUDA(cudaMemcpyAsync(ctr, s->ms_counters.ptr, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
+    for (size_t r = 0; r < table.size(); r++)
+      for (int a = 0; a < 3; a++) {
+        lo[a] = std::min(lo[a], bounds[6 * r + a]);
+        hi[a] = std::max(hi[a], bounds[6 * r + 3 + a]);
+      }
+    const bool any_ray = ctr[SM_CTR_RAYS] > 0;
+    SmBox box{};
+    unsigned long long cells = 0;
+    if (any_ray && !ms_box(lo, hi, c.r, box.lo, box.dims, &cells)) {
+      s->err = "build_mesh: a band box of " + std::to_string((long long)hi[0] - lo[0] + 1 + 2 * c.r) + " x " +
+               std::to_string((long long)hi[1] - lo[1] + 1 + 2 * c.r) + " x " + std::to_string((long long)hi[2] - lo[2] + 1 + 2 * c.r) +
+               " voxels exceeds 2^31 - 1 voxels";
+      return (int)B200REG_ERR_ARG;
+    }
+    const unsigned long long n_words = (cells + 31) / 32;
+    unsigned n_band = 0;
+    if (any_ray) {
+      // K21a: the band walks into the rank index, then the number of band voxels
+      m->index.ensure((size_t)n_words);
+      rank_index_clear(m->index.ptr, (int)n_words, s->stream);
+      ms_mark_launch(s->ms_table.ptr, n_entries, (unsigned)tiles, c, box, m->index.ptr, s->ms_counters.ptr, s->stream);
+      s->ms_scan.total.ensure(1);
+      rank_index_scan_async(m->index.ptr, (size_t)n_words, s->ms_scan, s->ms_scan.total.ptr, s->stream);
+      s->launches += 3;
+      B200_CUDA(cudaMemcpyAsync(&n_band, s->ms_scan.total.ptr, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaStreamSynchronize(s->stream));
+    }
+    const size_t nb = std::max<size_t>(n_band, 1);
+    m->sum.ensure(nb);
+    m->weight.ensure(nb);
+    m->ijk.ensure(3 * nb);
+    B200_CUDA(cudaMemsetAsync(m->sum.ptr, 0, nb * sizeof(unsigned long long), s->stream));
+    B200_CUDA(cudaMemsetAsync(m->weight.ptr, 0, nb * sizeof(uint32_t), s->stream));
+    unsigned n_vert = 0;
+    std::vector<unsigned> vtile;
+    const unsigned vtiles = (n_band + MS_THREADS - 1) / MS_THREADS;
+    if (n_band > 0) {
+      // K21b, the voxel list, K21c and its scan: the vertex count
+      ms_fuse_launch(s->ms_table.ptr, n_entries, (unsigned)tiles, c, box, m->index.ptr, n_band, m->sum.ptr, m->weight.ptr,
+                     s->ms_counters.ptr, s->stream);
+      sm_voxel_list_launch(m->index.ptr, n_words, box, n_band, m->ijk.ptr, s->stream);
+      s->ms_active.ensure(n_band);
+      s->ms_vcounts.ensure((size_t)vtiles + 1);
+      ms_active_launch(m->ijk.ptr, m->sum.ptr, m->weight.ptr, m->index.ptr, box, n_band, c.min_weight, s->ms_active.ptr,
+                       s->ms_vcounts.ptr, s->ms_counters.ptr, s->stream);
+      counter_scan_async(s->ms_vcounts.ptr, vtiles, s->ms_tiles_tmp, s->stream);
+      s->launches += 5;
+      B200_CUDA(cudaMemcpyAsync(&n_vert, s->ms_vcounts.ptr + vtiles, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaStreamSynchronize(s->stream));
+    }
+    m->xyz.ensure(3 * std::max<size_t>(n_vert, 1));
+    if (n_band > 0) {
+      // K21d and its scan: the vertices, and the face count read back with the counters
+      s->ms_vid.ensure(n_band);
+      s->ms_fcounts.ensure((size_t)vtiles + 1);
+      ms_vertex_launch(m->ijk.ptr, m->sum.ptr, m->weight.ptr, m->index.ptr, box, n_band, c, s->ms_active.ptr, s->ms_vcounts.ptr, n_vert,
+                       s->ms_vid.ptr, m->xyz.ptr, s->ms_fcounts.ptr, s->ms_counters.ptr, s->stream);
+      counter_scan_async(s->ms_fcounts.ptr, vtiles, s->ms_tiles_tmp, s->stream);
+      s->launches += 3;
+    }
+    B200_CUDA(cudaMemcpyAsync(ctr, s->ms_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    if (ctr[MS_CTR_FACES] > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_mesh: 2^32 faces or more");
+    const unsigned n_faces = (unsigned)ctr[MS_CTR_FACES];
+    m->faces.ensure(3 * std::max<size_t>(n_faces, 1));
+    if (n_faces > 0) {
+      // K21e
+      ms_face_launch(m->ijk.ptr, m->sum.ptr, m->weight.ptr, m->index.ptr, box, n_band, c.min_weight, s->ms_vid.ptr, s->ms_fcounts.ptr,
+                     n_faces, m->faces.ptr, s->ms_counters.ptr, s->stream);
+      s->launches += 1;
+      B200_CUDA(cudaMemcpyAsync(ctr, s->ms_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    }
+    B200_CUDA(cudaStreamSynchronize(s->stream));  // the host table goes out of scope; the counts are read
+    if (ctr[SM_CTR_TRIPPED])
+      return sm_fail(s, B200REG_ERR_CUDA, "build_mesh: a voxel outside the box or beyond the rank index, or a vertex or face beyond its count");
+    b200sm_mesh_info& I = m->info;
+    for (int a = 0; a < 3; a++) {
+      I.box_origin[a] = any_ray ? box.lo[a] : 0;
+      I.box_dims[a] = any_ray ? box.dims[a] : 0;
+    }
+    I.n_points = total;
+    I.n_rays = ctr[SM_CTR_RAYS];
+    I.n_skipped = ctr[SM_CTR_SKIPPED];
+    I.n_walked = ctr[MS_CTR_WALKED];
+    I.n_band_voxels = n_band;
+    I.n_observed_voxels = ctr[MS_CTR_OBSERVED];
+    I.n_vertices = n_vert;
+    I.n_faces = n_faces;
+    if (info) *info = I;
+    s->ms = std::move(m);
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_mesh(b200sm_t s, float* xyz, size_t vertex_capacity, size_t* n_vertices, unsigned* faces3, size_t face_capacity,
+                    size_t* n_faces) {
+  if (!s || (!xyz && vertex_capacity) || (!faces3 && face_capacity)) return B200REG_ERR_ARG;
+  if (!s->ms) return sm_fail(s, B200REG_ERR_ARG, "get_mesh: no mesh has been built");
+  return sm_guarded(s, [&]() {
+    const MeshBuild& m = *s->ms;
+    if (n_vertices) *n_vertices = (size_t)m.info.n_vertices;
+    if (n_faces) *n_faces = (size_t)m.info.n_faces;
+    const size_t kv = std::min(vertex_capacity, (size_t)m.info.n_vertices), kf = std::min(face_capacity, (size_t)m.info.n_faces);
+    if (kv) B200_CUDA(cudaMemcpyAsync(xyz, m.xyz.ptr, 3 * kv * sizeof(float), cudaMemcpyDeviceToHost, s->stream));
+    if (kf) B200_CUDA(cudaMemcpyAsync(faces3, m.faces.ptr, 3 * kf * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+    if (kv || kf) B200_CUDA(cudaStreamSynchronize(s->stream));
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_mesh_voxels(b200sm_t s, int* ijk3, long long* sdf_sum, unsigned* weight, size_t capacity, size_t* n) {
+  if (!s) return B200REG_ERR_ARG;
+  if (!s->ms) return sm_fail(s, B200REG_ERR_ARG, "get_mesh_voxels: no mesh has been built");
+  return sm_guarded(s, [&]() {
+    const MeshBuild& m = *s->ms;
+    const size_t nb = (size_t)m.info.n_band_voxels;
+    if (n) *n = nb;
+    const size_t k = std::min(capacity, nb);
+    if (k == 0) return (int)B200REG_OK;
+    if (ijk3) B200_CUDA(cudaMemcpyAsync(ijk3, m.ijk.ptr, 3 * k * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+    if (sdf_sum) B200_CUDA(cudaMemcpyAsync(sdf_sum, m.sum.ptr, k * sizeof(long long), cudaMemcpyDeviceToHost, s->stream));
+    if (weight) B200_CUDA(cudaMemcpyAsync(weight, m.weight.ptr, k * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_save_mesh_ply(b200sm_t s, const char* path, size_t* n_bytes) {
+  if (!s || !path) return B200REG_ERR_ARG;
+  if (!s->ms) return sm_fail(s, B200REG_ERR_ARG, "save_mesh_ply: no mesh has been built");
+  const MeshBuild& m = *s->ms;
+  const size_t V = (size_t)m.info.n_vertices, F = (size_t)m.info.n_faces;
+  if (F == 0) return sm_fail(s, B200REG_ERR_ARG, "save_mesh_ply: the mesh has no faces");
+  return sm_guarded(s, [&]() {
+    const std::string header = "ply\nformat binary_little_endian 1.0\nelement vertex " + std::to_string(V) +
+                               "\nproperty float x\nproperty float y\nproperty float z\nelement face " + std::to_string(F) +
+                               "\nproperty list uchar uint vertex_indices\nend_header\n";
+    if (n_bytes) *n_bytes = header.size() + 12 * V + 13 * F;
+    FILE* fp = std::fopen(path, "wb");
+    if (!fp) {
+      s->err = std::string("save_mesh_ply: cannot open ") + path + ": " + std::strerror(errno);
+      return (int)B200REG_ERR_IO;
+    }
+    // pieces: the vertices, then the faces, MS_PLY_PIECE records each (12 bytes on the device either way)
+    const size_t vp = (V + MS_PLY_PIECE - 1) / MS_PLY_PIECE, fpieces = (F + MS_PLY_PIECE - 1) / MS_PLY_PIECE, n = vp + fpieces;
+    auto span = [&](size_t piece, size_t* first, size_t* count) {
+      const bool face = piece >= vp;
+      const size_t q = face ? piece - vp : piece, all = face ? F : V;
+      *first = q * MS_PLY_PIECE;
+      *count = std::min(MS_PLY_PIECE, all - *first);
+      return face;
+    };
+    auto enqueue = [&](size_t piece, char* buf) {
+      size_t first, count;
+      const void* src = span(piece, &first, &count) ? (const void*)(m.faces.ptr + 3 * first) : (const void*)(m.xyz.ptr + 3 * first);
+      B200_CUDA(cudaMemcpyAsync(buf, src, 12 * count, cudaMemcpyDeviceToHost, s->stream));
+    };
+    std::vector<unsigned char> rec;
+    auto write = [&](size_t piece, const char* buf) {
+      size_t first, count;
+      bool ok = piece > 0 || std::fwrite(header.data(), 1, header.size(), fp) == header.size();
+      if (span(piece, &first, &count)) {
+        rec.resize(13 * count);  // a 0x03 byte, then the three little-endian ids
+        for (size_t f = 0; f < count; f++) {
+          rec[13 * f] = 3;
+          std::memcpy(&rec[13 * f + 1], buf + 12 * f, 12);
+        }
+        ok = ok && std::fwrite(rec.data(), 1, rec.size(), fp) == rec.size();
+      } else {
+        ok = ok && std::fwrite(buf, 1, 12 * count, fp) == 12 * count;
+      }
+      if (ok && piece + 1 == n) {
+        ok = std::fclose(fp) == 0;
+        fp = nullptr;
+      }
+      if (ok) return (int)B200REG_OK;
+      s->err = std::string("save_mesh_ply: writing ") + path + ": " + std::strerror(errno);
+      return (int)B200REG_ERR_IO;
+    };
+    return write_staged(s, n, 12 * MS_PLY_PIECE, fp, enqueue, write);
+  });
 }
 
 }  // extern "C"

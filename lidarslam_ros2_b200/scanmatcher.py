@@ -687,6 +687,52 @@ class ScanMatcher:
         self._check(self._lib.b200sm_save_updated_map_pcd_ascii(self._h, os.fsencode(path), C.byref(n), C.byref(size)))
         return int(n.value), int(size.value)
 
+    # ---- surface mesh: a TSDF of the submaps' rays, extracted by surface nets (b200sm_build_mesh, csrc/mesh.hpp) ----
+    def buildMesh(self, poses=None, resolution: float = 0.2, truncation: float = 0.6, max_range: float = 100.0,
+                  sensor_origin=(0.0, 0.0, 0.0), min_weight: int = 2) -> dict:
+        """The surface mesh of every submap at its own pose (poses None) or at `poses` (N, 4, 4), built on the device: each
+        ray fuses its signed distance into the voxels within `truncation` of its endpoint, and surface nets extracts the
+        zero crossing of the voxels at least `min_weight` rays observed. Returns the build's info as a dict (box_origin,
+        box_dims, n_points, n_rays, n_skipped, n_walked, n_band_voxels, n_observed_voxels, n_vertices, n_faces)."""
+        P = None
+        if poses is not None:
+            P = np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(self.numSubmaps(), 4, 4).transpose(0, 2, 1))
+        so = (C.c_double * 3)(*[float(v) for v in sensor_origin])
+        prm = _capi.SmMeshParams(float(resolution), float(truncation), float(max_range), so, int(min_weight))
+        info = _capi.SmMeshInfo()
+        self._check(self._lib.b200sm_build_mesh(self._h, _ptr(P) if P is not None else None, C.byref(prm), C.byref(info)))
+        return _struct_dict(info)
+
+    def mesh(self):
+        """The last build's mesh: (vertices (V, 3) float32 in the map frame, faces (F, 3) uint32, counter-clockwise seen
+        from free space)."""
+        nv, nf = C.c_size_t(0), C.c_size_t(0)
+        self._check(self._lib.b200sm_get_mesh(self._h, None, 0, C.byref(nv), None, 0, C.byref(nf)))
+        V, F = nv.value, nf.value
+        xyz = np.empty((max(V, 1), 3), dtype=np.float32)
+        faces = np.empty((max(F, 1), 3), dtype=np.uint32)
+        self._check(self._lib.b200sm_get_mesh(self._h, _ptr(xyz), V, C.byref(nv), _ptr(faces), F, C.byref(nf)))
+        return xyz[:V], faces[:F]
+
+    def meshVoxels(self) -> dict:
+        """The last build's band voxels in rank order: ijk (B, 3) int32, sdf_sum (B,) int64 (2^-16 voxel units), weight (B,)
+        uint32."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_get_mesh_voxels(self._h, None, None, None, 0, C.byref(n)))
+        B = n.value
+        out = dict(ijk=np.empty((max(B, 1), 3), dtype=np.int32), sdf_sum=np.empty(max(B, 1), dtype=np.int64),
+                   weight=np.empty(max(B, 1), dtype=np.uint32))
+        self._check(self._lib.b200sm_get_mesh_voxels(self._h, _ptr(out["ijk"]), _ptr(out["sdf_sum"]), _ptr(out["weight"]), B,
+                                                     C.byref(n)))
+        return {k: v[:B] for k, v in out.items()}
+
+    def saveMeshPly(self, path) -> int:
+        """The last build's mesh as binary little-endian PLY (MeshLab, CloudCompare, Open3D, Blender). Returns the file's
+        bytes."""
+        size = C.c_size_t(0)
+        self._check(self._lib.b200sm_save_mesh_ply(self._h, os.fsencode(path), C.byref(size)))
+        return int(size.value)
+
     # ---- map consistency: neighbourhood entropy and plane variance (b200sm_build_map_consistency, csrc/map_consistency.hpp) ----
     def buildMapConsistency(self, poses=None, radius: float = 0.5, min_neighbors: int = 10, query_stride: int = 1) -> dict:
         """How crisp the map of every submap at its own pose (poses None) or at `poses` (N, 4, 4) is, built on the device:
