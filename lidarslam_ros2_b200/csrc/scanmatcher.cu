@@ -253,6 +253,32 @@ using namespace b200;
 extern "C" int b200reg_adopt_source_device(b200reg_t h, const void* dev, size_t n);  // capi.cu (library-internal)
 extern "C" float b200reg_last_score_ms(b200reg_t h);                                 // capi.cu (library-internal)
 
+// The occupancy grid (b200sm_build_occupancy_grid): hits, frees, values and trinary image per cell. Its next build
+// overwrites it in place.
+struct OccupancyGrid {
+  DeviceBuffer<uint32_t> hits, frees;
+  DeviceBuffer<signed char> values;
+  DeviceBuffer<unsigned char> image;
+  bool built = false;
+  OgParams params;
+  unsigned width = 0, height = 0;
+  double origin[2] = {0, 0};
+};
+
+// The static map (b200sm_build_static_map): the rank index over its box, hits, frees and flags per occupied voxel, and the
+// static map with its per-submap offsets. Its next build overwrites it in place.
+struct StaticMap {
+  DeviceBuffer<RankWord> index;
+  DeviceBuffer<uint32_t> hits, frees;
+  DeviceBuffer<unsigned char> dynamic;
+  DeviceBuffer<float4> points;
+  bool built = false;
+  SmBox box{};
+  unsigned long long n_words = 0;
+  b200sm_static_map_info info{};
+  std::vector<size_t> offsets;  // n_submaps at the build + 1
+};
+
 // One elevation map (b200sm_build_elevation_map): its layers on the device, its parameters and its info.
 struct ElevationMap {
   DeviceBuffer<uint32_t> n;
@@ -301,6 +327,29 @@ struct MeshBuild {
   DeviceBuffer<uint32_t> weight, faces;
   DeviceBuffer<float> xyz;
   b200sm_mesh_info info{};
+};
+
+// The per-call workspace of the six map builds and of the voxel-list read-backs, buffers named by role and shared by the
+// builds that use one of the same type for the same role. Nothing in it outlives the call that filled it: no read-back
+// reads what a build left here.
+struct MapWorkspace {
+  DeviceBuffer<OgEntry> og_table;  // the occupancy grid's and the elevation map's table
+  DeviceBuffer<SmEntry> sm_table;  // the static map's, the map changes' and the mesh's
+  DeviceBuffer<McEntry> mc_table;  // the map consistency's
+  DeviceBuffer<int> bounds;        // the bounds pass's per-entry bounds
+  DeviceBuffer<unsigned long long> counters;
+  DeviceBuffer<uint32_t> bitmaps;  // a walk batch's hit and free bitmaps
+  RankIndexScratch rank_scan;      // the rank pass's scan
+  DeviceBuffer<unsigned> tiles;    // kept points per tile, scanned into tile offsets
+  DeviceBuffer<unsigned> scan_tmp;  // counter_scan_async's tile sums
+  DeviceBuffer<unsigned> map_first;  // map changes: each entry's first map index
+  DeviceBuffer<long long> zrange;    // elevation map: the height extent
+  DeviceBuffer<ushort4> cell_offs;   // map consistency: the points in cell order
+  DeviceBuffer<unsigned> cell_idx;
+  DeviceBuffer<unsigned char> active;  // mesh: ACTIVE flags, vertex ids, and vertex and face counts per tile
+  DeviceBuffer<uint32_t> vertex_id;
+  DeviceBuffer<unsigned> vertex_counts, face_counts;
+  DeviceBuffer<int> ijk;  // get_map_voxels / get_change_voxels: the voxel list
 };
 
 struct b200sm_session {
@@ -395,70 +444,15 @@ struct b200sm_session {
   DeviceBuffer<double> merge_dist, merge_sel_d;
   DeviceBuffer<int> merge_shift, merge_sel_a, merge_sel_s;
   size_t merge_nq = 0, merge_nc = 0;
-  // occupancy grid (b200sm_build_occupancy_grid): the per-call table, bounds and counters, the walks' bitmap scratch, and
-  // the last grid built (hits, frees, values, trinary image), kept until the next build
-  DeviceBuffer<OgEntry> og_table;
-  DeviceBuffer<int> og_bounds;
-  DeviceBuffer<unsigned long long> og_counters;
-  DeviceBuffer<uint32_t> og_scratch, og_hits, og_frees;
-  DeviceBuffer<signed char> og_values;
-  DeviceBuffer<unsigned char> og_image;
-  bool og_built = false;
-  OgParams og_params;
-  unsigned og_width = 0, og_height = 0;
-  double og_origin[2] = {0, 0};
-  // elevation map (b200sm_build_elevation_map): the per-call table, bounds, counters and height extent, and the last map
-  // built, kept until the next build succeeds
-  DeviceBuffer<OgEntry> el_table;
-  DeviceBuffer<int> el_bounds;
-  DeviceBuffer<unsigned long long> el_counters;
-  DeviceBuffer<long long> el_zrange;
+  // the map products built from the session's map. The occupancy grid and the static map are kept until their next build
+  // overwrites them; the other four are built beside the last one, which stays until the new one succeeds.
+  OccupancyGrid og;
   std::unique_ptr<ElevationMap> el;
-  // static map (b200sm_build_static_map): the per-call table, bounds, counters and tile counts, the walks' bitmap scratch,
-  // and the last build (rank index over the box, hits, frees and flags per occupied voxel, the static map), kept until
-  // the next build
-  DeviceBuffer<SmEntry> sm_table;
-  DeviceBuffer<int> sm_bounds;
-  DeviceBuffer<unsigned long long> sm_counters;
-  DeviceBuffer<unsigned> sm_tiles, sm_tiles_tmp;
-  DeviceBuffer<uint32_t> sm_scratch, sm_hits, sm_frees;
-  DeviceBuffer<unsigned char> sm_dynamic;
-  DeviceBuffer<RankWord> sm_index;
-  RankIndexScratch sm_scan;
-  DeviceBuffer<float4> sm_static;
-  DeviceBuffer<int> sm_ijk;
-  bool sm_built = false;
-  SmBox sm_box{};
-  unsigned long long sm_words = 0;
-  b200sm_static_map_info sm_info{};
-  std::vector<size_t> sm_offsets;  // n_submaps at the build + 1
-  // map consistency (b200sm_build_map_consistency): the per-call table, bounds and counters, the cell-ordered scratch of
-  // K19b / K19c, the scans' tile sums, and the last build, kept until the next build succeeds
-  DeviceBuffer<McEntry> mc_table;
-  DeviceBuffer<int> mc_bounds;
-  DeviceBuffer<unsigned long long> mc_counters;
-  DeviceBuffer<ushort4> mc_offs;
-  DeviceBuffer<unsigned> mc_idx, mc_tmp;
-  RankIndexScratch mc_scan;
-  std::unique_ptr<MapConsistency> mc;
-  // map changes (b200sm_build_map_changes): the per-call table, bounds, counters, first map index per entry and tile
-  // counts, the voxel list of the read-back, and the last build, kept until the next build succeeds. The walks' bitmap
-  // scratch and the rank scan's scratch are the static map's: per-call workspace that no read-back uses.
-  DeviceBuffer<SmEntry> ch_table;
-  DeviceBuffer<int> ch_bounds, ch_ijk;
-  DeviceBuffer<unsigned long long> ch_counters;
-  DeviceBuffer<unsigned> ch_map_first, ch_tiles, ch_tiles_tmp;
+  StaticMap sm;
   std::unique_ptr<MapChanges> ch;
-  // surface mesh (b200sm_build_mesh): the per-call table, bounds and counters, the per-call workspace of K21c-e (ACTIVE
-  // flags, vertex ids, tile counts and the scans' scratch), and the last build, kept until the next build succeeds
-  DeviceBuffer<SmEntry> ms_table;
-  DeviceBuffer<int> ms_bounds;
-  DeviceBuffer<unsigned long long> ms_counters;
-  DeviceBuffer<unsigned char> ms_active;
-  DeviceBuffer<uint32_t> ms_vid;
-  DeviceBuffer<unsigned> ms_vcounts, ms_fcounts, ms_tiles_tmp;
-  RankIndexScratch ms_scan;
   std::unique_ptr<MeshBuild> ms;
+  std::unique_ptr<MapConsistency> mc;
+  MapWorkspace work;
 };
 
 namespace {
@@ -2530,6 +2524,164 @@ int b200sm_get_session_graph(b200sm_t s, b200sm_loop_edge* loop_edges, size_t ca
 
 }  // extern "C"
 
+// ---- the map products' shared host steps: the prologue over the submaps, the bounds pass, the box, the rank pass and the
+// compacted clouds' read-backs ----
+namespace {
+
+// "<what>: the sensor origin of submap k lies beyond <beyond>"
+int origin_refused(b200sm_t s, const char* what, size_t k, const char* beyond) {
+  s->err = std::string(what) + ": the sensor origin of submap " + std::to_string(k) + " lies beyond " + beyond;
+  return (int)B200REG_ERR_ARG;
+}
+
+// A map build's prologue: refuses a session without submaps and non-finite poses, then before_tiles' message when it
+// returns one, and lays out the tiles of the submaps with points (`tile` points per block) into *t. Then every submap in
+// order gets a zeroed entry with its float pose, and its cloud, size and first tile when it has points; per_submap(k, e)
+// adds the build's own fields or refuses (an error code, s->err set), and the entries of the submaps with points are
+// appended to *table. `what` prefixes the messages.
+template <class Entry, class PerSubmap>
+int map_prologue(b200sm_t s, const char* what, const double* poses_colmajor16, size_t tile, const char* (*before_tiles)(b200sm_t),
+                 SubmapTiles* t, std::vector<Entry>* table, PerSubmap&& per_submap) {
+  const size_t n_sub = s->submaps.size();
+  const std::string w = std::string(what) + ": ";
+  if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, (w + "the session has no submaps").c_str());
+  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, (w + "a non-finite pose entry").c_str());
+  if (const char* why = before_tiles ? before_tiles(s) : nullptr) return sm_fail(s, B200REG_ERR_ARG, (w + why).c_str());
+  const int rc = submap_tiles(s, 0, tile, true, (w + "a submap of 2^32 points or more").c_str(),
+                              (w + "too many points for one launch").c_str(), t);
+  if (rc != B200REG_OK) return rc;
+  for (size_t k = 0; k < n_sub; k++) {
+    const Submap& sub = *s->submaps[k];
+    Entry e;
+    std::memset(&e, 0, sizeof(e));
+    submap_pose_f(s, k, poses_colmajor16, e.T);
+    if (sub.n) {
+      e.cloud = sub.cloud;
+      e.n = (unsigned)sub.n;
+      e.first_tile = t->first_tile[table->size()];
+    }
+    const int rc = per_submap(k, e);
+    if (rc != B200REG_OK) return rc;
+    if (sub.n) table->push_back(e);
+  }
+  return (int)B200REG_OK;
+}
+
+// One bounds pass (K14a, K15a, K19a) over a build's table, D = 2 or 3 axes: zeroes n_counters counters, uploads the table
+// and its bounds (2 D ints per entry: the lower corner, then the upper), runs `launch` when there are entries, reads back
+// the bounds and the first k counters into ctr, synchronises once, and reduces the entries' bounds per axis into lo[D] /
+// hi[D] (INT_MAX / INT_MIN without an entry). `bounds` comes in with the entries' seeds, or empty to start every entry
+// empty, and leaves as the launch widened it. Must run inside sm_guarded.
+template <int D, class Entry, class Const>
+void bounds_pass(b200sm_t s, void (*launch)(const Entry*, int, unsigned, const Const&, int*, unsigned long long*, cudaStream_t),
+                 const Const& c, const std::vector<Entry>& table, unsigned long long tiles, DeviceBuffer<Entry>& d_table,
+                 std::vector<int>& bounds, int n_counters, unsigned long long* ctr, int k, int* lo, int* hi) {
+  MapWorkspace& w = s->work;
+  const size_t n = table.size();
+  if (bounds.empty()) {
+    bounds.resize(2 * D * n);
+    for (size_t r = 0; r < n; r++)
+      for (int a = 0; a < D; a++) {
+        bounds[2 * D * r + a] = INT_MAX;
+        bounds[2 * D * r + D + a] = INT_MIN;
+      }
+  }
+  w.counters.ensure(n_counters);
+  B200_CUDA(cudaMemsetAsync(w.counters.ptr, 0, n_counters * sizeof(unsigned long long), s->stream));
+  if (n) {
+    d_table.ensure(n);
+    w.bounds.ensure(bounds.size());
+    B200_CUDA(cudaMemcpyAsync(d_table.ptr, table.data(), n * sizeof(Entry), cudaMemcpyHostToDevice, s->stream));
+    B200_CUDA(cudaMemcpyAsync(w.bounds.ptr, bounds.data(), bounds.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
+    launch(d_table.ptr, (int)n, (unsigned)tiles, c, w.bounds.ptr, w.counters.ptr, s->stream);
+    s->launches += 1;
+    B200_CUDA(cudaMemcpyAsync(bounds.data(), w.bounds.ptr, bounds.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+  }
+  B200_CUDA(cudaMemcpyAsync(ctr, w.counters.ptr, k * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
+  B200_CUDA(cudaStreamSynchronize(s->stream));
+  for (int a = 0; a < D; a++) {
+    lo[a] = INT_MAX;
+    hi[a] = INT_MIN;
+    for (size_t r = 0; r < n; r++) {
+      lo[a] = std::min(lo[a], bounds[2 * D * r + a]);
+      hi[a] = std::max(hi[a], bounds[2 * D * r + D + a]);
+    }
+  }
+}
+
+// The W x H grid over the cells lo[2] .. hi[2]; more than 2^28 cells is refused
+int grid_or_refuse(b200sm_t s, const char* what, const int* lo, const int* hi, unsigned long long* W, unsigned long long* H) {
+  *W = (unsigned long long)((long long)hi[0] - lo[0] + 1);
+  *H = (unsigned long long)((long long)hi[1] - lo[1] + 1);
+  if (*W * *H <= OG_MAX_CELLS) return (int)B200REG_OK;
+  s->err = std::string(what) + ": a grid of " + std::to_string(*W) + " x " + std::to_string(*H) + " cells exceeds 2^28 cells";
+  return (int)B200REG_ERR_ARG;
+}
+
+// The box over the cells lo[3] .. hi[3] widened by r on every side (the mesh's band; 0 for the others); more than 2^31 - 1
+// cells is refused as "<what>: <kind> of X x Y x Z <unit> exceeds 2^31 - 1 <unit>"
+int box_or_refuse(b200sm_t s, const char* what, const char* kind, const char* unit, const int* lo, const int* hi, int r, SmBox* box,
+                  unsigned long long* cells) {
+  if (ms_box(lo, hi, r, box->lo, box->dims, cells)) return (int)B200REG_OK;
+  auto width = [&](int a) { return std::to_string((long long)hi[a] - lo[a] + 1 + 2 * r); };
+  s->err = std::string(what) + ": " + kind + " of " + width(0) + " x " + width(1) + " x " + width(2) + " " + unit + " exceeds 2^31 - 1 " +
+           unit;
+  return (int)B200REG_ERR_ARG;
+}
+
+// One rank pass (K15b, K19b, K21a): the rank index over n_words words cleared, mark(index) run, the index scanned, and the
+// number of marked cells read back after one synchronise. Must run inside sm_guarded.
+template <class Mark>
+unsigned rank_pass(b200sm_t s, DeviceBuffer<RankWord>& index, unsigned long long n_words, Mark&& mark) {
+  RankIndexScratch& scan = s->work.rank_scan;
+  index.ensure((size_t)n_words);
+  rank_index_clear(index.ptr, (int)n_words, s->stream);
+  mark(index.ptr);
+  scan.total.ensure(1);
+  rank_index_scan_async(index.ptr, (size_t)n_words, scan, scan.total.ptr, s->stream);
+  s->launches += 3;
+  unsigned marked = 0;
+  B200_CUDA(cudaMemcpyAsync(&marked, scan.total.ptr, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+  B200_CUDA(cudaStreamSynchronize(s->stream));
+  return marked;
+}
+
+// Per-submap offsets into a compacted map of `kept` points, n_sub + 1 of them: a submap with points starts at its first
+// tile's offset, an empty one where the next one starts
+std::vector<size_t> submap_offsets(const SubmapTiles& t, size_t n_sub, const std::vector<unsigned>& tile_off, unsigned kept) {
+  std::vector<size_t> offsets(n_sub + 1, (size_t)kept);
+  size_t r = t.ids.size();
+  for (size_t k = n_sub; k-- > 0;) {
+    if (r > 0 && t.ids[r - 1] == k) offsets[k] = tile_off[t.first_tile[--r]];
+    else offsets[k] = offsets[k + 1];
+  }
+  return offsets;
+}
+
+// A compacted cloud of `total` points read back: its size, its per-submap offsets, and at most capacity points
+int get_compacted(b200sm_t s, const DeviceBuffer<float4>& pts, size_t total, const std::vector<size_t>& offs, float* out_xyzi,
+                  size_t capacity, size_t* n, size_t* offsets) {
+  return sm_guarded(s, [&]() {
+    if (offsets) std::memcpy(offsets, offs.data(), offs.size() * sizeof(size_t));
+    return read_back(s, pts.ptr, total, out_xyzi, capacity, n);
+  });
+}
+
+// A compacted cloud of `total` points saved as PCL's ASCII PCD; an empty one is refused as "<what>: <empty>"
+int save_compacted_pcd(b200sm_t s, const char* what, const char* empty, const DeviceBuffer<float4>& pts, size_t total, const char* path,
+                       size_t* n_points, size_t* n_bytes) {
+  if (total == 0) return sm_fail(s, B200REG_ERR_ARG, (std::string(what) + ": " + empty).c_str());
+  return sm_guarded(s, [&]() { return write_pcd_ascii(s, pts.ptr, total, path, what, n_points, n_bytes); });
+}
+
+// Enqueues the read-back of `count` elements of src into dst when dst is given
+template <class T>
+void get_if(b200sm_t s, void* dst, const T* src, size_t count) {
+  if (dst) B200_CUDA(cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyDeviceToHost, s->stream));
+}
+
+}  // namespace
+
 // ---- occupancy grid: free space ray-cast from every submap's sensor origin (csrc/occupancy_grid.hpp, csrc/occupancy.cu) ----
 namespace {
 
@@ -2582,87 +2734,53 @@ int b200sm_build_occupancy_grid(b200sm_t s, const double* poses_colmajor16, cons
   const OgParams p = og_params_from(params);
   OgConst c;
   if (const char* why = og_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_occupancy_grid: ") + why).c_str());
-  const size_t n_sub = s->submaps.size();
-  if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_occupancy_grid: the session has no submaps");
-  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, "build_occupancy_grid: a non-finite pose entry");
-  // the tiles of the submaps that have points (an empty submap's origin alone widens the grid)
+  // every submap's ray origin; the entries' bounds start at their origin's cell, and an empty submap's origin alone
+  // widens the grid
   SubmapTiles t;
-  const int rc = submap_tiles(s, 0, OG_TILE, true, "build_occupancy_grid: a submap of 2^32 points or more",
-                              "build_occupancy_grid: too many points for one launch", &t);
-  if (rc != B200REG_OK) return rc;
-  const std::vector<size_t>& ids = t.ids;
-  // every submap's float pose and ray origin
-  std::vector<OgEntry> all(n_sub);
-  std::vector<int> bounds(4 * n_sub);
-  for (size_t k = 0; k < n_sub; k++) {
-    const Submap& sub = *s->submaps[k];
-    OgEntry& e = all[k];
-    std::memset(&e, 0, sizeof(e));
-    submap_pose_f(s, k, poses_colmajor16, e.T);
+  std::vector<OgEntry> table;
+  std::vector<int> bounds, origins;
+  int rc = map_prologue(s, "build_occupancy_grid", poses_colmajor16, OG_TILE, nullptr, &t, &table, [&](size_t k, OgEntry& e) {
     long long o[3];
-    if (!og_origin(c, p, e.T, o)) {
-      s->err = "build_occupancy_grid: the sensor origin of submap " + std::to_string(k) +
-               " lies beyond 2^30 cells, or more than 2^16 cells from the height band";
-      return (int)B200REG_ERR_ARG;
-    }
-    e.cloud = sub.cloud;
-    e.n = (unsigned)sub.n;
+    if (!og_origin(c, p, e.T, o))
+      return origin_refused(s, "build_occupancy_grid", k, "2^30 cells, or more than 2^16 cells from the height band");
     e.xo = o[0];
     e.yo = o[1];
     e.zo = o[2];
-    bounds[4 * k + 0] = bounds[4 * k + 2] = og_cell(o[0]);
-    bounds[4 * k + 1] = bounds[4 * k + 3] = og_cell(o[1]);
-  }
+    const int x = og_cell(o[0]), y = og_cell(o[1]);
+    origins.insert(origins.end(), {x, y});
+    if (e.n) bounds.insert(bounds.end(), {x, y, x, y});
+    return (int)B200REG_OK;
+  });
+  if (rc != B200REG_OK) return rc;
   return sm_guarded(s, [&]() {
-    // K14a over the submaps with points: one launch, one read-back of the bounds and counts
-    std::vector<OgEntry> table;
-    for (size_t r = 0; r < ids.size(); r++) {
-      table.push_back(all[ids[r]]);
-      table.back().first_tile = t.first_tile[r];
-    }
-    std::vector<int> tb(4 * table.size());
-    for (size_t r = 0; r < ids.size(); r++) std::memcpy(&tb[4 * r], &bounds[4 * ids[r]], 4 * sizeof(int));
+    MapWorkspace& w = s->work;
+    OccupancyGrid& G = s->og;
+    // K14a over the submaps with points
     unsigned long long ctr[OG_CTR_COUNT] = {};
-    s->og_counters.ensure(OG_CTR_COUNT);
-    B200_CUDA(cudaMemsetAsync(s->og_counters.ptr, 0, OG_CTR_COUNT * sizeof(unsigned long long), s->stream));
-    if (!table.empty()) {
-      s->og_table.ensure(table.size());
-      s->og_bounds.ensure(tb.size());
-      B200_CUDA(cudaMemcpyAsync(s->og_table.ptr, table.data(), table.size() * sizeof(OgEntry), cudaMemcpyHostToDevice, s->stream));
-      B200_CUDA(cudaMemcpyAsync(s->og_bounds.ptr, tb.data(), tb.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
-      og_bounds_launch(s->og_table.ptr, (int)table.size(), (unsigned)t.tiles, c, s->og_bounds.ptr, s->og_counters.ptr, s->stream);
-      s->launches += 1;
-      B200_CUDA(cudaMemcpyAsync(tb.data(), s->og_bounds.ptr, tb.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
-    }
-    B200_CUDA(cudaMemcpyAsync(ctr, s->og_counters.ptr, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
-    B200_CUDA(cudaStreamSynchronize(s->stream));
-    for (size_t r = 0; r < ids.size(); r++) std::memcpy(&bounds[4 * ids[r]], &tb[4 * r], 4 * sizeof(int));
-    int gx0 = bounds[0], gy0 = bounds[1], gx1 = bounds[2], gy1 = bounds[3];
-    for (size_t k = 1; k < n_sub; k++) {
-      gx0 = std::min(gx0, bounds[4 * k]);
-      gy0 = std::min(gy0, bounds[4 * k + 1]);
-      gx1 = std::max(gx1, bounds[4 * k + 2]);
-      gy1 = std::max(gy1, bounds[4 * k + 3]);
-    }
-    const unsigned long long W = (unsigned long long)((long long)gx1 - gx0 + 1), H = (unsigned long long)((long long)gy1 - gy0 + 1);
-    if (W * H > OG_MAX_CELLS) {
-      s->err = "build_occupancy_grid: a grid of " + std::to_string(W) + " x " + std::to_string(H) + " cells exceeds 2^28 cells";
-      return (int)B200REG_ERR_ARG;
-    }
+    int lo[2], hi[2];
+    bounds_pass<2>(s, og_bounds_launch, c, table, t.tiles, w.og_table, bounds, OG_CTR_COUNT, ctr, 2, lo, hi);
+    for (size_t k = 0; k < origins.size(); k += 2)
+      for (int a = 0; a < 2; a++) {
+        lo[a] = std::min(lo[a], origins[k + a]);
+        hi[a] = std::max(hi[a], origins[k + a]);
+      }
+    unsigned long long W, H;
+    if ((rc = grid_or_refuse(s, "build_occupancy_grid", lo, hi, &W, &H)) != B200REG_OK) return rc;
+    const int gx0 = lo[0], gy0 = lo[1];
     // from here on the previous grid is replaced
-    s->og_built = false;
+    G.built = false;
     const size_t cells = (size_t)(W * H);
-    s->og_hits.ensure(cells);
-    s->og_frees.ensure(cells);
-    s->og_values.ensure(cells);
-    s->og_image.ensure(cells);
-    B200_CUDA(cudaMemsetAsync(s->og_hits.ptr, 0, cells * sizeof(uint32_t), s->stream));
-    B200_CUDA(cudaMemsetAsync(s->og_frees.ptr, 0, cells * sizeof(uint32_t), s->stream));
+    G.hits.ensure(cells);
+    G.frees.ensure(cells);
+    G.values.ensure(cells);
+    G.image.ensure(cells);
+    B200_CUDA(cudaMemsetAsync(G.hits.ptr, 0, cells * sizeof(uint32_t), s->stream));
+    B200_CUDA(cudaMemsetAsync(G.frees.ptr, 0, cells * sizeof(uint32_t), s->stream));
     // windows, then batches of consecutive submaps whose bitmaps fit the scratch budget (a submap whose bitmaps alone
     // exceed it forms a batch of its own); the scratch is sized to the largest batch so formed
     for (size_t r = 0; r < table.size(); r++) {
       OgEntry& e = table[r];
-      const int* b = &tb[4 * r];
+      const int* b = &bounds[4 * r];
       e.x0 = b[0];
       e.y0 = b[1];
       e.width = (unsigned)(b[2] - b[0] + 1);
@@ -2680,13 +2798,13 @@ int b200sm_build_occupancy_grid(b200sm_t s, const double* poses_colmajor16, cons
       Batch bt{b0, b0, 0, 0, 0};
       while (bt.b1 < table.size()) {
         OgEntry& e = table[bt.b1];
-        const unsigned long long w = 2ull * e.stride * e.rows;
-        if (bt.b1 > b0 && bt.words + w > OG_SCRATCH_WORDS) break;
+        const unsigned long long words = 2ull * e.stride * e.rows;
+        if (bt.b1 > b0 && bt.words + words > OG_SCRATCH_WORDS) break;
         e.words_at = bt.words;
         e.fold_first = bt.fold;
         e.first_tile = (unsigned)bt.tiles;
-        bt.words += w;
-        bt.fold += w / 2;
+        bt.words += words;
+        bt.fold += words / 2;
         bt.tiles += (e.n + OG_TILE - 1) / OG_TILE;
         bt.b1++;
       }
@@ -2694,38 +2812,37 @@ int b200sm_build_occupancy_grid(b200sm_t s, const double* poses_colmajor16, cons
       plan.push_back(bt);
       b0 = bt.b1;
     }
-    s->og_scratch.ensure((size_t)largest);
+    w.bitmaps.ensure((size_t)largest);
     for (const Batch& bt : plan) {
-      if (bt.words > s->og_scratch.cap || bt.b1 > s->og_table.cap)
+      if (bt.words > w.bitmaps.cap || bt.b1 > w.og_table.cap)
         return sm_fail(s, B200REG_ERR_CUDA, "build_occupancy_grid: a walk batch larger than its scratch");
       // the previous batch's kernels read the table: this copy is stream-ordered behind them
-      B200_CUDA(cudaMemcpyAsync(s->og_table.ptr + bt.b0, table.data() + bt.b0, (bt.b1 - bt.b0) * sizeof(OgEntry),
+      B200_CUDA(cudaMemcpyAsync(w.og_table.ptr + bt.b0, table.data() + bt.b0, (bt.b1 - bt.b0) * sizeof(OgEntry),
                                 cudaMemcpyHostToDevice, s->stream));
-      B200_CUDA(cudaMemsetAsync(s->og_scratch.ptr, 0, bt.words * sizeof(uint32_t), s->stream));
-      og_walk_launch(s->og_table.ptr + bt.b0, (int)(bt.b1 - bt.b0), (unsigned)bt.tiles, c, s->og_scratch.ptr, s->og_counters.ptr,
-                     s->stream);
-      og_fold_launch(s->og_table.ptr + bt.b0, (int)(bt.b1 - bt.b0), bt.fold, s->og_scratch.ptr, gx0, gy0, (unsigned)W,
-                     s->og_hits.ptr, s->og_frees.ptr, s->stream);
+      B200_CUDA(cudaMemsetAsync(w.bitmaps.ptr, 0, bt.words * sizeof(uint32_t), s->stream));
+      og_walk_launch(w.og_table.ptr + bt.b0, (int)(bt.b1 - bt.b0), (unsigned)bt.tiles, c, w.bitmaps.ptr, w.counters.ptr, s->stream);
+      og_fold_launch(w.og_table.ptr + bt.b0, (int)(bt.b1 - bt.b0), bt.fold, w.bitmaps.ptr, gx0, gy0, (unsigned)W, G.hits.ptr,
+                     G.frees.ptr, s->stream);
       s->launches += 2;
     }
     const int batches = (int)plan.size();
-    og_classify_launch(s->og_hits.ptr, s->og_frees.ptr, (unsigned)W, (unsigned)H, c.occ_value, c.free_value, s->og_values.ptr,
-                       s->og_image.ptr, s->og_counters.ptr, s->stream);
+    og_classify_launch(G.hits.ptr, G.frees.ptr, (unsigned)W, (unsigned)H, c.occ_value, c.free_value, G.values.ptr, G.image.ptr,
+                       w.counters.ptr, s->stream);
     s->launches += 1;
-    B200_CUDA(cudaMemcpyAsync(ctr, s->og_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaMemcpyAsync(ctr, w.counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));  // the host table goes out of scope; the counts are read
     if (ctr[OG_CTR_TRIPPED]) return sm_fail(s, B200REG_ERR_CUDA, "build_occupancy_grid: a walk left its submap's window");
-    s->og_built = true;
-    s->og_params = p;
-    s->og_width = (unsigned)W;
-    s->og_height = (unsigned)H;
-    s->og_origin[0] = (double)gx0 * p.resolution;
-    s->og_origin[1] = (double)gy0 * p.resolution;
+    G.built = true;
+    G.params = p;
+    G.width = (unsigned)W;
+    G.height = (unsigned)H;
+    G.origin[0] = (double)gx0 * p.resolution;
+    G.origin[1] = (double)gy0 * p.resolution;
     if (info) {
-      info->width = s->og_width;
-      info->height = s->og_height;
-      info->origin[0] = s->og_origin[0];
-      info->origin[1] = s->og_origin[1];
+      info->width = G.width;
+      info->height = G.height;
+      info->origin[0] = G.origin[0];
+      info->origin[1] = G.origin[1];
       info->resolution = p.resolution;
       info->n_rays = ctr[OG_CTR_RAYS];
       info->n_skipped = ctr[OG_CTR_SKIPPED];
@@ -2740,13 +2857,14 @@ int b200sm_build_occupancy_grid(b200sm_t s, const double* poses_colmajor16, cons
 
 int b200sm_get_occupancy_grid(b200sm_t s, signed char* data, unsigned* hits, unsigned* frees, size_t capacity) {
   if (!s) return B200REG_ERR_ARG;
-  if (!s->og_built) return sm_fail(s, B200REG_ERR_ARG, "get_occupancy_grid: no grid has been built");
+  if (!s->og.built) return sm_fail(s, B200REG_ERR_ARG, "get_occupancy_grid: no grid has been built");
   return sm_guarded(s, [&]() {
-    const size_t m = std::min(capacity, (size_t)s->og_width * s->og_height);
+    const OccupancyGrid& G = s->og;
+    const size_t m = std::min(capacity, (size_t)G.width * G.height);
     if (m) {
-      if (data) B200_CUDA(cudaMemcpyAsync(data, s->og_values.ptr, m, cudaMemcpyDeviceToHost, s->stream));
-      if (hits) B200_CUDA(cudaMemcpyAsync(hits, s->og_hits.ptr, m * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
-      if (frees) B200_CUDA(cudaMemcpyAsync(frees, s->og_frees.ptr, m * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      get_if(s, data, G.values.ptr, m);
+      get_if(s, hits, G.hits.ptr, m);
+      get_if(s, frees, G.frees.ptr, m);
       B200_CUDA(cudaStreamSynchronize(s->stream));
     }
     return (int)B200REG_OK;
@@ -2755,10 +2873,10 @@ int b200sm_get_occupancy_grid(b200sm_t s, signed char* data, unsigned* hits, uns
 
 int b200sm_save_occupancy_map(b200sm_t s, const char* pgm_path, const char* yaml_path) {
   if (!s || !pgm_path || !yaml_path) return B200REG_ERR_ARG;
-  if (!s->og_built) return sm_fail(s, B200REG_ERR_ARG, "save_occupancy_map: no grid has been built");
-  const OgParams& p = s->og_params;
-  return save_map_pair(s, "save_occupancy_map: ", s->og_image.ptr, s->og_width, s->og_height, p.resolution, s->og_origin,
-                       p.occupied_thresh, p.free_thresh, pgm_path, yaml_path);
+  if (!s->og.built) return sm_fail(s, B200REG_ERR_ARG, "save_occupancy_map: no grid has been built");
+  const OccupancyGrid& G = s->og;
+  return save_map_pair(s, "save_occupancy_map: ", G.image.ptr, G.width, G.height, G.params.resolution, G.origin,
+                       G.params.occupied_thresh, G.params.free_thresh, pgm_path, yaml_path);
 }
 
 }  // extern "C"
@@ -2796,61 +2914,26 @@ int b200sm_build_elevation_map(b200sm_t s, const double* poses_colmajor16, const
   const ElParams p = el_params_from(params);
   ElConst c;
   if (const char* why = el_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_elevation_map: ") + why).c_str());
-  const size_t n_sub = s->submaps.size();
-  if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_elevation_map: the session has no submaps");
-  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, "build_elevation_map: a non-finite pose entry");
-  SubmapTiles t;
-  const int rc = submap_tiles(s, 0, OG_TILE, true, "build_elevation_map: a submap of 2^32 points or more",
-                              "build_elevation_map: too many points for one launch", &t);
-  if (rc != B200REG_OK) return rc;
   // the submaps with points: float pose and horizontal origin (the band is the whole line, so zo plays no part)
-  std::vector<OgEntry> table(t.ids.size());
-  for (size_t r = 0; r < t.ids.size(); r++) {
-    const size_t k = t.ids[r];
-    OgEntry& e = table[r];
-    std::memset(&e, 0, sizeof(e));
-    submap_pose_f(s, k, poses_colmajor16, e.T);
-    if (!el_origin(c, p, e.T, &e.xo, &e.yo)) {
-      s->err = "build_elevation_map: the sensor origin of submap " + std::to_string(k) + " lies beyond 2^30 cells";
-      return (int)B200REG_ERR_ARG;
-    }
-    e.cloud = s->submaps[k]->cloud;
-    e.n = (unsigned)s->submaps[k]->n;
-    e.first_tile = t.first_tile[r];
-  }
+  SubmapTiles t;
+  std::vector<OgEntry> table;
+  int rc = map_prologue(s, "build_elevation_map", poses_colmajor16, OG_TILE, nullptr, &t, &table, [&](size_t k, OgEntry& e) {
+    if (e.n && !el_origin(c, p, e.T, &e.xo, &e.yo)) return origin_refused(s, "build_elevation_map", k, "2^30 cells");
+    return (int)B200REG_OK;
+  });
+  if (rc != B200REG_OK) return rc;
   if (table.empty()) return sm_fail(s, B200REG_ERR_ARG, "build_elevation_map: no submap has points");
   return sm_guarded(s, [&]() {
-    // K14a: the extent of the non-skipped points, bounds starting empty; one read-back
-    std::vector<int> tb(4 * table.size());
-    for (size_t r = 0; r < table.size(); r++) {
-      tb[4 * r] = tb[4 * r + 1] = INT_MAX;
-      tb[4 * r + 2] = tb[4 * r + 3] = INT_MIN;
-    }
+    MapWorkspace& w = s->work;
+    // K14a: the extent of the non-skipped points, bounds starting empty
+    std::vector<int> bounds;
     unsigned long long ctr[EL_CTR_COUNT] = {};
-    s->el_counters.ensure(EL_CTR_COUNT);
-    s->el_table.ensure(table.size());
-    s->el_bounds.ensure(tb.size());
-    B200_CUDA(cudaMemsetAsync(s->el_counters.ptr, 0, EL_CTR_COUNT * sizeof(unsigned long long), s->stream));
-    B200_CUDA(cudaMemcpyAsync(s->el_table.ptr, table.data(), table.size() * sizeof(OgEntry), cudaMemcpyHostToDevice, s->stream));
-    B200_CUDA(cudaMemcpyAsync(s->el_bounds.ptr, tb.data(), tb.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
-    og_bounds_launch(s->el_table.ptr, (int)table.size(), (unsigned)t.tiles, c.og, s->el_bounds.ptr, s->el_counters.ptr, s->stream);
-    B200_CUDA(cudaMemcpyAsync(tb.data(), s->el_bounds.ptr, tb.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
-    B200_CUDA(cudaMemcpyAsync(ctr, s->el_counters.ptr, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
-    B200_CUDA(cudaStreamSynchronize(s->stream));
-    s->launches += 1;
+    int lo[2], hi[2];
+    bounds_pass<2>(s, og_bounds_launch, c.og, table, t.tiles, w.og_table, bounds, EL_CTR_COUNT, ctr, 2, lo, hi);
     if (ctr[EL_CTR_POINTS] == 0) return sm_fail(s, B200REG_ERR_ARG, "build_elevation_map: every point is skipped");
-    int gx0 = INT_MAX, gy0 = INT_MAX, gx1 = INT_MIN, gy1 = INT_MIN;
-    for (size_t r = 0; r < table.size(); r++) {
-      gx0 = std::min(gx0, tb[4 * r]);
-      gy0 = std::min(gy0, tb[4 * r + 1]);
-      gx1 = std::max(gx1, tb[4 * r + 2]);
-      gy1 = std::max(gy1, tb[4 * r + 3]);
-    }
-    const unsigned long long W = (unsigned long long)((long long)gx1 - gx0 + 1), H = (unsigned long long)((long long)gy1 - gy0 + 1);
-    if (W * H > OG_MAX_CELLS) {
-      s->err = "build_elevation_map: a grid of " + std::to_string(W) + " x " + std::to_string(H) + " cells exceeds 2^28 cells";
-      return (int)B200REG_ERR_ARG;
-    }
+    unsigned long long W, H;
+    if ((rc = grid_or_refuse(s, "build_elevation_map", lo, hi, &W, &H)) != B200REG_OK) return rc;
+    const int gx0 = lo[0], gy0 = lo[1];
     // the new map is built beside the last one, which stays until this build succeeds
     const size_t cells = (size_t)(W * H);
     auto m = std::make_unique<ElevationMap>();
@@ -2866,21 +2949,21 @@ int b200sm_build_elevation_map(b200sm_t s, const double* poses_colmajor16, const
     B200_CUDA(cudaMemsetAsync(m->lo.ptr, 0x7f, cells * sizeof(long long), s->stream));   // EL_LO_EMPTY
     B200_CUDA(cudaMemsetAsync(m->top.ptr, 0x80, cells * sizeof(long long), s->stream));  // EL_TOP_EMPTY
     long long zrange[2] = {EL_LO_EMPTY, EL_TOP_EMPTY};
-    s->el_zrange.ensure(2);
-    B200_CUDA(cudaMemcpyAsync(s->el_zrange.ptr, zrange, sizeof(zrange), cudaMemcpyHostToDevice, s->stream));
-    el_lowest_launch(s->el_table.ptr, (int)table.size(), (unsigned)t.tiles, c, gx0, gy0, (unsigned)W, (unsigned)H, m->n.ptr, m->lo.ptr,
-                     s->el_counters.ptr, s->stream);
-    el_top_launch(s->el_table.ptr, (int)table.size(), (unsigned)t.tiles, c, gx0, gy0, (unsigned)W, (unsigned)H, m->lo.ptr, m->top.ptr,
-                  s->el_counters.ptr, s->el_zrange.ptr, s->stream);
-    B200_CUDA(cudaMemcpyAsync(zrange, s->el_zrange.ptr, sizeof(zrange), cudaMemcpyDeviceToHost, s->stream));
+    w.zrange.ensure(2);
+    B200_CUDA(cudaMemcpyAsync(w.zrange.ptr, zrange, sizeof(zrange), cudaMemcpyHostToDevice, s->stream));
+    el_lowest_launch(w.og_table.ptr, (int)table.size(), (unsigned)t.tiles, c, gx0, gy0, (unsigned)W, (unsigned)H, m->n.ptr, m->lo.ptr,
+                     w.counters.ptr, s->stream);
+    el_top_launch(w.og_table.ptr, (int)table.size(), (unsigned)t.tiles, c, gx0, gy0, (unsigned)W, (unsigned)H, m->lo.ptr, m->top.ptr,
+                  w.counters.ptr, w.zrange.ptr, s->stream);
+    B200_CUDA(cudaMemcpyAsync(zrange, w.zrange.ptr, sizeof(zrange), cudaMemcpyDeviceToHost, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     s->launches += 2;
     if (zrange[1] - zrange[0] >= EL_HEIGHT_EXTENT)
       return sm_fail(s, B200REG_ERR_ARG, "build_elevation_map: the map's height extent is 2^24 cells or more");
     el_window_launch(c, (unsigned)W, (unsigned)H, m->n.ptr, m->top.ptr, m->step.ptr, m->tan_slope.ptr, m->roughness.ptr, m->value.ptr,
-                     m->image.ptr, s->el_counters.ptr, s->stream);
+                     m->image.ptr, w.counters.ptr, s->stream);
     s->launches += 1;
-    B200_CUDA(cudaMemcpyAsync(ctr, s->el_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaMemcpyAsync(ctr, w.counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     if (ctr[EL_CTR_TRIPPED]) return sm_fail(s, B200REG_ERR_CUDA, "build_elevation_map: a point's cell left the grid");
     m->params = p;
@@ -2911,16 +2994,13 @@ int b200sm_get_elevation_map(b200sm_t s, unsigned* n, long long* h, long long* l
     const ElevationMap& m = *s->el;
     const size_t k = std::min(capacity, (size_t)m.info.width * m.info.height);
     if (k) {
-      auto get = [&](void* dst, const void* src, size_t bytes) {
-        if (dst) B200_CUDA(cudaMemcpyAsync(dst, src, k * bytes, cudaMemcpyDeviceToHost, s->stream));
-      };
-      get(n, m.n.ptr, sizeof(uint32_t));
-      get(h, m.top.ptr, sizeof(long long));
-      get(lo, m.lo.ptr, sizeof(long long));
-      get(step, m.step.ptr, sizeof(float));
-      get(tan_slope, m.tan_slope.ptr, sizeof(float));
-      get(roughness, m.roughness.ptr, sizeof(float));
-      get(value, m.value.ptr, 1);
+      get_if(s, n, m.n.ptr, k);
+      get_if(s, h, m.top.ptr, k);
+      get_if(s, lo, m.lo.ptr, k);
+      get_if(s, step, m.step.ptr, k);
+      get_if(s, tan_slope, m.tan_slope.ptr, k);
+      get_if(s, roughness, m.roughness.ptr, k);
+      get_if(s, value, m.value.ptr, k);
       B200_CUDA(cudaStreamSynchronize(s->stream));
     }
     return (int)B200REG_OK;
@@ -2958,14 +3038,6 @@ SmParams sm_params_from(const b200sm_static_map_params* p) {
   return q;
 }
 
-// A build's per-call buffers: the table, the entries' bounds and the counters (n_counters slots, SM_CTR_* first)
-struct SmWork {
-  DeviceBuffer<SmEntry>& table;
-  DeviceBuffer<int>& bounds;
-  DeviceBuffer<unsigned long long>& counters;
-  int n_counters;
-};
-
 // What the front half leaves for the rest of a build
 struct SmFront {
   SmBox box{};
@@ -2974,69 +3046,36 @@ struct SmFront {
   int batches = 0;
 };
 
-// The front half the static map and the map changes share: the table's upload, K15a and the box (refused here, before
-// anything is sized from it), then `replacing()` (the caller's last build is about to be overwritten), K15b with the rank
-// scan, and the walks K15c / K15d in batches of consecutive entries. The entries [0, split_entry) fold into hits[0] /
-// frees[0] and, when split_entry < table.size(), the entries [split_entry, table.size()) into hits[1] / frees[1]; no batch
-// crosses split_entry. The counts are sized and zeroed here (one slot when there is no occupied voxel). Must run inside
-// sm_guarded; `what` prefixes the messages.
+// The front half the static map and the map changes share, on the bounds pass and the rank pass: K15a and the box
+// (refused here, before anything is sized from it), then `replacing()` (the caller's last build is about to be
+// overwritten), K15b, and the walks K15c / K15d in batches of consecutive entries. The entries [0, split_entry) fold into
+// hits[0] / frees[0] and, when split_entry < table.size(), the entries [split_entry, table.size()) into hits[1] /
+// frees[1]; no batch crosses split_entry. The counts are sized and zeroed here (one slot when there is no occupied voxel).
+// n_counters counters are zeroed. Must run inside sm_guarded; `what` prefixes the messages.
 template <class Replacing>
-int sm_front_half(b200sm_t s, const char* what, std::vector<SmEntry>& table, unsigned long long tiles, const SmConst& c, SmWork w,
+int sm_front_half(b200sm_t s, const char* what, std::vector<SmEntry>& table, unsigned long long tiles, const SmConst& c, int n_counters,
                   size_t split_entry, DeviceBuffer<RankWord>& index, DeviceBuffer<uint32_t>* hits, DeviceBuffer<uint32_t>* frees,
                   Replacing&& replacing, SmFront* out) {
+  MapWorkspace& w = s->work;
   const int n_entries = (int)table.size();
-  // K15a: one launch, one read-back of the bounds and counts
-  std::vector<int> bounds(6 * table.size());
-  for (size_t r = 0; r < table.size(); r++)
-    for (int a = 0; a < 3; a++) {
-      bounds[6 * r + a] = INT_MAX;
-      bounds[6 * r + 3 + a] = INT_MIN;
-    }
+  std::vector<int> bounds;
   unsigned long long ctr[2] = {};
-  w.counters.ensure(w.n_counters);
-  B200_CUDA(cudaMemsetAsync(w.counters.ptr, 0, w.n_counters * sizeof(unsigned long long), s->stream));
-  if (n_entries) {
-    w.table.ensure(table.size());
-    w.bounds.ensure(bounds.size());
-    B200_CUDA(cudaMemcpyAsync(w.table.ptr, table.data(), table.size() * sizeof(SmEntry), cudaMemcpyHostToDevice, s->stream));
-    B200_CUDA(cudaMemcpyAsync(w.bounds.ptr, bounds.data(), bounds.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
-    sm_bounds_launch(w.table.ptr, n_entries, (unsigned)tiles, c, w.bounds.ptr, w.counters.ptr, s->stream);
-    s->launches += 1;
-    B200_CUDA(cudaMemcpyAsync(bounds.data(), w.bounds.ptr, bounds.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
-  }
-  B200_CUDA(cudaMemcpyAsync(ctr, w.counters.ptr, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
-  B200_CUDA(cudaStreamSynchronize(s->stream));
-  int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
-  for (size_t r = 0; r < table.size(); r++)
-    for (int a = 0; a < 3; a++) {
-      lo[a] = std::min(lo[a], bounds[6 * r + a]);
-      hi[a] = std::max(hi[a], bounds[6 * r + 3 + a]);
-    }
+  int lo[3], hi[3];
+  bounds_pass<3>(s, sm_bounds_launch, c, table, tiles, w.sm_table, bounds, n_counters, ctr, 2, lo, hi);
   const bool any_ray = ctr[SM_CTR_RAYS] > 0;
   SmBox box{};
   unsigned long long cells = 0;
-  if (any_ray && !sm_box(lo, hi, box.dims, &cells)) {
-    s->err = std::string(what) + ": a box of " + std::to_string((long long)hi[0] - lo[0] + 1) + " x " +
-             std::to_string((long long)hi[1] - lo[1] + 1) + " x " + std::to_string((long long)hi[2] - lo[2] + 1) +
-             " voxels exceeds 2^31 - 1 voxels";
-    return (int)B200REG_ERR_ARG;
+  if (any_ray) {
+    const int rc = box_or_refuse(s, what, "a box", "voxels", lo, hi, 0, &box, &cells);
+    if (rc != B200REG_OK) return rc;
   }
-  if (any_ray)
-    for (int a = 0; a < 3; a++) box.lo[a] = lo[a];
   replacing();
   const unsigned long long n_words = (cells + 31) / 32;
   unsigned n_voxels = 0;
-  if (any_ray) {
-    // K15b: the rank index over the box, then the number of occupied voxels
-    index.ensure((size_t)n_words);
-    rank_index_clear(index.ptr, (int)n_words, s->stream);
-    sm_mark_launch(w.table.ptr, n_entries, (unsigned)tiles, c, box, index.ptr, w.counters.ptr, s->stream);
-    s->sm_scan.total.ensure(1);
-    rank_index_scan_async(index.ptr, (size_t)n_words, s->sm_scan, s->sm_scan.total.ptr, s->stream);
-    s->launches += 3;
-    B200_CUDA(cudaMemcpyAsync(&n_voxels, s->sm_scan.total.ptr, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
-    B200_CUDA(cudaStreamSynchronize(s->stream));
-  }
+  if (any_ray)  // K15b: the rank index over the box, then the number of occupied voxels
+    n_voxels = rank_pass(s, index, n_words, [&](RankWord* idx) {
+      sm_mark_launch(w.sm_table.ptr, n_entries, (unsigned)tiles, c, box, idx, w.counters.ptr, s->stream);
+    });
   const int n_epochs = split_entry < table.size() ? 2 : 1;
   const size_t nv = std::max<size_t>(n_voxels, 1);
   for (int e = 0; e < n_epochs; e++) {
@@ -3051,7 +3090,7 @@ int sm_front_half(b200sm_t s, const char* what, std::vector<SmEntry>& table, uns
   if (n_voxels > 0) {
     const size_t per_batch = (size_t)std::max<unsigned long long>(1ull, SM_SCRATCH_WORDS / (2ull * words_per));
     const size_t largest = std::min(per_batch, table.size());
-    s->sm_scratch.ensure((size_t)(2ull * words_per * largest));
+    w.bitmaps.ensure((size_t)(2ull * words_per * largest));
     for (int e = 0; e < n_epochs; e++) {
       const size_t r0 = e == 0 ? 0 : split_entry, r1 = e == n_epochs - 1 ? table.size() : split_entry;
       for (size_t b0 = r0; b0 < r1; b0 += per_batch) {
@@ -3061,15 +3100,15 @@ int sm_front_half(b200sm_t s, const char* what, std::vector<SmEntry>& table, uns
           table[r].batch_tile = (unsigned)bt;
           bt += (table[r].n + SM_TILE - 1) / SM_TILE;
         }
-        if (2ull * words_per * (b1 - b0) > s->sm_scratch.cap || b1 > w.table.cap)
+        if (2ull * words_per * (b1 - b0) > w.bitmaps.cap || b1 > w.sm_table.cap)
           return sm_fail(s, B200REG_ERR_CUDA, (std::string(what) + ": a walk batch larger than its scratch").c_str());
         // the previous batch's kernels read the table: this copy is stream-ordered behind them
-        B200_CUDA(cudaMemcpyAsync(w.table.ptr + b0, table.data() + b0, (b1 - b0) * sizeof(SmEntry), cudaMemcpyHostToDevice,
+        B200_CUDA(cudaMemcpyAsync(w.sm_table.ptr + b0, table.data() + b0, (b1 - b0) * sizeof(SmEntry), cudaMemcpyHostToDevice,
                                   s->stream));
-        B200_CUDA(cudaMemsetAsync(s->sm_scratch.ptr, 0, 2ull * words_per * (b1 - b0) * sizeof(uint32_t), s->stream));
-        sm_walk_launch(w.table.ptr + b0, (int)(b1 - b0), (unsigned)bt, c, box, index.ptr, n_voxels, words_per, s->sm_scratch.ptr,
+        B200_CUDA(cudaMemsetAsync(w.bitmaps.ptr, 0, 2ull * words_per * (b1 - b0) * sizeof(uint32_t), s->stream));
+        sm_walk_launch(w.sm_table.ptr + b0, (int)(b1 - b0), (unsigned)bt, c, box, index.ptr, n_voxels, words_per, w.bitmaps.ptr,
                        w.counters.ptr, s->stream);
-        sm_fold_launch(s->sm_scratch.ptr, (int)(b1 - b0), words_per, n_voxels, hits[e].ptr, frees[e].ptr, s->stream);
+        sm_fold_launch(w.bitmaps.ptr, (int)(b1 - b0), words_per, n_voxels, hits[e].ptr, frees[e].ptr, s->stream);
         s->launches += 2;
         batches++;
       }
@@ -3092,85 +3131,60 @@ int b200sm_build_static_map(b200sm_t s, const double* poses_colmajor16, const b2
   const SmParams p = sm_params_from(params);
   SmConst c;
   if (const char* why = sm_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_static_map: ") + why).c_str());
-  const size_t n_sub = s->submaps.size();
-  if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_static_map: the session has no submaps");
-  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, "build_static_map: a non-finite pose entry");
-  SubmapTiles t;
-  const int rc = submap_tiles(s, 0, SM_TILE, true, "build_static_map: a submap of 2^32 points or more",
-                              "build_static_map: too many points for one launch", &t);
-  if (rc != B200REG_OK) return rc;
-  const std::vector<size_t>& ids = t.ids;
-  const unsigned long long tiles = t.tiles;
   // the entries of the submaps with points (empty ones own no tile), in submap order
+  SubmapTiles t;
   std::vector<SmEntry> table;
-  unsigned long long total = 0;
-  for (size_t k = 0; k < n_sub; k++) {
-    const Submap& sub = *s->submaps[k];
-    SmEntry e;
-    std::memset(&e, 0, sizeof(e));
-    submap_pose_f(s, k, poses_colmajor16, e.T);
-    if (!sm_origin(c, p, e.T, e.o)) {
-      s->err = "build_static_map: the sensor origin of submap " + std::to_string(k) + " lies beyond 2^30 voxels";
-      return (int)B200REG_ERR_ARG;
-    }
-    total += sub.n;
-    if (sub.n == 0) continue;
-    e.cloud = sub.cloud;
-    e.n = (unsigned)sub.n;
-    e.first_tile = t.first_tile[table.size()];
-    table.push_back(e);
-  }
+  const int rc = map_prologue(s, "build_static_map", poses_colmajor16, SM_TILE, nullptr, &t, &table, [&](size_t k, SmEntry& e) {
+    return sm_origin(c, p, e.T, e.o) ? (int)B200REG_OK : origin_refused(s, "build_static_map", k, "2^30 voxels");
+  });
+  if (rc != B200REG_OK) return rc;
+  const unsigned long long total = map_points(s);
   if (total > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_static_map: a map of 2^32 points or more");
+  const size_t n_sub = s->submaps.size();
+  const unsigned long long tiles = t.tiles;
   const int n_entries = (int)table.size();
   return sm_guarded(s, [&]() {
+    MapWorkspace& w = s->work;
+    StaticMap& M = s->sm;
     SmFront f;
-    const int rc = sm_front_half(s, "build_static_map", table, tiles, c, SmWork{s->sm_table, s->sm_bounds, s->sm_counters, SM_CTR_COUNT},
-                                 table.size(), s->sm_index, &s->sm_hits, &s->sm_frees, [&]() { s->sm_built = false; }, &f);
+    const int rc = sm_front_half(s, "build_static_map", table, tiles, c, SM_CTR_COUNT, table.size(), M.index, &M.hits, &M.frees,
+                                 [&]() { M.built = false; }, &f);
     if (rc != B200REG_OK) return rc;
     const SmBox& box = f.box;
-    const unsigned long long n_words = f.n_words;
     const unsigned n_voxels = f.n_voxels;
-    const int batches = f.batches;
     unsigned long long ctr[SM_CTR_COUNT] = {};
-    s->sm_dynamic.ensure(std::max<size_t>(n_voxels, 1));
+    M.dynamic.ensure(std::max<size_t>(n_voxels, 1));
     if (n_voxels > 0) {
       // K15e
-      sm_classify_launch(s->sm_hits.ptr, s->sm_frees.ptr, n_voxels, c, s->sm_dynamic.ptr, s->sm_counters.ptr, s->stream);
+      sm_classify_launch(M.hits.ptr, M.frees.ptr, n_voxels, c, M.dynamic.ptr, w.counters.ptr, s->stream);
       s->launches += 1;
     }
     // K15f: kept points per tile, scanned into tile offsets; the host reads the total and sizes the static map from it
     unsigned kept = 0;
     std::vector<unsigned> tile_off((size_t)tiles + 1, 0);
     if (tiles) {
-      s->sm_tiles.ensure((size_t)tiles + 1);
-      sm_count_launch(s->sm_table.ptr, n_entries, (unsigned)tiles, c, box, s->sm_index.ptr, s->sm_dynamic.ptr, n_voxels,
-                      s->sm_tiles.ptr, s->stream);
-      counter_scan_async(s->sm_tiles.ptr, (size_t)tiles, s->sm_tiles_tmp, s->stream);
+      w.tiles.ensure((size_t)tiles + 1);
+      sm_count_launch(w.sm_table.ptr, n_entries, (unsigned)tiles, c, box, M.index.ptr, M.dynamic.ptr, n_voxels, w.tiles.ptr, s->stream);
+      counter_scan_async(w.tiles.ptr, (size_t)tiles, w.scan_tmp, s->stream);
       s->launches += 3;
-      B200_CUDA(cudaMemcpyAsync(tile_off.data(), s->sm_tiles.ptr, tile_off.size() * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaMemcpyAsync(tile_off.data(), w.tiles.ptr, tile_off.size() * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
       B200_CUDA(cudaStreamSynchronize(s->stream));
       kept = tile_off[(size_t)tiles];
     }
     // K15g
-    s->sm_static.ensure(std::max<size_t>(kept, 1));
+    M.points.ensure(std::max<size_t>(kept, 1));
     if (kept) {
-      sm_write_launch(s->sm_table.ptr, n_entries, (unsigned)tiles, c, box, s->sm_index.ptr, s->sm_dynamic.ptr, n_voxels,
-                      s->sm_tiles.ptr, kept, s->sm_static.ptr, s->sm_counters.ptr, s->stream);
+      sm_write_launch(w.sm_table.ptr, n_entries, (unsigned)tiles, c, box, M.index.ptr, M.dynamic.ptr, n_voxels, w.tiles.ptr, kept,
+                      M.points.ptr, w.counters.ptr, s->stream);
       s->launches += 1;
     }
-    B200_CUDA(cudaMemcpyAsync(ctr, s->sm_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaMemcpyAsync(ctr, w.counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));  // the host table goes out of scope; the counts are read
     if (ctr[SM_CTR_TRIPPED]) return sm_fail(s, B200REG_ERR_CUDA, "build_static_map: a voxel outside the box or beyond the rank index");
-    // per-submap offsets: a submap with points starts at its first tile's offset; an empty one where the next one starts
-    s->sm_offsets.assign(n_sub + 1, (size_t)kept);
-    size_t r = table.size();
-    for (size_t k = n_sub; k-- > 0;) {
-      if (r > 0 && ids[r - 1] == k) s->sm_offsets[k] = tile_off[table[--r].first_tile];
-      else s->sm_offsets[k] = s->sm_offsets[k + 1];
-    }
-    s->sm_box = box;
-    s->sm_words = n_words;
-    b200sm_static_map_info& I = s->sm_info;
+    M.offsets = submap_offsets(t, n_sub, tile_off, kept);
+    M.box = box;
+    M.n_words = f.n_words;
+    b200sm_static_map_info& I = M.info;
     for (int a = 0; a < 3; a++) {
       I.box_origin[a] = box.lo[a];
       I.box_dims[a] = box.dims[a];
@@ -3181,8 +3195,8 @@ int b200sm_build_static_map(b200sm_t s, const double* poses_colmajor16, const b2
     I.n_dynamic_voxels = ctr[SM_CTR_DYNAMIC];
     I.n_points = total;
     I.n_static_points = kept;
-    I.n_batches = batches;
-    s->sm_built = true;
+    I.n_batches = f.batches;
+    M.built = true;
     if (info) *info = I;
     return (int)B200REG_OK;
   });
@@ -3190,37 +3204,30 @@ int b200sm_build_static_map(b200sm_t s, const double* poses_colmajor16, const b2
 
 int b200sm_get_static_map(b200sm_t s, float* out_xyzi, size_t capacity, size_t* n, size_t* offsets) {
   if (!s || (!out_xyzi && capacity)) return B200REG_ERR_ARG;
-  if (!s->sm_built) return sm_fail(s, B200REG_ERR_ARG, "get_static_map: no static map has been built");
-  return sm_guarded(s, [&]() {
-    const size_t total = (size_t)s->sm_info.n_static_points;
-    if (n) *n = total;
-    if (offsets) std::memcpy(offsets, s->sm_offsets.data(), s->sm_offsets.size() * sizeof(size_t));
-    const size_t m = std::min(capacity, total);
-    if (m) {
-      B200_CUDA(cudaMemcpyAsync(out_xyzi, s->sm_static.ptr, m * sizeof(float4), cudaMemcpyDeviceToHost, s->stream));
-      B200_CUDA(cudaStreamSynchronize(s->stream));
-    }
-    return (int)B200REG_OK;
-  });
+  if (!s->sm.built) return sm_fail(s, B200REG_ERR_ARG, "get_static_map: no static map has been built");
+  const StaticMap& M = s->sm;
+  return get_compacted(s, M.points, (size_t)M.info.n_static_points, M.offsets, out_xyzi, capacity, n, offsets);
 }
 
 int b200sm_get_map_voxels(b200sm_t s, int* ijk3, unsigned* hits, unsigned* frees, unsigned char* dynamic, size_t capacity, size_t* n) {
   if (!s) return B200REG_ERR_ARG;
-  if (!s->sm_built) return sm_fail(s, B200REG_ERR_ARG, "get_map_voxels: no static map has been built");
+  if (!s->sm.built) return sm_fail(s, B200REG_ERR_ARG, "get_map_voxels: no static map has been built");
   return sm_guarded(s, [&]() {
-    const unsigned n_voxels = (unsigned)s->sm_info.n_voxels;
+    const StaticMap& M = s->sm;
+    const unsigned n_voxels = (unsigned)M.info.n_voxels;
     if (n) *n = n_voxels;
     const size_t m = std::min(capacity, (size_t)n_voxels);
     if (m == 0) return (int)B200REG_OK;
     if (ijk3) {
-      s->sm_ijk.ensure(3 * (size_t)n_voxels);
-      sm_voxel_list_launch(s->sm_index.ptr, s->sm_words, s->sm_box, n_voxels, s->sm_ijk.ptr, s->stream);
+      DeviceBuffer<int>& ijk = s->work.ijk;
+      ijk.ensure(3 * (size_t)n_voxels);
+      sm_voxel_list_launch(M.index.ptr, M.n_words, M.box, n_voxels, ijk.ptr, s->stream);
       s->launches += 1;
-      B200_CUDA(cudaMemcpyAsync(ijk3, s->sm_ijk.ptr, 3 * m * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+      get_if(s, ijk3, ijk.ptr, 3 * m);
     }
-    if (hits) B200_CUDA(cudaMemcpyAsync(hits, s->sm_hits.ptr, m * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
-    if (frees) B200_CUDA(cudaMemcpyAsync(frees, s->sm_frees.ptr, m * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
-    if (dynamic) B200_CUDA(cudaMemcpyAsync(dynamic, s->sm_dynamic.ptr, m, cudaMemcpyDeviceToHost, s->stream));
+    get_if(s, hits, M.hits.ptr, m);
+    get_if(s, frees, M.frees.ptr, m);
+    get_if(s, dynamic, M.dynamic.ptr, m);
     B200_CUDA(cudaStreamSynchronize(s->stream));
     return (int)B200REG_OK;
   });
@@ -3228,10 +3235,9 @@ int b200sm_get_map_voxels(b200sm_t s, int* ijk3, unsigned* hits, unsigned* frees
 
 int b200sm_save_static_map_pcd_ascii(b200sm_t s, const char* path, size_t* n_points, size_t* n_bytes) {
   if (!s || !path) return B200REG_ERR_ARG;
-  if (!s->sm_built) return sm_fail(s, B200REG_ERR_ARG, "save_static_map_pcd_ascii: no static map has been built");
-  const size_t total = (size_t)s->sm_info.n_static_points;
-  if (total == 0) return sm_fail(s, B200REG_ERR_ARG, "save_static_map_pcd_ascii: the static map has no points");
-  return sm_guarded(s, [&]() { return write_pcd_ascii(s, s->sm_static.ptr, total, path, "save_static_map_pcd_ascii", n_points, n_bytes); });
+  if (!s->sm.built) return sm_fail(s, B200REG_ERR_ARG, "save_static_map_pcd_ascii: no static map has been built");
+  return save_compacted_pcd(s, "save_static_map_pcd_ascii", "the static map has no points", s->sm.points,
+                            (size_t)s->sm.info.n_static_points, path, n_points, n_bytes);
 }
 
 }  // extern "C"
@@ -3247,50 +3253,36 @@ int b200sm_build_map_changes(b200sm_t s, const double* poses_colmajor16, const b
   SmConst c;
   if (const char* why = sm_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_map_changes: ") + why).c_str());
   const size_t n_sub = s->submaps.size();
-  if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_map_changes: the session has no submaps");
   unsigned long long split = 0;
   const unsigned long long last_first = s->seg_first.size() > 1 ? (unsigned long long)s->seg_first.back() : 0ull;
-  if (const char* why = ch_split(split_submap, n_sub, last_first, &split))
-    return sm_fail(s, B200REG_ERR_ARG, (std::string("build_map_changes: ") + why).c_str());
-  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, "build_map_changes: a non-finite pose entry");
-  SubmapTiles t;
-  const int rc = submap_tiles(s, 0, SM_TILE, true, "build_map_changes: a submap of 2^32 points or more",
-                              "build_map_changes: too many points for one launch", &t);
-  if (rc != B200REG_OK) return rc;
-  const std::vector<size_t>& ids = t.ids;
-  const unsigned long long tiles = t.tiles;
+  if (n_sub)  // a session without submaps is refused first, by the prologue
+    if (const char* why = ch_split(split_submap, n_sub, last_first, &split))
+      return sm_fail(s, B200REG_ERR_ARG, (std::string("build_map_changes: ") + why).c_str());
   // the entries of the submaps with points, in submap order, their first map index, and the first AFTER entry
+  SubmapTiles t;
   std::vector<SmEntry> table;
   std::vector<unsigned> map_first;
   size_t split_entry = 0;
-  unsigned long long total = 0;
-  for (size_t k = 0; k < n_sub; k++) {
-    const Submap& sub = *s->submaps[k];
-    SmEntry e;
-    std::memset(&e, 0, sizeof(e));
-    submap_pose_f(s, k, poses_colmajor16, e.T);
-    if (!sm_origin(c, p, e.T, e.o)) {
-      s->err = "build_map_changes: the sensor origin of submap " + std::to_string(k) + " lies beyond 2^30 voxels";
-      return (int)B200REG_ERR_ARG;
-    }
+  unsigned long long at = 0;
+  const int rc = map_prologue(s, "build_map_changes", poses_colmajor16, SM_TILE, nullptr, &t, &table, [&](size_t k, SmEntry& e) {
+    if (!sm_origin(c, p, e.T, e.o)) return origin_refused(s, "build_map_changes", k, "2^30 voxels");
     if (k == split) split_entry = table.size();
-    const unsigned long long at = total;
-    total += sub.n;
-    if (sub.n == 0) continue;
-    e.cloud = sub.cloud;
-    e.n = (unsigned)sub.n;
-    e.first_tile = t.first_tile[table.size()];
-    table.push_back(e);
-    map_first.push_back((unsigned)at);
-  }
+    if (e.n) map_first.push_back((unsigned)at);
+    at += e.n;
+    return (int)B200REG_OK;
+  });
+  if (rc != B200REG_OK) return rc;
+  const unsigned long long total = at;
   if (total > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_map_changes: a map of 2^32 points or more");
+  const unsigned long long tiles = t.tiles;
   const int n_entries = (int)table.size();
   return sm_guarded(s, [&]() {
+    MapWorkspace& w = s->work;
     // the new build is made beside the last one, which stays until this one succeeds
     auto m = std::make_unique<MapChanges>();
     SmFront f;
-    const int rc = sm_front_half(s, "build_map_changes", table, tiles, c, SmWork{s->ch_table, s->ch_bounds, s->ch_counters, CH_CTR_COUNT},
-                                 split_entry, m->index, m->hits, m->frees, []() {}, &f);
+    const int rc = sm_front_half(s, "build_map_changes", table, tiles, c, CH_CTR_COUNT, split_entry, m->index, m->hits, m->frees, []() {},
+                                 &f);
     if (rc != B200REG_OK) return rc;
     const unsigned n_voxels = f.n_voxels;
     const size_t nv = std::max<size_t>(n_voxels, 1);
@@ -3305,7 +3297,7 @@ int b200sm_build_map_changes(b200sm_t s, const double* poses_colmajor16, const b
     m->label.ensure(nv);
     if (n_voxels > 0) {
       ch_classify_launch(m->hits[CH_BEFORE].ptr, m->frees[CH_BEFORE].ptr, m->hits[CH_AFTER].ptr, m->frees[CH_AFTER].ptr, n_voxels, c,
-                         m->label.ptr, s->ch_counters.ptr, s->stream);
+                         m->label.ptr, w.counters.ptr, s->stream);
       s->launches += 1;
     }
     // K20b: the point labels and the kept points per tile, scanned into tile offsets; the host reads the total and sizes
@@ -3314,37 +3306,31 @@ int b200sm_build_map_changes(b200sm_t s, const double* poses_colmajor16, const b
     unsigned kept = 0;
     std::vector<unsigned> tile_off((size_t)tiles + 1, 0);
     if (tiles) {
-      s->ch_map_first.ensure(map_first.size());
-      B200_CUDA(cudaMemcpyAsync(s->ch_map_first.ptr, map_first.data(), map_first.size() * sizeof(unsigned), cudaMemcpyHostToDevice,
+      w.map_first.ensure(map_first.size());
+      B200_CUDA(cudaMemcpyAsync(w.map_first.ptr, map_first.data(), map_first.size() * sizeof(unsigned), cudaMemcpyHostToDevice,
                                 s->stream));
-      s->ch_tiles.ensure((size_t)tiles + 1);
-      ch_label_launch(s->ch_table.ptr, n_entries, (unsigned)tiles, c, f.box, m->index.ptr, m->label.ptr, n_voxels, (int)split_entry,
-                      s->ch_map_first.ptr, m->point_label.ptr, s->ch_tiles.ptr, s->ch_counters.ptr, s->stream);
-      counter_scan_async(s->ch_tiles.ptr, (size_t)tiles, s->ch_tiles_tmp, s->stream);
+      w.tiles.ensure((size_t)tiles + 1);
+      ch_label_launch(w.sm_table.ptr, n_entries, (unsigned)tiles, c, f.box, m->index.ptr, m->label.ptr, n_voxels, (int)split_entry,
+                      w.map_first.ptr, m->point_label.ptr, w.tiles.ptr, w.counters.ptr, s->stream);
+      counter_scan_async(w.tiles.ptr, (size_t)tiles, w.scan_tmp, s->stream);
       s->launches += 3;
-      B200_CUDA(cudaMemcpyAsync(tile_off.data(), s->ch_tiles.ptr, tile_off.size() * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaMemcpyAsync(tile_off.data(), w.tiles.ptr, tile_off.size() * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
       B200_CUDA(cudaStreamSynchronize(s->stream));
       kept = tile_off[(size_t)tiles];
     }
     // K20c
     m->updated.ensure(std::max<size_t>(kept, 1));
     if (kept) {
-      ch_write_launch(s->ch_table.ptr, n_entries, (unsigned)tiles, s->ch_map_first.ptr, m->point_label.ptr, s->ch_tiles.ptr, kept,
-                      m->updated.ptr, s->ch_counters.ptr, s->stream);
+      ch_write_launch(w.sm_table.ptr, n_entries, (unsigned)tiles, w.map_first.ptr, m->point_label.ptr, w.tiles.ptr, kept, m->updated.ptr,
+                      w.counters.ptr, s->stream);
       s->launches += 1;
     }
     unsigned long long ctr[CH_CTR_COUNT] = {};
-    B200_CUDA(cudaMemcpyAsync(ctr, s->ch_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaMemcpyAsync(ctr, w.counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));  // the host tables go out of scope; the counts are read
     if (ctr[SM_CTR_TRIPPED])
       return sm_fail(s, B200REG_ERR_CUDA, "build_map_changes: a voxel outside the box or beyond the rank index, or a point beyond the map");
-    // per-submap offsets: a submap with points starts at its first tile's offset; an empty one where the next one starts
-    m->offsets.assign(n_sub + 1, (size_t)kept);
-    size_t r = table.size();
-    for (size_t k = n_sub; k-- > 0;) {
-      if (r > 0 && ids[r - 1] == k) m->offsets[k] = tile_off[table[--r].first_tile];
-      else m->offsets[k] = m->offsets[k + 1];
-    }
+    m->offsets = submap_offsets(t, n_sub, tile_off, kept);
     m->box = f.box;
     m->n_words = f.n_words;
     b200sm_map_change_info& I = m->info;
@@ -3377,7 +3363,7 @@ int b200sm_get_map_changes(b200sm_t s, unsigned char* labels, size_t capacity, s
     if (n) *n = (size_t)m.info.n_points;
     const size_t k = std::min(capacity, (size_t)m.info.n_points);
     if (k) {
-      B200_CUDA(cudaMemcpyAsync(labels, m.point_label.ptr, k, cudaMemcpyDeviceToHost, s->stream));
+      get_if(s, labels, m.point_label.ptr, k);
       B200_CUDA(cudaStreamSynchronize(s->stream));
     }
     return (int)B200REG_OK;
@@ -3395,19 +3381,17 @@ int b200sm_get_change_voxels(b200sm_t s, int* ijk3, unsigned* hits_before, unsig
     const size_t k = std::min(capacity, (size_t)n_voxels);
     if (k == 0) return (int)B200REG_OK;
     if (ijk3) {
-      s->ch_ijk.ensure(3 * (size_t)n_voxels);
-      sm_voxel_list_launch(m.index.ptr, m.n_words, m.box, n_voxels, s->ch_ijk.ptr, s->stream);
+      DeviceBuffer<int>& ijk = s->work.ijk;
+      ijk.ensure(3 * (size_t)n_voxels);
+      sm_voxel_list_launch(m.index.ptr, m.n_words, m.box, n_voxels, ijk.ptr, s->stream);
       s->launches += 1;
-      B200_CUDA(cudaMemcpyAsync(ijk3, s->ch_ijk.ptr, 3 * k * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+      get_if(s, ijk3, ijk.ptr, 3 * k);
     }
-    auto get = [&](unsigned* dst, const DeviceBuffer<uint32_t>& src) {
-      if (dst) B200_CUDA(cudaMemcpyAsync(dst, src.ptr, k * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
-    };
-    get(hits_before, m.hits[CH_BEFORE]);
-    get(frees_before, m.frees[CH_BEFORE]);
-    get(hits_after, m.hits[CH_AFTER]);
-    get(frees_after, m.frees[CH_AFTER]);
-    if (label) B200_CUDA(cudaMemcpyAsync(label, m.label.ptr, k, cudaMemcpyDeviceToHost, s->stream));
+    get_if(s, hits_before, m.hits[CH_BEFORE].ptr, k);
+    get_if(s, frees_before, m.frees[CH_BEFORE].ptr, k);
+    get_if(s, hits_after, m.hits[CH_AFTER].ptr, k);
+    get_if(s, frees_after, m.frees[CH_AFTER].ptr, k);
+    get_if(s, label, m.label.ptr, k);
     B200_CUDA(cudaStreamSynchronize(s->stream));
     return (int)B200REG_OK;
   });
@@ -3416,26 +3400,15 @@ int b200sm_get_change_voxels(b200sm_t s, int* ijk3, unsigned* hits_before, unsig
 int b200sm_get_updated_map(b200sm_t s, float* out_xyzi, size_t capacity, size_t* n, size_t* offsets) {
   if (!s || (!out_xyzi && capacity)) return B200REG_ERR_ARG;
   if (!s->ch) return sm_fail(s, B200REG_ERR_ARG, "get_updated_map: no build yet");
-  return sm_guarded(s, [&]() {
-    const MapChanges& m = *s->ch;
-    const size_t total = (size_t)m.info.n_updated_points;
-    if (n) *n = total;
-    if (offsets) std::memcpy(offsets, m.offsets.data(), m.offsets.size() * sizeof(size_t));
-    const size_t k = std::min(capacity, total);
-    if (k) {
-      B200_CUDA(cudaMemcpyAsync(out_xyzi, m.updated.ptr, k * sizeof(float4), cudaMemcpyDeviceToHost, s->stream));
-      B200_CUDA(cudaStreamSynchronize(s->stream));
-    }
-    return (int)B200REG_OK;
-  });
+  const MapChanges& m = *s->ch;
+  return get_compacted(s, m.updated, (size_t)m.info.n_updated_points, m.offsets, out_xyzi, capacity, n, offsets);
 }
 
 int b200sm_save_updated_map_pcd_ascii(b200sm_t s, const char* path, size_t* n_points, size_t* n_bytes) {
   if (!s || !path) return B200REG_ERR_ARG;
   if (!s->ch) return sm_fail(s, B200REG_ERR_ARG, "save_updated_map_pcd_ascii: no build yet");
-  const size_t total = (size_t)s->ch->info.n_updated_points;
-  if (total == 0) return sm_fail(s, B200REG_ERR_ARG, "save_updated_map_pcd_ascii: the updated map has no points");
-  return sm_guarded(s, [&]() { return write_pcd_ascii(s, s->ch->updated.ptr, total, path, "save_updated_map_pcd_ascii", n_points, n_bytes); });
+  return save_compacted_pcd(s, "save_updated_map_pcd_ascii", "the updated map has no points", s->ch->updated,
+                            (size_t)s->ch->info.n_updated_points, path, n_points, n_bytes);
 }
 
 }  // extern "C"
@@ -3467,86 +3440,38 @@ int b200sm_build_mesh(b200sm_t s, const double* poses_colmajor16, const b200sm_m
   const MsParams p = ms_params_from(params);
   MsConst c;
   if (const char* why = ms_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_mesh: ") + why).c_str());
-  const size_t n_sub = s->submaps.size();
-  if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_mesh: the session has no submaps");
-  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, "build_mesh: a non-finite pose entry");
   SubmapTiles t;
-  const int rc = submap_tiles(s, 0, SM_TILE, true, "build_mesh: a submap of 2^32 points or more", "build_mesh: too many points for one launch",
-                              &t);
-  if (rc != B200REG_OK) return rc;
-  const unsigned long long tiles = t.tiles;
   std::vector<SmEntry> table;
-  unsigned long long total = 0;
-  for (size_t k = 0; k < n_sub; k++) {
-    const Submap& sub = *s->submaps[k];
-    SmEntry e;
-    std::memset(&e, 0, sizeof(e));
-    submap_pose_f(s, k, poses_colmajor16, e.T);
-    if (!ms_origin(c, p, e.T, e.o)) {
-      s->err = "build_mesh: the sensor origin of submap " + std::to_string(k) + " lies beyond 2^30 voxels";
-      return (int)B200REG_ERR_ARG;
-    }
-    total += sub.n;
-    if (sub.n == 0) continue;
-    e.cloud = sub.cloud;
-    e.n = (unsigned)sub.n;
-    e.first_tile = t.first_tile[table.size()];
-    table.push_back(e);
-  }
+  const int rc = map_prologue(s, "build_mesh", poses_colmajor16, SM_TILE, nullptr, &t, &table, [&](size_t k, SmEntry& e) {
+    return ms_origin(c, p, e.T, e.o) ? (int)B200REG_OK : origin_refused(s, "build_mesh", k, "2^30 voxels");
+  });
+  if (rc != B200REG_OK) return rc;
+  const unsigned long long total = map_points(s);
   if (total > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_mesh: a map of 2^32 points or more");
+  const unsigned long long tiles = t.tiles;
   const int n_entries = (int)table.size();
   return sm_guarded(s, [&]() {
+    MapWorkspace& w = s->work;
     // the new build is made beside the last one, which stays until this one succeeds
     auto m = std::make_unique<MeshBuild>();
+    // K15a: the endpoint voxels' bounds and the ray counts
+    std::vector<int> bounds;
     unsigned long long ctr[MS_CTR_COUNT] = {};
-    s->ms_counters.ensure(MS_CTR_COUNT);
-    B200_CUDA(cudaMemsetAsync(s->ms_counters.ptr, 0, sizeof(ctr), s->stream));
-    // K15a: the endpoint voxels' bounds and the ray counts, one read-back
-    std::vector<int> bounds(6 * table.size());
-    for (size_t r = 0; r < table.size(); r++)
-      for (int a = 0; a < 3; a++) {
-        bounds[6 * r + a] = INT_MAX;
-        bounds[6 * r + 3 + a] = INT_MIN;
-      }
-    if (n_entries) {
-      s->ms_table.ensure(table.size());
-      s->ms_bounds.ensure(bounds.size());
-      B200_CUDA(cudaMemcpyAsync(s->ms_table.ptr, table.data(), table.size() * sizeof(SmEntry), cudaMemcpyHostToDevice, s->stream));
-      B200_CUDA(cudaMemcpyAsync(s->ms_bounds.ptr, bounds.data(), bounds.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
-      sm_bounds_launch(s->ms_table.ptr, n_entries, (unsigned)tiles, c.sm, s->ms_bounds.ptr, s->ms_counters.ptr, s->stream);
-      s->launches += 1;
-      B200_CUDA(cudaMemcpyAsync(bounds.data(), s->ms_bounds.ptr, bounds.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
-    }
-    B200_CUDA(cudaMemcpyAsync(ctr, s->ms_counters.ptr, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
-    B200_CUDA(cudaStreamSynchronize(s->stream));
-    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
-    for (size_t r = 0; r < table.size(); r++)
-      for (int a = 0; a < 3; a++) {
-        lo[a] = std::min(lo[a], bounds[6 * r + a]);
-        hi[a] = std::max(hi[a], bounds[6 * r + 3 + a]);
-      }
+    int lo[3], hi[3];
+    bounds_pass<3>(s, sm_bounds_launch, c.sm, table, tiles, w.sm_table, bounds, MS_CTR_COUNT, ctr, 2, lo, hi);
     const bool any_ray = ctr[SM_CTR_RAYS] > 0;
     SmBox box{};
     unsigned long long cells = 0;
-    if (any_ray && !ms_box(lo, hi, c.r, box.lo, box.dims, &cells)) {
-      s->err = "build_mesh: a band box of " + std::to_string((long long)hi[0] - lo[0] + 1 + 2 * c.r) + " x " +
-               std::to_string((long long)hi[1] - lo[1] + 1 + 2 * c.r) + " x " + std::to_string((long long)hi[2] - lo[2] + 1 + 2 * c.r) +
-               " voxels exceeds 2^31 - 1 voxels";
-      return (int)B200REG_ERR_ARG;
+    if (any_ray) {
+      const int rc = box_or_refuse(s, "build_mesh", "a band box", "voxels", lo, hi, c.r, &box, &cells);
+      if (rc != B200REG_OK) return rc;
     }
     const unsigned long long n_words = (cells + 31) / 32;
     unsigned n_band = 0;
-    if (any_ray) {
-      // K21a: the band walks into the rank index, then the number of band voxels
-      m->index.ensure((size_t)n_words);
-      rank_index_clear(m->index.ptr, (int)n_words, s->stream);
-      ms_mark_launch(s->ms_table.ptr, n_entries, (unsigned)tiles, c, box, m->index.ptr, s->ms_counters.ptr, s->stream);
-      s->ms_scan.total.ensure(1);
-      rank_index_scan_async(m->index.ptr, (size_t)n_words, s->ms_scan, s->ms_scan.total.ptr, s->stream);
-      s->launches += 3;
-      B200_CUDA(cudaMemcpyAsync(&n_band, s->ms_scan.total.ptr, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
-      B200_CUDA(cudaStreamSynchronize(s->stream));
-    }
+    if (any_ray)  // K21a: the band walks into the rank index, then the number of band voxels
+      n_band = rank_pass(s, m->index, n_words, [&](RankWord* idx) {
+        ms_mark_launch(w.sm_table.ptr, n_entries, (unsigned)tiles, c, box, idx, w.counters.ptr, s->stream);
+      });
     const size_t nb = std::max<size_t>(n_band, 1);
     m->sum.ensure(nb);
     m->weight.ensure(nb);
@@ -3554,43 +3479,42 @@ int b200sm_build_mesh(b200sm_t s, const double* poses_colmajor16, const b200sm_m
     B200_CUDA(cudaMemsetAsync(m->sum.ptr, 0, nb * sizeof(unsigned long long), s->stream));
     B200_CUDA(cudaMemsetAsync(m->weight.ptr, 0, nb * sizeof(uint32_t), s->stream));
     unsigned n_vert = 0;
-    std::vector<unsigned> vtile;
     const unsigned vtiles = (n_band + MS_THREADS - 1) / MS_THREADS;
     if (n_band > 0) {
       // K21b, the voxel list, K21c and its scan: the vertex count
-      ms_fuse_launch(s->ms_table.ptr, n_entries, (unsigned)tiles, c, box, m->index.ptr, n_band, m->sum.ptr, m->weight.ptr,
-                     s->ms_counters.ptr, s->stream);
+      ms_fuse_launch(w.sm_table.ptr, n_entries, (unsigned)tiles, c, box, m->index.ptr, n_band, m->sum.ptr, m->weight.ptr, w.counters.ptr,
+                     s->stream);
       sm_voxel_list_launch(m->index.ptr, n_words, box, n_band, m->ijk.ptr, s->stream);
-      s->ms_active.ensure(n_band);
-      s->ms_vcounts.ensure((size_t)vtiles + 1);
-      ms_active_launch(m->ijk.ptr, m->sum.ptr, m->weight.ptr, m->index.ptr, box, n_band, c.min_weight, s->ms_active.ptr,
-                       s->ms_vcounts.ptr, s->ms_counters.ptr, s->stream);
-      counter_scan_async(s->ms_vcounts.ptr, vtiles, s->ms_tiles_tmp, s->stream);
+      w.active.ensure(n_band);
+      w.vertex_counts.ensure((size_t)vtiles + 1);
+      ms_active_launch(m->ijk.ptr, m->sum.ptr, m->weight.ptr, m->index.ptr, box, n_band, c.min_weight, w.active.ptr, w.vertex_counts.ptr,
+                       w.counters.ptr, s->stream);
+      counter_scan_async(w.vertex_counts.ptr, vtiles, w.scan_tmp, s->stream);
       s->launches += 5;
-      B200_CUDA(cudaMemcpyAsync(&n_vert, s->ms_vcounts.ptr + vtiles, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaMemcpyAsync(&n_vert, w.vertex_counts.ptr + vtiles, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
       B200_CUDA(cudaStreamSynchronize(s->stream));
     }
     m->xyz.ensure(3 * std::max<size_t>(n_vert, 1));
     if (n_band > 0) {
       // K21d and its scan: the vertices, and the face count read back with the counters
-      s->ms_vid.ensure(n_band);
-      s->ms_fcounts.ensure((size_t)vtiles + 1);
-      ms_vertex_launch(m->ijk.ptr, m->sum.ptr, m->weight.ptr, m->index.ptr, box, n_band, c, s->ms_active.ptr, s->ms_vcounts.ptr, n_vert,
-                       s->ms_vid.ptr, m->xyz.ptr, s->ms_fcounts.ptr, s->ms_counters.ptr, s->stream);
-      counter_scan_async(s->ms_fcounts.ptr, vtiles, s->ms_tiles_tmp, s->stream);
+      w.vertex_id.ensure(n_band);
+      w.face_counts.ensure((size_t)vtiles + 1);
+      ms_vertex_launch(m->ijk.ptr, m->sum.ptr, m->weight.ptr, m->index.ptr, box, n_band, c, w.active.ptr, w.vertex_counts.ptr, n_vert,
+                       w.vertex_id.ptr, m->xyz.ptr, w.face_counts.ptr, w.counters.ptr, s->stream);
+      counter_scan_async(w.face_counts.ptr, vtiles, w.scan_tmp, s->stream);
       s->launches += 3;
     }
-    B200_CUDA(cudaMemcpyAsync(ctr, s->ms_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaMemcpyAsync(ctr, w.counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     if (ctr[MS_CTR_FACES] > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_mesh: 2^32 faces or more");
     const unsigned n_faces = (unsigned)ctr[MS_CTR_FACES];
     m->faces.ensure(3 * std::max<size_t>(n_faces, 1));
     if (n_faces > 0) {
       // K21e
-      ms_face_launch(m->ijk.ptr, m->sum.ptr, m->weight.ptr, m->index.ptr, box, n_band, c.min_weight, s->ms_vid.ptr, s->ms_fcounts.ptr,
-                     n_faces, m->faces.ptr, s->ms_counters.ptr, s->stream);
+      ms_face_launch(m->ijk.ptr, m->sum.ptr, m->weight.ptr, m->index.ptr, box, n_band, c.min_weight, w.vertex_id.ptr, w.face_counts.ptr,
+                     n_faces, m->faces.ptr, w.counters.ptr, s->stream);
       s->launches += 1;
-      B200_CUDA(cudaMemcpyAsync(ctr, s->ms_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaMemcpyAsync(ctr, w.counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
     }
     B200_CUDA(cudaStreamSynchronize(s->stream));  // the host table goes out of scope; the counts are read
     if (ctr[SM_CTR_TRIPPED])
@@ -3623,8 +3547,8 @@ int b200sm_get_mesh(b200sm_t s, float* xyz, size_t vertex_capacity, size_t* n_ve
     if (n_vertices) *n_vertices = (size_t)m.info.n_vertices;
     if (n_faces) *n_faces = (size_t)m.info.n_faces;
     const size_t kv = std::min(vertex_capacity, (size_t)m.info.n_vertices), kf = std::min(face_capacity, (size_t)m.info.n_faces);
-    if (kv) B200_CUDA(cudaMemcpyAsync(xyz, m.xyz.ptr, 3 * kv * sizeof(float), cudaMemcpyDeviceToHost, s->stream));
-    if (kf) B200_CUDA(cudaMemcpyAsync(faces3, m.faces.ptr, 3 * kf * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+    if (kv) get_if(s, xyz, m.xyz.ptr, 3 * kv);
+    if (kf) get_if(s, faces3, m.faces.ptr, 3 * kf);
     if (kv || kf) B200_CUDA(cudaStreamSynchronize(s->stream));
     return (int)B200REG_OK;
   });
@@ -3639,9 +3563,9 @@ int b200sm_get_mesh_voxels(b200sm_t s, int* ijk3, long long* sdf_sum, unsigned* 
     if (n) *n = nb;
     const size_t k = std::min(capacity, nb);
     if (k == 0) return (int)B200REG_OK;
-    if (ijk3) B200_CUDA(cudaMemcpyAsync(ijk3, m.ijk.ptr, 3 * k * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
-    if (sdf_sum) B200_CUDA(cudaMemcpyAsync(sdf_sum, m.sum.ptr, k * sizeof(long long), cudaMemcpyDeviceToHost, s->stream));
-    if (weight) B200_CUDA(cudaMemcpyAsync(weight, m.weight.ptr, k * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+    get_if(s, ijk3, m.ijk.ptr, 3 * k);
+    get_if(s, sdf_sum, m.sum.ptr, k);
+    get_if(s, weight, m.weight.ptr, k);
     B200_CUDA(cudaStreamSynchronize(s->stream));
     return (int)B200REG_OK;
   });
@@ -3718,6 +3642,9 @@ McParams mc_params_from(const b200sm_map_consistency_params* p) {
   return q;
 }
 
+// refused after the poses are checked and before the tiles are laid out
+const char* mc_too_many_points(b200sm_t s) { return map_points(s) > MC_MAX_POINTS ? "a map of 2^31 points or more" : nullptr; }
+
 }  // namespace
 
 extern "C" {
@@ -3728,82 +3655,45 @@ int b200sm_build_map_consistency(b200sm_t s, const double* poses_colmajor16, con
   const McParams p = mc_params_from(params);
   McConst c;
   if (const char* why = mc_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_map_consistency: ") + why).c_str());
+  // the entries of the submaps with points, in submap order, every submap's first map index and its double pose
   const size_t n_sub = s->submaps.size();
-  if (n_sub == 0) return sm_fail(s, B200REG_ERR_ARG, "build_map_consistency: the session has no submaps");
-  if (!finite_poses(poses_colmajor16, n_sub)) return sm_fail(s, B200REG_ERR_ARG, "build_map_consistency: a non-finite pose entry");
-  unsigned long long total = 0;
-  for (size_t k = 0; k < n_sub; k++) total += s->submaps[k]->n;
-  if (total > MC_MAX_POINTS) return sm_fail(s, B200REG_ERR_ARG, "build_map_consistency: a map of 2^31 points or more");
   SubmapTiles t;
-  const int rc = submap_tiles(s, 0, MC_TILE, true, "build_map_consistency: a submap of 2^32 points or more",
-                              "build_map_consistency: too many points for one launch", &t);
-  if (rc != B200REG_OK) return rc;
-  // the entries of the submaps with points, in submap order, and every submap's first map index
   std::vector<McEntry> table;
   std::vector<unsigned> sub_first(n_sub);
   std::vector<double> poses(16 * n_sub);
   unsigned long long at = 0;
-  for (size_t k = 0; k < n_sub; k++) {
-    const Submap& sub = *s->submaps[k];
-    for (int r = 0; r < 4; r++)
-      for (int col = 0; col < 4; col++)
-        poses[16 * k + col * 4 + r] = poses_colmajor16 ? poses_colmajor16[16 * k + col * 4 + r] : sub.pose[r * 4 + col];
-    sub_first[k] = (unsigned)at;
-    if (sub.n) {
-      McEntry e;
-      std::memset(&e, 0, sizeof(e));
-      e.cloud = sub.cloud;
-      e.n = (unsigned)sub.n;
-      e.first_tile = t.first_tile[table.size()];
-      e.map_offset = (unsigned)at;
-      submap_pose_f(s, k, poses_colmajor16, e.T);
-      table.push_back(e);
-    }
-    at += sub.n;
-  }
+  const int rc = map_prologue(s, "build_map_consistency", poses_colmajor16, MC_TILE, mc_too_many_points, &t, &table,
+                              [&](size_t k, McEntry& e) {
+                                const Submap& sub = *s->submaps[k];
+                                for (int r = 0; r < 4; r++)
+                                  for (int col = 0; col < 4; col++)
+                                    poses[16 * k + col * 4 + r] =
+                                        poses_colmajor16 ? poses_colmajor16[16 * k + col * 4 + r] : sub.pose[r * 4 + col];
+                                sub_first[k] = (unsigned)at;
+                                e.map_offset = (unsigned)at;
+                                at += e.n;
+                                return (int)B200REG_OK;
+                              });
+  if (rc != B200REG_OK) return rc;
+  const unsigned long long total = at;
   const int n_entries = (int)table.size();
   const unsigned tiles = (unsigned)t.tiles;
   return sm_guarded(s, [&]() {
-    // K19a: one launch, one read-back of the bounds and counts; the refusals it decides come before anything is sized
-    std::vector<int> bounds(6 * table.size());
-    for (size_t r = 0; r < table.size(); r++)
-      for (int a = 0; a < 3; a++) {
-        bounds[6 * r + a] = INT_MAX;
-        bounds[6 * r + 3 + a] = INT_MIN;
-      }
+    MapWorkspace& w = s->work;
+    // K19a; the refusals it decides come before anything is sized
+    std::vector<int> bounds;
     unsigned long long ctr[MC_CTR_COUNT] = {};
-    s->mc_counters.ensure(MC_CTR_COUNT);
-    B200_CUDA(cudaMemsetAsync(s->mc_counters.ptr, 0, MC_CTR_COUNT * sizeof(unsigned long long), s->stream));
-    if (n_entries) {
-      s->mc_table.ensure(table.size());
-      s->mc_bounds.ensure(bounds.size());
-      B200_CUDA(cudaMemcpyAsync(s->mc_table.ptr, table.data(), table.size() * sizeof(McEntry), cudaMemcpyHostToDevice, s->stream));
-      B200_CUDA(cudaMemcpyAsync(s->mc_bounds.ptr, bounds.data(), bounds.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
-      mc_bounds_launch(s->mc_table.ptr, n_entries, tiles, c, s->mc_bounds.ptr, s->mc_counters.ptr, s->stream);
-      s->launches += 1;
-      B200_CUDA(cudaMemcpyAsync(bounds.data(), s->mc_bounds.ptr, bounds.size() * sizeof(int), cudaMemcpyDeviceToHost, s->stream));
-    }
-    B200_CUDA(cudaMemcpyAsync(ctr, s->mc_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
-    B200_CUDA(cudaStreamSynchronize(s->stream));
+    int lo[3], hi[3];
+    bounds_pass<3>(s, mc_bounds_launch, c, table, tiles, w.mc_table, bounds, MC_CTR_COUNT, ctr, MC_CTR_COUNT, lo, hi);
     if (ctr[MC_CTR_RANGE])
       return sm_fail(s, B200REG_ERR_ARG, "build_map_consistency: a point's fixed-point coordinate is 2^46 or more in magnitude");
     const unsigned long long used = total - ctr[MC_CTR_SKIPPED];
-    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
-    for (size_t r = 0; r < table.size(); r++)
-      for (int a = 0; a < 3; a++) {
-        lo[a] = std::min(lo[a], bounds[6 * r + a]);
-        hi[a] = std::max(hi[a], bounds[6 * r + 3 + a]);
-      }
     SmBox box{};
     unsigned long long cells = 0;
-    if (used && !sm_box(lo, hi, box.dims, &cells)) {
-      s->err = "build_map_consistency: a box of " + std::to_string((long long)hi[0] - lo[0] + 1) + " x " +
-               std::to_string((long long)hi[1] - lo[1] + 1) + " x " + std::to_string((long long)hi[2] - lo[2] + 1) +
-               " cells exceeds 2^31 - 1 cells";
-      return (int)B200REG_ERR_ARG;
+    if (used) {
+      const int rc = box_or_refuse(s, "build_map_consistency", "a box", "cells", lo, hi, 0, &box, &cells);
+      if (rc != B200REG_OK) return rc;
     }
-    if (used)
-      for (int a = 0; a < 3; a++) box.lo[a] = lo[a];
     // the new build is made beside the last one, which stays until this one succeeds
     auto m = std::make_unique<MapConsistency>();
     m->c = c;
@@ -3820,14 +3710,9 @@ int b200sm_build_map_consistency(b200sm_t s, const double* poses_colmajor16, con
     unsigned n_cells = 0, n_chunks = 0;
     if (used) {
       // K19b: the occupied cells' rank index, their counts, the chunks of K19c, and the points in cell order
-      m->index.ensure((size_t)n_words);
-      rank_index_clear(m->index.ptr, (int)n_words, s->stream);
-      mc_mark_launch(s->mc_table.ptr, n_entries, tiles, c, box, m->index.ptr, s->mc_counters.ptr, s->stream);
-      s->mc_scan.total.ensure(1);
-      rank_index_scan_async(m->index.ptr, (size_t)n_words, s->mc_scan, s->mc_scan.total.ptr, s->stream);
-      s->launches += 3;
-      B200_CUDA(cudaMemcpyAsync(&n_cells, s->mc_scan.total.ptr, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
-      B200_CUDA(cudaStreamSynchronize(s->stream));
+      n_cells = rank_pass(s, m->index, n_words, [&](RankWord* idx) {
+        mc_mark_launch(w.mc_table.ptr, n_entries, tiles, c, box, idx, w.counters.ptr, s->stream);
+      });
       const size_t nc = (size_t)n_cells + 1;
       m->start.ensure(nc);
       m->queries.ensure(nc);
@@ -3839,29 +3724,29 @@ int b200sm_build_map_consistency(b200sm_t s, const double* poses_colmajor16, con
       B200_CUDA(cudaMemsetAsync(m->queries.ptr, 0, nc * sizeof(unsigned), s->stream));
       B200_CUDA(cudaMemsetAsync(m->qcursor.ptr, 0, nc * sizeof(unsigned), s->stream));
       B200_CUDA(cudaMemsetAsync(m->ocursor.ptr, 0, nc * sizeof(unsigned), s->stream));
-      mc_count_launch(s->mc_table.ptr, n_entries, tiles, c, box, m->index.ptr, m->start.ptr, m->queries.ptr, s->stream);
-      counter_scan_async(m->start.ptr, n_cells, s->mc_tmp, s->stream);
+      mc_count_launch(w.mc_table.ptr, n_entries, tiles, c, box, m->index.ptr, m->start.ptr, m->queries.ptr, s->stream);
+      counter_scan_async(m->start.ptr, n_cells, w.scan_tmp, s->stream);
       mc_chunks_launch(m->queries.ptr, n_cells, m->chunks.ptr, s->stream);
-      counter_scan_async(m->chunks.ptr, n_cells, s->mc_tmp, s->stream);
+      counter_scan_async(m->chunks.ptr, n_cells, w.scan_tmp, s->stream);
       sm_voxel_list_launch(m->index.ptr, n_words, box, n_cells, m->ijk.ptr, s->stream);
       s->launches += 9;
       B200_CUDA(cudaMemcpyAsync(&n_chunks, m->chunks.ptr + n_cells, sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
-      s->mc_offs.ensure((size_t)used);
-      s->mc_idx.ensure((size_t)used);
+      w.cell_offs.ensure((size_t)used);
+      w.cell_idx.ensure((size_t)used);
     }
     // the scatter also resets every point's layers, skipped ones included
-    mc_scatter_launch(s->mc_table.ptr, n_entries, tiles, c, box, m->index.ptr, m->start.ptr, m->queries.ptr, m->qcursor.ptr,
-                      m->ocursor.ptr, s->mc_offs.ptr, s->mc_idx.ptr, m->n.ptr, m->h.ptr, m->plane.ptr, s->mc_counters.ptr, s->stream);
+    mc_scatter_launch(w.mc_table.ptr, n_entries, tiles, c, box, m->index.ptr, m->start.ptr, m->queries.ptr, m->qcursor.ptr,
+                      m->ocursor.ptr, w.cell_offs.ptr, w.cell_idx.ptr, m->n.ptr, m->h.ptr, m->plane.ptr, w.counters.ptr, s->stream);
     s->launches += tiles ? 1 : 0;
     B200_CUDA(cudaStreamSynchronize(s->stream));  // n_chunks
     // K19c + K19d
-    mc_neighbour_launch(m->chunks.ptr, n_chunks, n_cells, m->start.ptr, m->queries.ptr, m->ijk.ptr, box, m->index.ptr, s->mc_offs.ptr,
-                        s->mc_idx.ptr, m->sub_first.ptr, (int)n_sub, c, m->n.ptr, m->h.ptr, m->plane.ptr, m->rows.ptr,
-                        s->mc_counters.ptr, s->stream);
+    mc_neighbour_launch(m->chunks.ptr, n_chunks, n_cells, m->start.ptr, m->queries.ptr, m->ijk.ptr, box, m->index.ptr, w.cell_offs.ptr,
+                        w.cell_idx.ptr, m->sub_first.ptr, (int)n_sub, c, m->n.ptr, m->h.ptr, m->plane.ptr, m->rows.ptr, w.counters.ptr,
+                        s->stream);
     s->launches += n_chunks ? 1 : 0;
     std::vector<unsigned long long> rows(MC_ROW_COUNT * n_sub);
     B200_CUDA(cudaMemcpyAsync(rows.data(), m->rows.ptr, rows.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
-    B200_CUDA(cudaMemcpyAsync(ctr, s->mc_counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaMemcpyAsync(ctr, w.counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
     B200_CUDA(cudaStreamSynchronize(s->stream));
     if (ctr[MC_CTR_TRIPPED]) return sm_fail(s, B200REG_ERR_CUDA, "build_map_consistency: a cell outside the box or a slot beyond its cell");
     b200sm_map_consistency_info& I = m->info;
@@ -3906,9 +3791,9 @@ int b200sm_get_map_consistency(b200sm_t s, unsigned* n, double* h, double* plane
     const MapConsistency& m = *s->mc;
     const size_t k = std::min(capacity, (size_t)m.info.n_points);
     if (k) {
-      if (n) B200_CUDA(cudaMemcpyAsync(n, m.n.ptr, k * sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
-      if (h) B200_CUDA(cudaMemcpyAsync(h, m.h.ptr, k * sizeof(double), cudaMemcpyDeviceToHost, s->stream));
-      if (plane_var) B200_CUDA(cudaMemcpyAsync(plane_var, m.plane.ptr, k * sizeof(double), cudaMemcpyDeviceToHost, s->stream));
+      get_if(s, n, m.n.ptr, k);
+      get_if(s, h, m.h.ptr, k);
+      get_if(s, plane_var, m.plane.ptr, k);
       B200_CUDA(cudaStreamSynchronize(s->stream));
     }
     return (int)B200REG_OK;
