@@ -5,7 +5,7 @@ cd "$(dirname "$0")/lidarslam_ros2_b200/csrc"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -ccbin $(command -v g++) ${B200_NVCC_EXTRA}"
 OBJS=""
-for f in grid_index voxel_map ndt_solver ndt_aux ndt_score nn_grid voxelgrid gicp cloud_codec pcd_codec pcd_load deskew comm capi scanmatcher place_recognition occupancy static_map relocalize elevation consistency map_changes mesh; do
+for f in grid_index voxel_map ndt_solver ndt_aux ndt_score nn_grid voxelgrid gicp cloud_codec pcd_codec pcd_load deskew comm capi scanmatcher place_recognition occupancy static_map relocalize elevation consistency map_changes mesh octomap; do
   if [ ! -f $f.o ] || [ $f.cu -nt $f.o ] || [ -n "$(find . -name '*.cuh' -newer $f.o -o -name '*.hpp' -newer $f.o -o -name 'b200reg.h' -newer $f.o 2>/dev/null)" ] || [ ../../include/b200reg.h -nt $f.o ] || [ ../../include/b200comm.h -nt $f.o ]; then
     echo "nvcc $f.cu"
     # gicp.cu: no FMA contraction. The reference builds for baseline x86-64 (no FMA) and GICP's line search compares f32

@@ -908,6 +908,48 @@ int b200sm_get_mesh_voxels(b200sm_t s, int* ijk3, long long* sdf_sum, unsigned* 
  * staging buffers. n_bytes (may be NULL) = the file size. No build yet, or a mesh without faces (no file is created):
  * B200REG_ERR_ARG. A file that cannot be opened or written: B200REG_ERR_IO. */
 int b200sm_save_mesh_ply(b200sm_t s, const char* path, size_t* n_bytes);
+
+/* ---- OctoMap: free and occupied voxels from every submap's rays, pruned into an octree, saved as a .bt file ------------
+ * No counterpart in the reference. The rays, walks and parameters are exactly those of b200sm_build_static_map. The box
+ * bounds every ray's endpoint voxel and the origin voxel of every submap with a ray, so every freed walk lies in it. A box
+ * voxel is OCCUPIED (2) when the static map at the same parameters counts it as an occupied voxel that is not dynamic,
+ * FREE (1) when it is not OCCUPIED and some ray's freed walk crosses it or some ray ends in it (a dynamic voxel is FREE:
+ * what moved leaves free space behind), UNKNOWN (0) otherwise. The known voxels form OctoMap's depth-16 key tree (key =
+ * voxel index + 32768), pruned where 8 leaf children share a state, and the file is the bytes octomap 1.9's
+ * OcTree::writeBinary writes for that tree (octomap_server, MoveIt and rviz load it). The counts are per-submap booleans;
+ * there are no clamped log-odds. The exact definitions are in csrc/octomap.hpp; DESIGN.md section 7b describes the
+ * build. Bitwise deterministic; the session's submaps, poses and other products are not changed. */
+typedef struct b200sm_octomap_info {
+  int box_origin[3];                 /* voxel (i, j, k) of the box's lower corner (0 when there is no ray)            */
+  unsigned box_dims[3];              /* voxels (0 when there is no ray)                                                */
+  unsigned long long n_rays, n_skipped; /* points cast as rays / not cast (as the static map's)                        */
+  unsigned long long n_occupied_voxels, n_dynamic_voxels, n_free_voxels; /* box voxels by state; the static map's
+                                        dynamic voxels, all of them FREE                                               */
+  unsigned long long n_inner_nodes, n_occupied_leaves, n_free_leaves; /* the pruned tree's nodes by kind              */
+  unsigned long long tree_size;      /* its nodes, the .bt header's size: inner nodes + leaves                        */
+  unsigned long long n_bytes;        /* the .bt file: header + 2 bytes per inner node                                  */
+  int n_batches;                     /* launches of the static map's walks                                             */
+} b200sm_octomap_info;
+/* Build the OctoMap from every submap at its own pose (poses_colmajor16 NULL) or at the given 16 * n_submaps doubles
+ * (e.g. b200sm_pose_adjust's output). params NULL: the static map's defaults. Refused with B200REG_ERR_ARG, the previous
+ * build staying readable: everything b200sm_build_static_map refuses, a resolution that printf("%g") does not give back
+ * exactly (the header's res), and a box of more than 2^31 - 1 voxels or with a voxel index outside [-32768, 32767] on
+ * some axis (all before anything is sized from the box). The session keeps the build until the next successful one or
+ * destroy, beside every other product: 1 byte per box voxel (its state) and 2 bytes per inner node (the .bt data). The
+ * call's scratch: the static map's (its rank index, 9 bytes per occupied voxel and the walks' bitmaps), 1 bit per box
+ * voxel (the freed walks) and 5 bytes per pyramid cell (about a seventh of the box's voxels). info may be NULL. */
+int b200sm_build_octomap(b200sm_t s, const double* poses_colmajor16, const b200sm_static_map_params* params,
+                         b200sm_octomap_info* info);
+/* The last build's box voxel states (0 UNKNOWN, 1 FREE, 2 OCCUPIED) in linear order, x fastest, then y, then z: *n = the
+ * box's voxels; min(*n, capacity) are copied (capacity 0: a size query). No build yet: B200REG_ERR_ARG. */
+int b200sm_get_octomap_states(b200sm_t s, unsigned char* states, size_t capacity, size_t* n);
+/* The last build's .bt file bytes: *n_bytes = its size; min(*n_bytes, capacity) bytes are copied (capacity 0: a size
+ * query). An empty tree is the header with size 0. No build yet: B200REG_ERR_ARG. */
+int b200sm_get_octomap_bt(b200sm_t s, unsigned char* bytes, size_t capacity, size_t* n_bytes);
+/* The last build's .bt file written to path through pinned staging buffers. n_bytes (may be NULL) = the file size. No
+ * build yet, or an empty tree (no file is created): B200REG_ERR_ARG. A file that cannot be opened or written:
+ * B200REG_ERR_IO. */
+int b200sm_save_octomap_bt(b200sm_t s, const char* path, size_t* n_bytes);
 /* The same text for a HOST PointXYZI cloud (records as in b200sm_import_submap; intensity_offset_bytes >= 0), formatted
  * on `device`. *n_bytes = size of the whole file content (header and data); min(*n_bytes, capacity) bytes are copied to
  * out, so capacity 0 is a size query. B200REG_ERR_ARG for n == 0, a negative intensity offset, or a stride or offset that

@@ -694,6 +694,20 @@ class ScanMatcherSession {
     check(b200sm_save_mesh_ply(s_.get(), path.c_str(), &n));
     return n;
   }
+
+  // ---- OctoMap (b200sm_build_octomap): free and occupied voxels of every submap's rays, pruned into OctoMap's key tree;
+  // poses empty = the submaps' own; p nullptr = the static map's defaults
+  b200sm_octomap_info buildOctoMap(const std::vector<double>& poses_colmajor16 = {}, const b200sm_static_map_params* p = nullptr) {
+    b200sm_octomap_info info{};
+    check(b200sm_build_octomap(s_.get(), poses_colmajor16.empty() ? nullptr : poses_colmajor16.data(), p, &info));
+    return info;
+  }
+  // the last OctoMap as an OctoMap .bt file (octomap_server, MoveIt, rviz); returns the file's bytes
+  size_t saveOctoMapBt(const std::string& path) {
+    size_t n = 0;
+    check(b200sm_save_octomap_bt(s_.get(), path.c_str(), &n));
+    return n;
+  }
   b200sm_localize_stats localizeStats() const {
     b200sm_localize_stats st{};
     check(b200sm_get_localize_stats(s_.get(), &st));

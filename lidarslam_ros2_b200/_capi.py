@@ -58,6 +58,7 @@ SYMBOLS = [
     "b200sm_build_map_changes", "b200sm_get_map_changes", "b200sm_get_change_voxels", "b200sm_get_updated_map",
     "b200sm_save_updated_map_pcd_ascii",
     "b200sm_build_mesh", "b200sm_get_mesh", "b200sm_get_mesh_voxels", "b200sm_save_mesh_ply",
+    "b200sm_build_octomap", "b200sm_get_octomap_states", "b200sm_get_octomap_bt", "b200sm_save_octomap_bt",
     "b200sm_merge_session", "b200sm_get_merge_scores", "b200sm_get_segments",
     "b200sm_save_session", "b200sm_load_session", "b200sm_get_session_graph",
     # include/b200comm.h
@@ -143,6 +144,13 @@ class SmMeshInfo(C.Structure):
     _fields_ = [("box_origin", C.c_int * 3), ("box_dims", C.c_uint * 3), ("n_points", C.c_ulonglong), ("n_rays", C.c_ulonglong),
                 ("n_skipped", C.c_ulonglong), ("n_walked", C.c_ulonglong), ("n_band_voxels", C.c_ulonglong),
                 ("n_observed_voxels", C.c_ulonglong), ("n_vertices", C.c_ulonglong), ("n_faces", C.c_ulonglong)]
+
+
+class SmOctoMapInfo(C.Structure):
+    _fields_ = [("box_origin", C.c_int * 3), ("box_dims", C.c_uint * 3), ("n_rays", C.c_ulonglong), ("n_skipped", C.c_ulonglong),
+                ("n_occupied_voxels", C.c_ulonglong), ("n_dynamic_voxels", C.c_ulonglong), ("n_free_voxels", C.c_ulonglong),
+                ("n_inner_nodes", C.c_ulonglong), ("n_occupied_leaves", C.c_ulonglong), ("n_free_leaves", C.c_ulonglong),
+                ("tree_size", C.c_ulonglong), ("n_bytes", C.c_ulonglong), ("n_batches", C.c_int)]
 
 
 class SmMapChangeInfo(C.Structure):
@@ -399,6 +407,10 @@ def lib() -> C.CDLL:
     L.b200sm_get_mesh.argtypes = [vp, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]
     L.b200sm_get_mesh_voxels.argtypes = [vp, vp, vp, vp, sz, C.POINTER(sz)]
     L.b200sm_save_mesh_ply.argtypes = [vp, C.c_char_p, C.POINTER(sz)]
+    L.b200sm_build_octomap.argtypes = [vp, vp, C.POINTER(SmStaticMapParams), C.POINTER(SmOctoMapInfo)]
+    L.b200sm_get_octomap_states.argtypes = [vp, vp, sz, C.POINTER(sz)]
+    L.b200sm_get_octomap_bt.argtypes = [vp, vp, sz, C.POINTER(sz)]
+    L.b200sm_save_octomap_bt.argtypes = [vp, C.c_char_p, C.POINTER(sz)]
     L.b200sm_merge_session.argtypes = [vp, vp, vp, C.POINTER(SmMergeParams), vp, i, vp, sz, C.POINTER(sz), vp,
                                         C.POINTER(SmMergeResult)]
     L.b200sm_get_merge_scores.argtypes = [vp, sz, C.POINTER(sz), C.POINTER(sz), vp, vp]

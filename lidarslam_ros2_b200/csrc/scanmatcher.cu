@@ -48,6 +48,7 @@
 #include "mesh.cuh"
 #include "map_cut.hpp"
 #include "occupancy.cuh"
+#include "octomap.cuh"
 #include "place_recognition.cuh"
 #include "pose_graph.hpp"
 #include "relocalize.cuh"
@@ -329,7 +330,15 @@ struct MeshBuild {
   b200sm_mesh_info info{};
 };
 
-// The per-call workspace of the six map builds and of the voxel-list read-backs, buffers named by role and shared by the
+// One OctoMap build (b200sm_build_octomap): the states of the box's voxels, the .bt file's data bytes (two per inner
+// node) and its header.
+struct OctoMapBuild {
+  DeviceBuffer<unsigned char> states, data;
+  std::string header;
+  b200sm_octomap_info info{};
+};
+
+// The per-call workspace of the seven map builds and of the voxel-list read-backs, buffers named by role and shared by the
 // builds that use one of the same type for the same role. Nothing in it outlives the call that filled it: no read-back
 // reads what a build left here.
 struct MapWorkspace {
@@ -349,6 +358,12 @@ struct MapWorkspace {
   DeviceBuffer<unsigned char> active;  // mesh: ACTIVE flags, vertex ids, and vertex and face counts per tile
   DeviceBuffer<uint32_t> vertex_id;
   DeviceBuffer<unsigned> vertex_counts, face_counts;
+  DeviceBuffer<RankWord> occ_index;  // octomap: the static map's front half on its own rank index, counts and flags,
+  DeviceBuffer<uint32_t> occ_hits, occ_frees;  // so that the static map's result stays as it is
+  DeviceBuffer<unsigned char> occ_dynamic;
+  DeviceBuffer<uint32_t> freed;          // octomap: one bit per box voxel that a freed walk crosses
+  DeviceBuffer<unsigned char> pyr_codes;  // octomap: the pyramid's codes and inner counts (then byte offsets) per cell
+  DeviceBuffer<unsigned> pyr_counts;
   DeviceBuffer<int> ijk;  // get_map_voxels / get_change_voxels: the voxel list
 };
 
@@ -445,13 +460,14 @@ struct b200sm_session {
   DeviceBuffer<int> merge_shift, merge_sel_a, merge_sel_s;
   size_t merge_nq = 0, merge_nc = 0;
   // the map products built from the session's map. The occupancy grid and the static map are kept until their next build
-  // overwrites them; the other four are built beside the last one, which stays until the new one succeeds.
+  // overwrites them; the other five are built beside the last one, which stays until the new one succeeds.
   OccupancyGrid og;
   std::unique_ptr<ElevationMap> el;
   StaticMap sm;
   std::unique_ptr<MapChanges> ch;
   std::unique_ptr<MeshBuild> ms;
   std::unique_ptr<MapConsistency> mc;
+  std::unique_ptr<OctoMapBuild> om;
   MapWorkspace work;
 };
 
@@ -3046,9 +3062,9 @@ struct SmFront {
   int batches = 0;
 };
 
-// The front half the static map and the map changes share, on the bounds pass and the rank pass: K15a and the box
-// (refused here, before anything is sized from it), then `replacing()` (the caller's last build is about to be
-// overwritten), K15b, and the walks K15c / K15d in batches of consecutive entries. The entries [0, split_entry) fold into
+// The front half the static map, the map changes and the OctoMap share, on the bounds pass and the rank pass: K15a and the
+// box (refused here, before anything is sized from it), then `replacing(bounds)` with K15a's per-entry bounds (the
+// caller's last build is about to be overwritten; it may refuse with an error code, s->err set, or return B200REG_OK), K15b, and the walks K15c / K15d in batches of consecutive entries. The entries [0, split_entry) fold into
 // hits[0] / frees[0] and, when split_entry < table.size(), the entries [split_entry, table.size()) into hits[1] /
 // frees[1]; no batch crosses split_entry. The counts are sized and zeroed here (one slot when there is no occupied voxel).
 // n_counters counters are zeroed. Must run inside sm_guarded; `what` prefixes the messages.
@@ -3069,7 +3085,7 @@ int sm_front_half(b200sm_t s, const char* what, std::vector<SmEntry>& table, uns
     const int rc = box_or_refuse(s, what, "a box", "voxels", lo, hi, 0, &box, &cells);
     if (rc != B200REG_OK) return rc;
   }
-  replacing();
+  if (const int rc = replacing(bounds); rc != B200REG_OK) return rc;
   const unsigned long long n_words = (cells + 31) / 32;
   unsigned n_voxels = 0;
   if (any_ray)  // K15b: the rank index over the box, then the number of occupied voxels
@@ -3148,7 +3164,11 @@ int b200sm_build_static_map(b200sm_t s, const double* poses_colmajor16, const b2
     StaticMap& M = s->sm;
     SmFront f;
     const int rc = sm_front_half(s, "build_static_map", table, tiles, c, SM_CTR_COUNT, table.size(), M.index, &M.hits, &M.frees,
-                                 [&]() { M.built = false; }, &f);
+                                 [&](const std::vector<int>&) {
+                                   M.built = false;
+                                   return (int)B200REG_OK;
+                                 },
+                                 &f);
     if (rc != B200REG_OK) return rc;
     const SmBox& box = f.box;
     const unsigned n_voxels = f.n_voxels;
@@ -3281,8 +3301,8 @@ int b200sm_build_map_changes(b200sm_t s, const double* poses_colmajor16, const b
     // the new build is made beside the last one, which stays until this one succeeds
     auto m = std::make_unique<MapChanges>();
     SmFront f;
-    const int rc = sm_front_half(s, "build_map_changes", table, tiles, c, CH_CTR_COUNT, split_entry, m->index, m->hits, m->frees, []() {},
-                                 &f);
+    const int rc = sm_front_half(s, "build_map_changes", table, tiles, c, CH_CTR_COUNT, split_entry, m->index, m->hits, m->frees,
+                                 [](const std::vector<int>&) { return (int)B200REG_OK; }, &f);
     if (rc != B200REG_OK) return rc;
     const unsigned n_voxels = f.n_voxels;
     const size_t nv = std::max<size_t>(n_voxels, 1);
@@ -3624,6 +3644,186 @@ int b200sm_save_mesh_ply(b200sm_t s, const char* path, size_t* n_bytes) {
       return (int)B200REG_ERR_IO;
     };
     return write_staged(s, n, 12 * MS_PLY_PIECE, fp, enqueue, write);
+  });
+}
+
+}  // extern "C"
+
+// ---- OctoMap: free and occupied voxels from every submap's rays, pruned into OctoMap's key tree and saved as a .bt file
+// (csrc/octomap.hpp, csrc/octomap.cu, and the static map's front half) ----
+namespace {
+
+constexpr size_t OM_BT_PIECE = 8u << 20;  // data bytes per piece of the .bt write
+
+}  // namespace
+
+extern "C" {
+
+int b200sm_build_octomap(b200sm_t s, const double* poses_colmajor16, const b200sm_static_map_params* params, b200sm_octomap_info* info) {
+  if (!s) return B200REG_ERR_ARG;
+  const SmParams p = sm_params_from(params);
+  SmConst c;
+  if (const char* why = sm_prepare(p, &c)) return sm_fail(s, B200REG_ERR_ARG, (std::string("build_octomap: ") + why).c_str());
+  if (!om_resolution_exact(p.resolution))
+    return sm_fail(s, B200REG_ERR_ARG, "build_octomap: the resolution does not read back from printf(\"%g\"), the .bt header's res");
+  SubmapTiles t;
+  std::vector<SmEntry> table;
+  const int rc = map_prologue(s, "build_octomap", poses_colmajor16, SM_TILE, nullptr, &t, &table, [&](size_t k, SmEntry& e) {
+    return sm_origin(c, p, e.T, e.o) ? (int)B200REG_OK : origin_refused(s, "build_octomap", k, "2^30 voxels");
+  });
+  if (rc != B200REG_OK) return rc;
+  const unsigned long long total = map_points(s);
+  if (total > 0xffffffffull) return sm_fail(s, B200REG_ERR_ARG, "build_octomap: a map of 2^32 points or more");
+  const unsigned long long tiles = t.tiles;
+  const int n_entries = (int)table.size();
+  return sm_guarded(s, [&]() {
+    MapWorkspace& w = s->work;
+    // the new build is made beside the last one, which stays until this one succeeds
+    auto m = std::make_unique<OctoMapBuild>();
+    // K15a-K15d on the workspace's own buffers; the box is the endpoint voxels' and the origin voxels of the entries
+    // with a ray (K15a left INT_MAX in an entry without one), refused before anything is sized from it
+    SmBox box{};
+    unsigned long long cells = 0;
+    bool any_ray = false;
+    SmFront f;
+    const int rc = sm_front_half(s, "build_octomap", table, tiles, c, OM_CTR_COUNT, table.size(), w.occ_index, &w.occ_hits, &w.occ_frees,
+                                 [&](const std::vector<int>& bounds) {
+                                   int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
+                                   for (size_t r = 0; r < table.size(); r++) {
+                                     if (bounds[6 * r] == INT_MAX) continue;
+                                     any_ray = true;
+                                     for (int a = 0; a < 3; a++) {
+                                       const int o = og_cell(table[r].o[a]);
+                                       lo[a] = std::min({lo[a], bounds[6 * r + a], o});
+                                       hi[a] = std::max({hi[a], bounds[6 * r + 3 + a], o});
+                                     }
+                                   }
+                                   if (!any_ray) return (int)B200REG_OK;
+                                   if (const char* why = om_box(lo, hi, box.dims, &cells)) {
+                                     auto width = [&](int a) { return std::to_string((long long)hi[a] - lo[a] + 1); };
+                                     s->err = "build_octomap: a box of " + width(0) + " x " + width(1) + " x " + width(2) + " voxels: " + why;
+                                     return (int)B200REG_ERR_ARG;
+                                   }
+                                   for (int a = 0; a < 3; a++) box.lo[a] = lo[a];
+                                   return (int)B200REG_OK;
+                                 },
+                                 &f);
+    if (rc != B200REG_OK) return rc;
+    unsigned inner = 0;
+    if (any_ray) {
+      const OmPyramid pyr = om_pyramid(box);
+      const unsigned long long n_cells = pyr.first[OM_DEPTH + 1], words = (cells + 31) / 32;
+      w.occ_dynamic.ensure(f.n_voxels);
+      w.freed.ensure((size_t)words);
+      w.pyr_codes.ensure((size_t)n_cells);
+      w.pyr_counts.ensure((size_t)n_cells);
+      m->states.ensure((size_t)cells);
+      B200_CUDA(cudaMemsetAsync(w.freed.ptr, 0, words * sizeof(uint32_t), s->stream));
+      // K15e, K22a, K22b, K22c per level up to the root, K22d per level down from it
+      sm_classify_launch(w.occ_hits.ptr, w.occ_frees.ptr, f.n_voxels, c, w.occ_dynamic.ptr, w.counters.ptr, s->stream);
+      om_free_launch(w.sm_table.ptr, n_entries, (unsigned)tiles, c, box, w.freed.ptr, w.counters.ptr, s->stream);
+      om_leaf_launch(pyr, f.box, w.occ_index.ptr, w.occ_dynamic.ptr, f.n_voxels, w.freed.ptr, m->states.ptr, w.pyr_codes.ptr,
+                     w.pyr_counts.ptr, w.counters.ptr, s->stream);
+      for (int l = 2; l <= OM_DEPTH; l++) om_reduce_launch(pyr, l, w.pyr_codes.ptr, w.pyr_counts.ptr, s->stream);
+      for (int l = OM_DEPTH; l >= 2; l--) om_offset_launch(pyr, l, w.pyr_codes.ptr, w.pyr_counts.ptr, s->stream);
+      s->launches += 3 + 2 * (OM_DEPTH - 1);
+      // the root's inner count sizes the data; K22e writes it
+      B200_CUDA(cudaMemcpyAsync(&inner, w.pyr_counts.ptr + pyr.first[OM_DEPTH], sizeof(unsigned), cudaMemcpyDeviceToHost, s->stream));
+      B200_CUDA(cudaStreamSynchronize(s->stream));
+      m->data.ensure(2 * (size_t)inner);
+      om_write_launch(pyr, m->states.ptr, w.pyr_codes.ptr, w.pyr_counts.ptr, m->data.ptr, 2ull * inner, w.counters.ptr, s->stream);
+      s->launches += 1;
+    }
+    unsigned long long ctr[OM_CTR_COUNT] = {};
+    B200_CUDA(cudaMemcpyAsync(ctr, w.counters.ptr, sizeof(ctr), cudaMemcpyDeviceToHost, s->stream));
+    B200_CUDA(cudaStreamSynchronize(s->stream));  // the host table goes out of scope; the counts are read
+    if (ctr[SM_CTR_TRIPPED] || ctr[OM_CTR_INNER] != inner)
+      return sm_fail(s, B200REG_ERR_CUDA, "build_octomap: a voxel outside the box or beyond the rank index, or a node beyond the data");
+    b200sm_octomap_info& I = m->info;
+    for (int a = 0; a < 3; a++) {
+      I.box_origin[a] = box.lo[a];
+      I.box_dims[a] = box.dims[a];
+    }
+    I.n_rays = ctr[SM_CTR_RAYS];
+    I.n_skipped = ctr[SM_CTR_SKIPPED];
+    I.n_occupied_voxels = ctr[OM_CTR_OCCUPIED_VOXELS];
+    I.n_dynamic_voxels = ctr[SM_CTR_DYNAMIC];
+    I.n_free_voxels = ctr[OM_CTR_FREE_VOXELS];
+    I.n_inner_nodes = inner;
+    I.n_occupied_leaves = ctr[OM_CTR_OCCUPIED_LEAVES];
+    I.n_free_leaves = ctr[OM_CTR_FREE_LEAVES];
+    I.tree_size = I.n_inner_nodes + I.n_occupied_leaves + I.n_free_leaves;
+    m->header = om_header(I.tree_size, p.resolution);
+    I.n_bytes = m->header.size() + 2ull * inner;
+    I.n_batches = f.batches;
+    if (info) *info = I;
+    s->om = std::move(m);
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_octomap_states(b200sm_t s, unsigned char* states, size_t capacity, size_t* n) {
+  if (!s || (!states && capacity)) return B200REG_ERR_ARG;
+  if (!s->om) return sm_fail(s, B200REG_ERR_ARG, "get_octomap_states: no build yet");
+  return sm_guarded(s, [&]() {
+    const OctoMapBuild& m = *s->om;
+    const size_t cells = (size_t)m.info.box_dims[0] * m.info.box_dims[1] * m.info.box_dims[2];
+    if (n) *n = cells;
+    const size_t k = std::min(capacity, cells);
+    if (k) {
+      get_if(s, states, m.states.ptr, k);
+      B200_CUDA(cudaStreamSynchronize(s->stream));
+    }
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_get_octomap_bt(b200sm_t s, unsigned char* bytes, size_t capacity, size_t* n_bytes) {
+  if (!s || (!bytes && capacity)) return B200REG_ERR_ARG;
+  if (!s->om) return sm_fail(s, B200REG_ERR_ARG, "get_octomap_bt: no build yet");
+  return sm_guarded(s, [&]() {
+    const OctoMapBuild& m = *s->om;
+    const size_t head = m.header.size(), data = 2 * (size_t)m.info.n_inner_nodes;
+    if (n_bytes) *n_bytes = head + data;
+    if (capacity) std::memcpy(bytes, m.header.data(), std::min(capacity, head));
+    const size_t k = capacity > head ? std::min(capacity - head, data) : 0;
+    if (k) {
+      get_if(s, bytes + head, m.data.ptr, k);
+      B200_CUDA(cudaStreamSynchronize(s->stream));
+    }
+    return (int)B200REG_OK;
+  });
+}
+
+int b200sm_save_octomap_bt(b200sm_t s, const char* path, size_t* n_bytes) {
+  if (!s || !path) return B200REG_ERR_ARG;
+  if (!s->om) return sm_fail(s, B200REG_ERR_ARG, "save_octomap_bt: no build yet");
+  const OctoMapBuild& m = *s->om;
+  if (m.info.tree_size == 0) return sm_fail(s, B200REG_ERR_ARG, "save_octomap_bt: the tree is empty");
+  return sm_guarded(s, [&]() {
+    const size_t data = 2 * (size_t)m.info.n_inner_nodes, n = (data + OM_BT_PIECE - 1) / OM_BT_PIECE;
+    if (n_bytes) *n_bytes = m.header.size() + data;
+    FILE* fp = std::fopen(path, "wb");
+    if (!fp) {
+      s->err = std::string("save_octomap_bt: cannot open ") + path + ": " + std::strerror(errno);
+      return (int)B200REG_ERR_IO;
+    }
+    auto count = [&](size_t piece) { return std::min(OM_BT_PIECE, data - piece * OM_BT_PIECE); };
+    auto enqueue = [&](size_t piece, char* buf) {
+      B200_CUDA(cudaMemcpyAsync(buf, m.data.ptr + piece * OM_BT_PIECE, count(piece), cudaMemcpyDeviceToHost, s->stream));
+    };
+    auto write = [&](size_t piece, const char* buf) {
+      bool ok = piece > 0 || std::fwrite(m.header.data(), 1, m.header.size(), fp) == m.header.size();
+      ok = ok && std::fwrite(buf, 1, count(piece), fp) == count(piece);
+      if (ok && piece + 1 == n) {
+        ok = std::fclose(fp) == 0;
+        fp = nullptr;
+      }
+      if (ok) return (int)B200REG_OK;
+      s->err = std::string("save_octomap_bt: writing ") + path + ": " + std::strerror(errno);
+      return (int)B200REG_ERR_IO;
+    };
+    return write_staged(s, n, OM_BT_PIECE, fp, enqueue, write);
   });
 }
 

@@ -733,6 +733,50 @@ class ScanMatcher:
         self._check(self._lib.b200sm_save_mesh_ply(self._h, os.fsencode(path), C.byref(size)))
         return int(size.value)
 
+    # ---- OctoMap: free and occupied voxels pruned into OctoMap's key tree (b200sm_build_octomap, csrc/octomap.hpp) ----
+    def buildOctoMap(self, poses=None, resolution: float = 0.2, max_range: float = 100.0, sensor_origin=(0.0, 0.0, 0.0),
+                     ray_fraction: float = 0.85, min_frees: int = 2, dynamic_thresh: float = 0.4) -> dict:
+        """The OctoMap of every submap at its own pose (poses None) or at `poses` (N, 4, 4), built on the device from the
+        static map's rays and parameters: a voxel is OCCUPIED when the static map keeps it as an occupied, non-dynamic
+        voxel, FREE when a ray's freed part crosses it or a ray ends in it and it is not OCCUPIED, UNKNOWN otherwise; the
+        known voxels pruned into OctoMap's depth-16 key tree. Returns the build's info as a dict (box_origin, box_dims,
+        n_rays, n_skipped, n_occupied_voxels, n_dynamic_voxels, n_free_voxels, n_inner_nodes, n_occupied_leaves,
+        n_free_leaves, tree_size, n_bytes, n_batches)."""
+        P = None
+        if poses is not None:
+            P = np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(self.numSubmaps(), 4, 4).transpose(0, 2, 1))
+        so = (C.c_double * 3)(*[float(v) for v in sensor_origin])
+        prm = _capi.SmStaticMapParams(float(resolution), float(max_range), so, float(ray_fraction), int(min_frees),
+                                      float(dynamic_thresh))
+        info = _capi.SmOctoMapInfo()
+        self._check(self._lib.b200sm_build_octomap(self._h, _ptr(P) if P is not None else None, C.byref(prm), C.byref(info)))
+        self._om_box = (tuple(info.box_origin), tuple(info.box_dims))
+        return _struct_dict(info)
+
+    def octoMapStates(self) -> dict:
+        """The last build's box: box_origin (3,) voxel of its lower corner, and states (D, H, W) uint8 indexed [k, j, i]:
+        0 UNKNOWN, 1 FREE, 2 OCCUPIED."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_get_octomap_states(self._h, None, 0, C.byref(n)))
+        out = np.empty(max(n.value, 1), dtype=np.uint8)
+        self._check(self._lib.b200sm_get_octomap_states(self._h, _ptr(out), n.value, C.byref(n)))
+        origin, (W, H, D) = getattr(self, "_om_box", ((0, 0, 0), (0, 0, 0)))
+        return dict(box_origin=np.array(origin, dtype=np.int64), states=out[:n.value].reshape(D, H, W))
+
+    def octoMapBytes(self) -> bytes:
+        """The last build's OctoMap .bt file, header and data."""
+        n = C.c_size_t(0)
+        self._check(self._lib.b200sm_get_octomap_bt(self._h, None, 0, C.byref(n)))
+        out = np.empty(max(n.value, 1), dtype=np.uint8)
+        self._check(self._lib.b200sm_get_octomap_bt(self._h, _ptr(out), n.value, C.byref(n)))
+        return out[:n.value].tobytes()
+
+    def saveOctoMapBt(self, path) -> int:
+        """The last build's OctoMap as a .bt file (octomap_server, MoveIt, rviz). Returns the file's bytes."""
+        size = C.c_size_t(0)
+        self._check(self._lib.b200sm_save_octomap_bt(self._h, os.fsencode(path), C.byref(size)))
+        return int(size.value)
+
     # ---- map consistency: neighbourhood entropy and plane variance (b200sm_build_map_consistency, csrc/map_consistency.hpp) ----
     def buildMapConsistency(self, poses=None, radius: float = 0.5, min_neighbors: int = 10, query_stride: int = 1) -> dict:
         """How crisp the map of every submap at its own pose (poses None) or at `poses` (N, 4, 4) is, built on the device:
